@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- Llama-3-8B-shaped 4-bit (gs=64, axis=1) decode tokens/s on B200 through hqq_b200.
+"""bench.py -- Llama-3-8B-shaped 4-bit (gs=64, axis=1) decode tokens/s on H100 through hqq_b200.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A "step" is one decoded token (bs=1, seq=1) through all 32 blocks + lm_head of a random-init Llama-3-8B-shaped
@@ -14,6 +14,10 @@ all-reduce with HQQ_B200_TP_MODE=nccl), i.e. strong scaling.
 
 `--impl reference` times the reference algorithm's CPU implementation (the oracle port of HQQBackend.PYTORCH:
 dequantise -> matmul per linear) on this box's host cores on a bounded sample of the same workload.
+
+`--dump-outputs DIR` writes what the last timed step of the device-resident loop produced -- the logits over the whole
+vocabulary and the picked token of every sequence -- as DIR/logits.npy (float32) and DIR/next_token.npy (float64).  Weights and
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -39,8 +43,9 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"hbm_gbs": float(d["hbm_gbs"]), "tensor_tflops": float(d.get("bf16_tflops", 1590.0)), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tensor_tflops": 1590.0, "source": "fallback (B200_PROFILING.md)"}
+        return {"hbm_gbs": float(d["hbm_gbs"]), "tensor_tflops": float(d.get("bf16_tflops", 989.0)), "source": "measured (MEASURED_PEAKS.json)"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16/bf16 -- not reached figures
+    return {"hbm_gbs": 3350.0, "tensor_tflops": 989.0, "source": "H100 SXM data sheet"}
 
 
 # ----------------------------------------------------------------------------------------------- clocks
@@ -259,7 +264,7 @@ def kernel_roofline(model, torch, peaks, reps=4):
     (q+k+v, o, gate+up, down -- the matrices that share an activation go out in ONE launch).  All launches of one group over
     all layers (x reps) are captured into a CUDA graph so the measurement is not bound by Python launch overhead, replayed,
     and timed with CUDA events on the launching stream.  Cycling through every layer's weights means each launch streams cold
-    weights (per-group footprint x 32 layers exceeds the 126 MB L2).
+    weights (per-group footprint x 32 layers exceeds the 50 MB L2).
     achieved = algorithmic bytes of the 128 launches (224 matrices) of one step / their summed average durations."""
     from hqq_b200 import ops
     dev = model.device
@@ -286,25 +291,11 @@ def kernel_roofline(model, torch, peaks, reps=4):
         tot_bytes += nbytes
         tot_ms += ms
     achieved = tot_bytes / tot_ms / 1e6
-    # dram bytes per launch (average over the four launch groups) from the committed `ncu --set full` capture of the shipped kernel
-    # -- it was taken on the unsharded Llama-3-8B matrices: for any other launch shapes (tensor-parallel shards, the 70B model)
-    # there is no capture and `traffic` is null rather than a number that belongs to other launches
-    traffic, traffic_src = None, None
-    for name in ("r2_decode1_traffic.json", "r1_decode1_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as fh:
-                cap = json.load(fh)
-            if abs(cap["algorithmic_bytes_per_launch_avg"] / (tot_bytes / len(groups)) - 1.0) < 0.01:
-                traffic, traffic_src = cap["traffic_bytes_per_launch_avg"], "profiles/" + name
-            break
-        except (OSError, KeyError, ValueError, ZeroDivisionError):
-            continue
     return {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-            "traffic": traffic, "algorithmic_bytes_per_launch": tot_bytes / len(groups),
+            "algorithmic_bytes_per_launch": tot_bytes / len(groups),
             "kernel": "hqq::linear_decode1_kernel<half,4,64,...,MR=1> (scale/zero on the cp.async ring; 4 launches/block, 128/step)",
             "peak_source": peaks["source"], "per_launch_group": per, "linear_us_per_step": round(tot_ms * 1e3 * len(model.blocks), 1),
-            "note": "event-timed graph replay of back-to-back launches over all layers (cold weights); traffic: "
-                    + (f"{traffic_src} (ncu dram bytes, same launch shapes)" if traffic_src else "no ncu capture for these launch shapes")}
+            "note": "event-timed graph replay of back-to-back launches over all layers (cold weights)"}
 
 
 def quantizer_roofline(torch, peaks, dev, reps=3):
@@ -342,10 +333,10 @@ def quantizer_roofline(torch, peaks, dev, reps=3):
 
 
 def gemm_sweep(torch, peaks, dev, quick=False):
-    """BASELINE configs[2] / the second half of `metric`: the fused dequant-GEMM (hqq_b200_linear_fwd, tcgen05 route) on the
+    """BASELINE configs[2] / the second half of `metric`: the fused dequant-GEMM (hqq_b200_linear_fwd, wgmma route) on the
     per-linear sweep -- (N, K) in {4096x4096, 11008x4096, 4096x11008} x nbits {8,4,3,2,1}, gs 64, fp16 -- at M = 4096 (tensor
     roofline) and M = 128, event-timed alone, against the measured dense tensor peak; cuBLAS on the pre-dequantised matrix
-    beside it.  3-bit has no tcgen05 route yet: its figure is our dequantize kernel + the library GEMM."""
+    beside it.  3-bit has no fused route: its figure is our dequantize kernel + our dense wgmma GEMM."""
     from hqq_b200 import ops
     from hqq_b200.core.quantize import BaseQuantizeConfig, HQQLinear
     peak_tf = peaks["tensor_tflops"]
@@ -388,9 +379,9 @@ def gemm_sweep(torch, peaks, dev, quick=False):
             del layer, Wd
     head = per["b4_4096x4096_M4096"]
     return {"bound": "tensor", "achieved": head["TFLOPs"], "peak": peak_tf, "unit": "TFLOP/s", "frac": head["frac_of_tensor_peak"],
-            "shape": "M=4096 N=4096 K=4096 nbits=4 gs=64 fp16", "kernel": "hqq::gemm::linear_gemm_kernel (persistent tcgen05 / TMA / TMEM)",
+            "shape": "M=4096 N=4096 K=4096 nbits=4 gs=64 fp16", "kernel": "hqq::gemm::linear_gemm_kernel (persistent wgmma / TMA)",
             "peak_source": peaks["source"] + " bf16_tflops (burst: kernel timed alone)", "per": per,
-            "note": "route 2 = fused tcgen05 kernel, 0 = dequantize kernel + library GEMM (3-bit); cuBLAS runs on the 16-bit matrix our dequantize kernel wrote"}
+            "note": "route 2 = fused wgmma kernel, 3 = dequantize kernel + dense wgmma GEMM (3-bit); cuBLAS runs on the 16-bit matrix our dequantize kernel wrote"}
 
 
 def _finite(o):
@@ -468,6 +459,26 @@ def tokens_agree(model, torch, n_tokens=16):
     return bool(flag.item()), detail
 
 
+def dump_outputs(model, torch, out_dir, rank, world):
+    """What the last decode step returned to its caller: the logits of every sequence over the whole vocabulary (the ranks'
+    vocabulary shards gathered) and the token picked from them.  0.5 MB per sequence for the 128256-entry vocabulary."""
+    import numpy as np
+    logits = model._bufs["logits"] if hasattr(model, "_bufs") else None
+    if logits is None:
+        raise RuntimeError("bench.py --dump-outputs: this decode path keeps no logits buffer")
+    if world > 1:
+        import torch.distributed as dist
+        parts = [torch.empty_like(logits) for _ in range(world)]
+        dist.all_gather(parts, logits.contiguous())
+        logits = torch.cat(parts, dim=-1)
+    torch.cuda.synchronize(model.device)
+    if rank == 0:
+        os.makedirs(out_dir, exist_ok=True)
+        rows = max(1, (64 << 20) // (logits.shape[-1] * 4 + 8))  # the dump stays under 64 MB: the first `rows` sequences at most
+        np.save(os.path.join(out_dir, "logits.npy"), logits[:rows].float().cpu().numpy())
+        np.save(os.path.join(out_dir, "next_token.npy"), model.next_tok[:rows].cpu().numpy().astype(np.float64))
+
+
 def run_gpu(args, rank, world, local_rank):
     import torch
     import torch.distributed as dist
@@ -535,6 +546,8 @@ def run_gpu(args, rank, world, local_rank):
     e1.record(stream)
     barrier()
     dev_ms = e0.elapsed_time(e1)
+    if getattr(args, "dump_outputs", ""):
+        dump_outputs(model, torch, args.dump_outputs, rank, world)
 
     # ---- end-to-end loop through the public API with host buffers ------------------------------
     h_in = torch.ones(B, dtype=torch.long).pin_memory()
@@ -572,8 +585,8 @@ def run_gpu(args, rank, world, local_rank):
                 "ms_per_step": dev_ms / args.steps, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f16",
                 "data": "synthetic",
                 "config": {"workload": workload,
-                           "path": f"fused sm_100a kernels, kv cache {args.cache_len}, CUDA graph; {bytes_rank / 1e9:.2f} GB streamed per step and rank "
-                                   ">> 126 MB L2 (inputs larger than L2, no flush needed)",
+                           "path": f"fused sm_90a kernels, kv cache {args.cache_len}, CUDA graph; {bytes_rank / 1e9:.2f} GB streamed per step and rank "
+                                   ">> 50 MB L2 (inputs larger than L2, no flush needed)",
                            "parallelism": f"tp{world}", "layers": n_layers, "global_batch": B,
                            "tp_mode": (model.tp_mode if (world > 1 and B == 1) else ("nccl" if world > 1 else None)), "tokens_agree": agree, "token_check": token_check},
                 "clocks": clocks,
@@ -657,9 +670,10 @@ def main():
     ap.add_argument("--no-token-check", action="store_true", help="N>1: skip the p2p-vs-nccl token agreement check before timing")
     ap.add_argument("--extras-deadline", type=float, default=240.0, help="seconds the objects added after the measurement (GEMM sweep, "
                     "quantizer, CPU baselines) may take before the line is printed without the unfinished ones")
-    ap.add_argument("--batch", type=int, default=1, help="sequences decoded in lock-step (BASELINE configs[4]: 32); > 1 runs the small-M / tcgen05 "
+    ap.add_argument("--batch", type=int, default=1, help="sequences decoded in lock-step (BASELINE configs[4]: 32); > 1 runs the small-M / wgmma "
                     "kernels between the batched glue kernels, NCCL all-reduce for the tensor-parallel partials")
     ap.add_argument("--model", default="8b", choices=["8b", "70b"], help="70b = BASELINE configs[4] (use with --gpus 8)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed step's logits and tokens as DIR/*.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

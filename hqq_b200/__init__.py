@@ -1,4 +1,4 @@
-"""hqq_b200 -- the HQQ quantize-and-infer hot path, written for NVIDIA B200 (sm_100a).
+"""hqq_b200 -- the HQQ quantize-and-infer hot path, written for NVIDIA H100 (sm_90a).
 
 Public surface mirrors ``hqq.core``:
 
@@ -16,7 +16,7 @@ from . import _lib  # noqa: F401  (import does not load the .so; first use does)
 
 def install_as_hqq() -> None:
     """Register this package's modules under the reference's import names (``hqq.core.quantize`` ...), so code
-    written against mobiusml/hqq runs on the B200 path unchanged.  See INTEGRATION.md."""
+    written against mobiusml/hqq runs on the H100 path unchanged.  See INTEGRATION.md."""
     import sys
     import types
 

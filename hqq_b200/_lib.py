@@ -95,7 +95,7 @@ def load(path: str | None = None) -> ctypes.CDLL:
     p = path or LIB_PATH
     if not os.path.exists(p):
         raise RuntimeError(
-            f"hqq_b200: {p} not found. Build it with `python -m hqq_b200.build` (needs nvcc, sm_100a). "
+            f"hqq_b200: {p} not found. Build it with `python -m hqq_b200.build` (needs nvcc, sm_90a). "
             "There is no CPU or PyTorch fallback for this package.")
     lib = ctypes.CDLL(p)
     for name, (res, args) in SIGNATURES.items():

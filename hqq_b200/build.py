@@ -1,9 +1,9 @@
-"""In-tree build of the sm_100a C-ABI library (``libhqq_b200.so``) with nvcc.
+"""In-tree build of the sm_90a C-ABI library (``libhqq_b200.so``) with nvcc.
 
     python -m hqq_b200.build [--force] [--verbose]
 
-The .so lands next to this file (git-ignored, but it travels to the GPU box with the
-repo snapshot).  There is exactly one target architecture: ``sm_100a``.
+The .so lands next to this file (git-ignored: every checkout builds its own).  There is
+exactly one target architecture: ``sm_90a`` (H100).
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ OBJ_DIR = os.path.join(PKG_DIR, "build")
 STAMP = os.path.join(PKG_DIR, "libhqq_b200.stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-I", INCLUDE,
@@ -33,7 +33,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found: hqq_b200 needs the CUDA 12.9 toolkit to build its sm_100a library")
+    raise RuntimeError("nvcc not found: hqq_b200 needs the CUDA 12 toolkit to build its sm_90a library")
 
 
 def _sources():
@@ -80,7 +80,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", *objs, "-o", LIB_PATH]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", *objs, "-o", LIB_PATH]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,4 +1,4 @@
-"""``BitPack`` with the reference's API (hqq/core/bitpack.py:10-144), executed by the sm_100a library.
+"""``BitPack`` with the reference's API (hqq/core/bitpack.py:10-144), executed by the sm_90a library.
 
 Layout is bit-identical to the reference ("slab interleave" along dim 0, most significant field
 first; 3-bit = 10 fields per int32 with zero-padded rows); see tests/test_bitpack.py.

@@ -1,5 +1,5 @@
 """Drop-in surface of ``hqq.core.quantize`` -- ``Quantizer``, ``HQQLinear``, ``HQQBackend``,
-``BaseQuantizeConfig`` -- backed by ONE sm_100a code path (``libhqq_b200.so``).
+``BaseQuantizeConfig`` -- backed by ONE sm_90a code path (``libhqq_b200.so``).
 
 What maps to what (reference: mobiusml/hqq @ e0b1d00, hqq/core/quantize.py):
   Quantizer.quantize          :76-180   -> hqq_b200_quantize (fused min/max init + proximal solver + pack)
@@ -43,7 +43,7 @@ def _cuda_device(device) -> torch.device:
     dev = torch.device(device) if device is not None else torch.device("cuda")
     if dev.type != "cuda":
         if not torch.cuda.is_available():
-            raise RuntimeError("hqq_b200: a CUDA device (B200, sm_100a) is required; there is no CPU path")
+            raise RuntimeError("hqq_b200: a CUDA device (H100, sm_90a) is required; there is no CPU path")
         dev = torch.device("cuda", torch.cuda.current_device())
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -219,7 +219,7 @@ class HQQMatmulNoCacheMul(torch.autograd.Function):
         x, bias = ctx.saved_tensors
         grad_input = grad_bias = None
         if ctx.needs_input_grad[0]:
-            grad_input = ctx.layer.matmul(grad_output, transpose=False)  # grad @ W_r on the dense tcgen05 kernel (W_r^T as the weight)
+            grad_input = ctx.layer.matmul(grad_output, transpose=False)  # grad @ W_r on the dense wgmma kernel (W_r^T as the weight)
         if bias is not None and ctx.needs_input_grad[2]:
             grad_bias = grad_output.reshape(-1, grad_output.shape[-1]).sum(0)
         return grad_input, None, grad_bias
@@ -292,7 +292,7 @@ class HQQLinear(nn.Module):
 
     @classmethod
     def set_backend(cls, backend: HQQBackend):
-        # All members lead to the same sm_100a kernels; the attribute is kept for API compatibility.
+        # All members lead to the same sm_90a kernels; the attribute is kept for API compatibility.
         HQQLinear.backend = backend
         cls.forward = getattr(cls, backend.value)
 
@@ -488,7 +488,7 @@ class HQQLinear(nn.Module):
     def matmul(self, x: Tensor, transpose: bool = True) -> Tensor:
         if transpose:
             return self._fused_forward(x, with_bias=False)
-        # x @ W_r (the backward of the forward, quantize.py:322-352): the dense tcgen05 GEMM on W_r^T -- K and N swap roles
+        # x @ W_r (the backward of the forward, quantize.py:322-352): the dense wgmma GEMM on W_r^T -- K and N swap roles
         W_r = self.dequantize()
         if x.is_cuda and x.dtype in (float16, bfloat16) and W_r.dtype == x.dtype:
             out = ops.dense_gemm(x.reshape(-1, W_r.shape[0]), W_r.t().contiguous())
@@ -513,7 +513,7 @@ class HQQLinear(nn.Module):
             if y is not None:
                 return y.reshape(*x.shape[:-1], N)
         # what no route of hqq_b200_linear_fwd covers (float32 compute, quantised meta): our dequantize kernel, then the dense
-        # tcgen05 GEMM when the compute dtype allows it; float32 has no tensor-core path here and goes to the library GEMM
+        # wgmma GEMM when the compute dtype allows it; float32 has no tensor-core path here and goes to the library GEMM
         W_r = self.dequantize()
         x2d = x.reshape(-1, K)
         out = ops.dense_gemm(x2d, W_r.to(x.dtype), bias) if (x.is_cuda and x.dtype in (float16, bfloat16)) else None
@@ -532,7 +532,7 @@ class HQQLinear(nn.Module):
     def forward_pytorch(self, x: Tensor) -> Tensor:
         return self._fused_forward(x)
 
-    # The remaining backend names resolve to the same kernels (north star: one sm_100a path behind HQQBackend).
+    # The remaining backend names resolve to the same kernels (north star: one sm_90a path behind HQQBackend).
     forward_pytorch_backprop_compile = forward_pytorch_backprop
     forward_pytorch_compile = forward_pytorch
     forward_aten_backprop = forward_pytorch_backprop

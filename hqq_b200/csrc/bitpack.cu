@@ -1,4 +1,4 @@
-// BitPack pack / unpack and the standalone dequantize kernels (sm_100a).
+// BitPack pack / unpack and the standalone dequantize kernels (sm_90a).
 //
 // The reference's "slab interleave" (hqq/core/bitpack.py) is one-dimensional once the matrix
 // is flattened: with n = packed_rows*cols packed elements, field f of packed element i is the

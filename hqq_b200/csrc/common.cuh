@@ -1,4 +1,4 @@
-// Shared helpers for the hqq_b200 sm_100a kernels.
+// Shared helpers for the hqq_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -47,7 +47,7 @@ extern std::atomic<int> g_env_epoch;  // bumped by hqq_b200_reload_env(): cached
 static inline bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) % a) == 0; }
 static inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 static inline int fields_of(int nbits) { return nbits == 3 ? 10 : 8 / nbits; }
 static inline bool valid_nbits(int nbits) { return nbits == 8 || nbits == 4 || nbits == 3 || nbits == 2 || nbits == 1; }

@@ -28,12 +28,10 @@ static bool dequant_ok(int64_t N, int64_t K, int gs, int nbits, int axis) {
 
 static size_t dense_ws_bytes(int64_t N, int64_t K, int dtype) { return (size_t)((N * K * (int64_t)dtype_size(dtype) + 255) & ~(int64_t)255); }
 
-// Where the single-matrix entry point hands over from the small-M kernel (mma.sync, streams x per tile) to the tcgen05 kernel when
-// both take the shape.  Measured on the B200 (round 2, tools/prof_route_boundary.py, profiles/r2_route_boundary.log, CUDA-graph
-// timed, 4-bit gs 64): up to M = 16 the small kernel wins everywhere (14336x4096: 22 vs 29 us); at M = 17..32 it still wins or
-// ties on matrices up to 4096x4096 = 2^24 weights (11-12.5 vs 12.5 us; 1280x8192: 11.5 vs 11.9; 8192x1024: 11.8 vs 10.5) and loses
-// on larger ones (3584x8192: 20-21 vs 17.4 us, 8192x3584: 20-22.5 vs 17-18, 14336x4096: 34-38 vs 28.5, 4096x14336: 33-35 vs 26,
-// 28672x4096: 63-72 vs 51).  HQQ_B200_SMALL_M_MAX=<m> (measurement hook) replaces the rule by "small kernel up to M = m".
+// Where the single-matrix entry point hands over from the small-M kernel (mma.sync, streams x per tile) to the wgmma kernel when
+// both take the shape: up to M = 16 everywhere, and up to M = 32 on matrices of at most 2^24 weights, where the weight stream the
+// small kernel is bound by still dominates; larger problems go to the wgmma kernel.  tools/prof_route_boundary.py times both
+// sides.  HQQ_B200_SMALL_M_MAX=<m> (measurement hook) replaces the rule by "small kernel up to M = m".
 static bool prefer_small(int64_t M, int64_t N, int64_t K) {
   HQQ_ENV_KNOB(m, ([] { const char* e = getenv("HQQ_B200_SMALL_M_MAX"); return e ? atoi(e) : 0; })());
   if (m > 0) return M <= m;
@@ -44,7 +42,7 @@ extern "C" int hqq_b200_linear_fwd_route(int64_t M, int64_t N, int64_t K, int gr
   const bool small = small_route_ok(M, N, K, group_size, nbits, axis, dtype);
   if (small && (prefer_small(M, N, K) || !gemm_route_ok(M, N, K, group_size, nbits, axis, dtype))) return 1;
   if (gemm_route_ok(M, N, K, group_size, nbits, axis, dtype)) return 2;
-  if (dequant_ok(N, K, group_size, nbits, axis) && dense_route_ok(M, N, K, dtype)) return 3;  // dequantize kernel -> dense tcgen05 GEMM
+  if (dequant_ok(N, K, group_size, nbits, axis) && dense_route_ok(M, N, K, dtype)) return 3;  // dequantize kernel -> dense wgmma GEMM
   return 0;
 }
 

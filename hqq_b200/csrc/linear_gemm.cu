@@ -1,24 +1,23 @@
-// HQQLinear.forward for M >= 33 (prefill / batched decode): fused unpack -> group-dequant -> tcgen05 GEMM.
+// HQQLinear.forward for M >= 33 (prefill / batched decode): fused unpack -> group-dequant -> wgmma GEMM.
 //
 //   y[M,N] = x[M,K] @ dequantize(W_q)^T (+bias)          reference: hqq/core/quantize.py:184-199, 880-898
 //
-// ONE persistent kernel, one CTA per SM, 14 warps with fixed roles; a CTA walks a static list of output tiles
-// [128 weight rows] x [UN tokens] (UN = 256, or 128 for the ragged part of the schedule, see `Sched`):
-//   warp 0       TMA producer: the activation tile [UN tokens x 64 k] of every k-block (cp.async.bulk.tensor.2d, 128B swizzle,
-//                out-of-range tokens zero-filled by the hardware) into a 4-stage shared-memory ring = B operand (N = UN)
-//   warps 2..9   dequant: stream the packed bytes of the weight tile from HBM/L2 (the reference's slab layout, bitpack.py: 128/F
+// ONE persistent kernel, one CTA per SM, 16 warps with fixed roles; a CTA walks a static list of output tiles
+// [128 weight rows] x [UN tokens] (UN = 128, or 64 for the ragged part of the schedule, see `Sched`):
+//   warps 0..7   dequant: stream the packed bytes of the weight tile from HBM/L2 (the reference's slab layout, bitpack.py: 128/F
 //                packed rows x F slabs = 128 output rows), expand them in registers with the reference's two roundings
 //                W_r = fl(fl(q - z) * s) (bit-identical to Quantizer.dequantize) and store K-major SWIZZLE_128B fp16/bf16 rows
-//                into the ring = A operand (M = 128).  The dequantised matrix never exists in HBM.
-//   warp 1       one elected thread issues tcgen05.mma (4 per 64-k stage) into one of TWO fp32 accumulators in TMEM
-//                (2 x 256 columns = all 512); tcgen05.commit frees the stage / publishes the accumulator
-//   warps 10..13 epilogue: tcgen05.ld (lane = weight row, column = token) -> bias -> y, for tile i while the other roles are
-//                already in the main loop of tile i+1 (the rings never drain between tiles)
-// Round 1 launched one CTA per tile: 512 tiles on 148 SMs = 3.46 -> 4 waves, prologue/epilogue exposed per tile, tensor pipe
-// 61 % active.  tools/ummabench.cu (round 2) measured the same MMA stream alone at 1.35-1.40 PFLOP/s on this part, with A from
-// TMEM (tcgen05.mma "ts" form) no faster than from shared memory -- so A stays in shared memory and the TMEM goes to the
-// second accumulator.
-// sm_100a only: tcgen05 / TMEM / TMA, no mma.sync fallback.
+//                into a 4-stage shared-memory ring = A operand.  The dequantised matrix never exists in HBM.  As soon as a stage
+//                is free, lane 0 of warp 0 also starts the TMA load of its activation tile [UN tokens x 64 k]
+//                (cp.async.bulk.tensor.2d, 128B swizzle, out-of-range tokens zero-filled by the hardware) = B operand (N = UN).
+//                Dense mode (NBITS = 16): no dequant; lane 0 of warp 0 loads both operands by TMA.
+//   warps 8..15  two MMA warpgroups, 64 weight rows each: wgmma.mma_async m64nUNk16 (4 per 64-k stage) from the two shared-memory
+//                operands into fp32 register accumulators; a stage is freed once the wgmma group that read it has retired
+//                (one group stays in flight), and after the last k-block the warpgroup writes its accumulators -> bias -> y
+//                itself while the producers already fill the ring for its next tile.
+// The accumulators live in registers, so the tile is 128 x 128: two warpgroups hold 64 fp32 each per thread, which leaves every
+// role 128 registers at 512 threads per SM without setmaxnreg (a 17th warp, e.g. a TMA-only producer, would cut that to 96).
+// sm_90a: wgmma / TMA / mbarrier, no mma.sync fallback.
 #include <stdlib.h>
 #include <cuda.h>  // CUtensorMap types only; the encode entry point is resolved through the runtime (no -lcuda)
 
@@ -30,25 +29,23 @@ namespace gemm {
 
 constexpr int kStages = 4;
 constexpr int kBlockK = 64;          // k elements per stage = one 128-byte swizzle row
-constexpr int kTileRows = 128;       // weight rows per CTA = UMMA M
+constexpr int kTileRows = 128;       // weight rows per CTA = two wgmma M of 64
 constexpr int kDequantThreads = 256;
-constexpr int kEpilogueThreads = 128;
-constexpr int kThreads = 64 + kDequantThreads + kEpilogueThreads;  // warp 0: TMA + TMEM alloc, warp 1: MMA issue, 2..9: dequant, 10..13: epilogue
-constexpr int kUN = 256;             // tokens per full tile = UMMA N; half tiles use 128
-constexpr int kTmemCols = 512;       // two accumulators of kUN fp32 columns
+constexpr int kMmaThreads = 256;     // two warpgroups
+constexpr int kThreads = kDequantThreads + kMmaThreads;  // warps 0..7: dequant + activation TMA, 8..15: wgmma + epilogue
+constexpr int kUN = 128;             // tokens per full tile = wgmma N; half tiles use 64
 
-// Static tile schedule.  Items 0 .. i_split-1 are full tiles: item j = (row tile j / n_tok, token tile j % n_tok), 256 tokens
-// (128 when no more than 128 tokens remain).  The last r_split full tiles are cut into two 128-token halves each (items
-// i_split ..): with T full tiles on P persistent CTAs the last round holds T % P tiles; as halves they spread over twice as
-// many CTAs and the round costs half a tile (512 tiles on 148 SMs: 3.5 tile-times instead of 4).  CTA b owns items b, b + P, ...
+// Static tile schedule.  Items 0 .. i_split-1 are full tiles: item j = (row tile j / n_tok, token tile j % n_tok), kUN tokens
+// (kUN / 2 when no more than that remain).  The last r_split full tiles are cut into two halves each (items i_split ..): with
+// T full tiles on P persistent CTAs the last round holds T % P tiles; as halves they spread over twice as many CTAs and the
+// round costs half a tile.  CTA b owns items b, b + P, ...
 struct Sched {
-  int n_tok;     // token tiles of 256
+  int n_tok;     // token tiles of kUN
   int i_split;   // first item that is a half tile
   int n_items;
-  // Few tiles (M <= 512 on most matrices): `ksplit` CTAs share a tile, each accumulating a contiguous run of k-blocks and writing
-  // its fp32 partial tile to the caller's workspace; splitk_reduce_kernel adds the partials in slice order (deterministic) and
-  // rounds.  Without it a [128 x K] tile is ONE serial stream per CTA with four stages in flight: ~960 cycles per 64-k block
-  // (first-touch DRAM latency), 32 CTAs busy out of 148 -- 32 us for 4096 x 4096 at any M <= 512 (profiles/r2_midm_options.log).
+  // Few tiles: `ksplit` CTAs share a tile, each accumulating a contiguous run of k-blocks and writing its fp32 partial tile to
+  // the caller's workspace; splitk_reduce_kernel adds the partials in slice order (deterministic) and rounds.  Without it a
+  // [128 x K] tile is ONE serial stream per CTA with four stages in flight, and most SMs idle.
   int ksplit;    // 1 = off; items are then (tile, slice), slice fastest
   int n_row;     // row tiles
 };
@@ -59,7 +56,7 @@ struct Args {
   const void* zero;
   const void* bias;
   void* y;
-  float* ws;     // ksplit > 1: [ksplit][n_row * n_tok][256 tokens][128 rows] fp32 partials
+  float* ws;     // ksplit > 1: [ksplit][n_row * n_tok][kUN tokens][128 rows] fp32 partials
   int M, N, K;
   int step;  // packed rows = N / F
   int Gk;    // groups per row = K / GS
@@ -84,8 +81,8 @@ __host__ __device__ __forceinline__ Item decode_item(const Args& a, int j) {
   it.tile = base;
   it.tile_n = base / a.sched.n_tok;
   it.m0 = (base % a.sched.n_tok) * kUN;
-  it.un = (a.M - it.m0 > 128) ? 256 : 128;
-  if (half >= 0) { it.m0 += half * 128; it.un = 128; }
+  it.un = (a.M - it.m0 > kUN / 2) ? kUN : kUN / 2;
+  if (half >= 0) { it.m0 += half * (kUN / 2); it.un = kUN / 2; }
   it.valid = it.m0 < a.M && it.kb0 < it.kb1;
   return it;
 }
@@ -101,7 +98,7 @@ __device__ __forceinline__ void pdl_release_dependents() { asm volatile("griddep
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------
 #ifdef HQQ_EMU
-// CPU emulation (tests/emu): the same entry points, backed by a functional model of mbarrier / TMA / tcgen05 / TMEM
+// CPU emulation (tests/emu): the same entry points, backed by a functional model of mbarrier / TMA / wgmma
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return ::emu::smem_offset(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) { ::emu::mbar_init(bar, count); }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) { ::emu::mbar_arrive(bar); }
@@ -110,15 +107,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { ::em
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) { ::emu::tma_load_2d(smem_dst, map, bar, c0, c1); }
 __device__ __forceinline__ void fence_async_smem() {}
 __device__ __forceinline__ void fence_barrier_init() {}
-__device__ __forceinline__ void tc_fence_before() {}
-__device__ __forceinline__ void tc_fence_after() {}
-__device__ __forceinline__ void tc_commit(uint64_t* bar) { ::emu::tc_commit(bar); }  // arrives once the MMAs issued before it have executed
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  ::emu::umma_f16(tmem_d, adesc, bdesc, idesc, accumulate);
+__device__ __forceinline__ void wgmma_fence() {}
+__device__ __forceinline__ void wgmma_commit() { ::emu::wgmma_commit(); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { ::emu::wgmma_wait(N); }
+template <typename T, int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  ::emu::wgmma_f16(d, N, adesc, bdesc, accumulate != 0, std::is_same<T, __nv_bfloat16>::value);
 }
-template <int NCOLS> __device__ __forceinline__ void tmem_alloc(uint32_t* dst_in_smem) { ::emu::tmem_alloc(dst_in_smem, NCOLS); }
-template <int NCOLS> __device__ __forceinline__ void tmem_dealloc(uint32_t) {}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) { ::emu::tmem_ld32(taddr, v); }
 #define HQQ_STS_V4(addr, a, b, c, d) ::emu::sts(addr, a, b, c, d)
 #define HQQ_STS_V2(addr, a, b) ::emu::sts(addr, a, b)
 #define HQQ_PREFETCH_TENSORMAP(p) ((void)(p))
@@ -156,41 +151,56 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_in_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_in_smem)), "n"(NCOLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-        "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]),
-        "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory, fp32 accumulators in registers
+// (thread (warp w, lane l) of the warpgroup holds rows 16w + l/4 (+8), columns 8j + 2(l%4) (+1) at d[4j .. 4j+3]).
+template <typename T, int N> struct Wgmma;
+#define HQQ_WGMMA_N128(TY)                                                                                                              \
+  template <> struct Wgmma<TY##_t, 128> {                                                                                               \
+    __device__ __forceinline__ static void run(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {                       \
+      asm volatile(                                                                                                                     \
+          "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"                                                                                  \
+          "wgmma.mma_async.sync.aligned.m64n128k16.f32." #TY "." #TY " "                                                               \
+          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "  \
+          "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, " \
+          "%51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"                             \
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),      \
+            "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),        \
+            "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),        \
+            "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),        \
+            "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),        \
+            "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),        \
+            "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])         \
+          : "l"(adesc), "l"(bdesc), "r"(acc));                                                                                          \
+    }                                                                                                                                   \
+  };
+#define HQQ_WGMMA_N64(TY)                                                                                                               \
+  template <> struct Wgmma<TY##_t, 64> {                                                                                                \
+    __device__ __forceinline__ static void run(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t acc) {                       \
+      asm volatile(                                                                                                                     \
+          "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"                                                                                  \
+          "wgmma.mma_async.sync.aligned.m64n64k16.f32." #TY "." #TY " "                                                                \
+          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, "  \
+          "%26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"                                                                \
+          : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),      \
+            "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),        \
+            "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),        \
+            "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])                                                                          \
+          : "l"(adesc), "l"(bdesc), "r"(acc));                                                                                          \
+    }                                                                                                                                   \
+  };
+typedef __half f16_t;
+typedef __nv_bfloat16 bf16_t;
+HQQ_WGMMA_N128(f16)
+HQQ_WGMMA_N128(bf16)
+HQQ_WGMMA_N64(f16)
+HQQ_WGMMA_N64(bf16)
+template <typename T, int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  Wgmma<T, N>::run(d, adesc, bdesc, accumulate);
 }
 
 #define HQQ_STS_V4(addr, a, b, c, d) asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory")
@@ -200,29 +210,15 @@ __device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
 #define HQQ_NAMED_BAR_SYNC(id, n) asm volatile("bar.sync %0, %1;" ::"n"(id), "n"(n) : "memory")
 #endif  // HQQ_EMU
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address >> 4 in bits [0,14),
-// leading byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset = 1024 B between 8-row groups in
-// [32,46), descriptor version 1 (Blackwell) in [46,48), layout type 2 = SWIZZLE_128B in [61,64).
+// K-major, SWIZZLE_128B wgmma shared-memory matrix descriptor (PTX ISA "matrix descriptor"): start address >> 4 in bits
+// [0,14), leading byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset = 1024 B between 8-row groups in
+// [32,46), base offset 0 (every operand tile is 1024-byte aligned), layout type 1 = SWIZZLE_128B in [62,64).
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor): D = F32, A/B = F16 or BF16, both K-major, M = 128, N = UN.
-template <typename T>
-__device__ __forceinline__ uint32_t make_idesc(int UN) {
-  const uint32_t fmt = std::is_same<T, __nv_bfloat16>::value ? 1u : 0u;
-  uint32_t d = 0;
-  d |= 1u << 4;                      // c_format = F32
-  d |= fmt << 7;                     // a_format
-  d |= fmt << 10;                    // b_format
-  d |= (uint32_t)(UN >> 3) << 17;    // n_dim
-  d |= (uint32_t)(128 >> 4) << 24;   // m_dim
+  d |= (uint64_t)1 << 62;
   return d;
 }
 
@@ -282,10 +278,10 @@ struct Smem {
 
 // NBITS = 16 ("dense"): the A operand is an ordinary [N, K] fp16/bf16 matrix fetched by TMA like B -- the dequant warps idle.  It is
 // the second half of the routes no fused expansion exists for (3-bit's 10-field int32 slabs, axis = 0 groups, other group sizes,
-// the backward pass): our dequantize kernel writes W_r once, this kernel multiplies (hqq_b200_linear_fwd route 4).
+// the backward pass): our dequantize kernel writes W_r once, this kernel multiplies (hqq_b200_linear_fwd route 3).
 template <typename T, int NBITS, int GS>
-__global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_constant__ CUtensorMap xmap256,
-                                                                  const __grid_constant__ CUtensorMap xmap128,
+__global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_constant__ CUtensorMap xmap_full,
+                                                                  const __grid_constant__ CUtensorMap xmap_half,
                                                                   const __grid_constant__ CUtensorMap amap, const Args a) {
   constexpr bool DENSE = NBITS == 16;
   constexpr int F = DENSE ? 1 : 8 / NBITS;  // slabs per byte
@@ -294,6 +290,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
   static_assert(BPT >= 4, "a dequant thread expands at least four packed bytes per k-block");
   constexpr int TPR = 64 / BPT;            // dequant threads per packed row
   constexpr uint32_t MASK = (1u << NBITS) - 1u;
+  constexpr int kMmaWarp0 = kDequantThreads / 32;
   using S = Smem;
   using P2 = Pair<T>;
 
@@ -304,42 +301,44 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * (S::A_STAGE + S::B_STAGE));
   uint64_t* full_a = bars;                 // [kStages] dequant warps -> MMA (one arrival per warp)
   uint64_t* full_b = bars + kStages;       // [kStages] TMA -> MMA (1 arrival + tx bytes)
-  uint64_t* empty = bars + 2 * kStages;    // [kStages] MMA (tcgen05.commit) -> both producers
-  uint64_t* acc_full = bars + 3 * kStages;       // [2] MMA (tcgen05.commit) -> epilogue
-  uint64_t* acc_empty = bars + 3 * kStages + 2;  // [2] epilogue (one arrival per warp) -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStages + 4);
+  uint64_t* empty = bars + 2 * kStages;    // [kStages] MMA warps (one arrival per warp, after its wgmma read the stage) -> both producers
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_kb = (a.K + kBlockK - 1) / kBlockK;  // quantised routes: K % 256 == 0; dense: the TMA zero-fills a ragged last block
   const int n_items = a.sched.n_items;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int s = 0; s < kStages; ++s) { mbar_init(&full_a[s], kDequantThreads / 32); mbar_init(&full_b[s], 1); mbar_init(&empty[s], 1); }
-      for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], kEpilogueThreads / 32); }
-      fence_barrier_init();
-      HQQ_PREFETCH_TENSORMAP(&xmap256);
-      HQQ_PREFETCH_TENSORMAP(&xmap128);
-      if constexpr (DENSE) HQQ_PREFETCH_TENSORMAP(&amap);
-    }
-    __syncwarp();
-    tmem_alloc<kTmemCols>(tmem_slot);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_a[s], kDequantThreads / 32); mbar_init(&full_b[s], 1); mbar_init(&empty[s], kMmaThreads / 32); }
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // Programmatic dependent launch, both sides.  Our dependents (the split-K second pass; the next forward of a chain of layers) may
   // become resident as our CTAs retire -- they block in griddepcontrol.wait until this grid has completed and flushed, so only
   // their launch latency and prologue move under our tail.  As a dependent ourselves, the one thing we read that a PDL-aware
   // predecessor may still be writing is the activation x (and, dense mode, W written by the dequantize kernel): the TMA producer
   // waits before its first load, and nothing is written (y, split-K partials) before an accumulator fed by those loads is full.
   // Packed weights, scale, zero and bias are never produced by a kernel that releases its dependents early.
-  if (threadIdx.x == 0) pdl_release_dependents();
+  if (threadIdx.x == 0) {
+    pdl_release_dependents();
+    HQQ_PREFETCH_TENSORMAP(&xmap_full);
+    HQQ_PREFETCH_TENSORMAP(&xmap_half);
+    if constexpr (DENSE) HQQ_PREFETCH_TENSORMAP(&amap);
+  }
+  // TMA of k-block kb of item `im` into free stage s (thread 0 only; the caller has waited for empty[s])
+  auto load_stage = [&](const Item& im, int kb, int s) {
+    constexpr uint32_t A_TX = DENSE ? S::A_STAGE : 0;  // dense: the weight tile rides the same barrier
+    if (im.un == kUN) {
+      mbar_expect_tx(&full_b[s], S::B_STAGE + A_TX);
+      tma_load_2d(sB + s * S::B_STAGE, &xmap_full, &full_b[s], kb * kBlockK, im.m0);
+    } else {
+      mbar_expect_tx(&full_b[s], S::B_STAGE / 2 + A_TX);
+      tma_load_2d(sB + s * S::B_STAGE, &xmap_half, &full_b[s], kb * kBlockK, im.m0);
+    }
+    if constexpr (DENSE) tma_load_2d(sA + s * S::A_STAGE, &amap, &full_b[s], kb * kBlockK, im.tile_n * kTileRows);
+  };
 
-  if (warp == 0) {
-    // ================= TMA producer: activation tiles =================
-    if (lane == 0) {
+  if (DENSE && warp < kMmaWarp0) {
+    // ================= dense mode: TMA producer for both operands =================
+    if (threadIdx.x == 0) {
       uint32_t it = 0;  // k-blocks issued so far (ring position)
       pdl_wait_primary();
       for (int j = blockIdx.x; j < n_items; j += gridDim.x) {
@@ -348,53 +347,83 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
         for (int kb = im.kb0; kb < im.kb1; ++kb, ++it) {
           const int s = it % kStages;
           mbar_wait(&empty[s], ((it / kStages) & 1) ^ 1);
-          constexpr uint32_t A_TX = DENSE ? S::A_STAGE : 0;  // dense: the weight tile rides the same barrier
-          if (im.un == kUN) {
-            mbar_expect_tx(&full_b[s], S::B_STAGE + A_TX);
-            tma_load_2d(sB + s * S::B_STAGE, &xmap256, &full_b[s], kb * kBlockK, im.m0);
-          } else {
-            mbar_expect_tx(&full_b[s], S::B_STAGE / 2 + A_TX);
-            tma_load_2d(sB + s * S::B_STAGE, &xmap128, &full_b[s], kb * kBlockK, im.m0);
-          }
-          if constexpr (DENSE) tma_load_2d(sA + s * S::A_STAGE, &amap, &full_b[s], kb * kBlockK, im.tile_n * kTileRows);
+          load_stage(im, kb, s);
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer (one elected thread) =================
-    uint32_t it = 0, q = 0;  // k-blocks consumed, tiles started
+  } else if (warp >= kMmaWarp0) {
+    // ================= MMA warpgroups: wgmma into register accumulators, then the epilogue =================
+    const int wg = (warp - kMmaWarp0) >> 2;     // weight rows 64 * wg .. + 63 of the tile
+    const int tw = threadIdx.x & 127;           // thread in the warpgroup
+    const int r0 = 64 * wg + 16 * (tw >> 5) + ((tw & 31) >> 2);  // tile rows r0 and r0 + 8
+    const int c0 = 2 * (tw & 3);                // token columns 8j + c0, + 1
+    T* y = reinterpret_cast<T*>(a.y);
+    const T* bias = reinterpret_cast<const T*>(a.bias);
+    const bool has_bias = bias != nullptr;
+    float acc[kUN / 2];
+    uint32_t it = 0;  // k-blocks consumed
     for (int j = blockIdx.x; j < n_items; j += gridDim.x) {
       const Item im = decode_item(a, j);
       if (!im.valid) continue;
-      const uint32_t buf = q & 1, use = q >> 1;
-      mbar_wait(&acc_empty[buf], (use & 1) ^ 1);  // the epilogue has drained this accumulator (passes at once the first time)
-      tc_fence_after();
-      const uint32_t idesc = make_idesc<T>(im.un);
-      const uint32_t tmem_d = tmem_base + buf * kUN;
       for (int kb = im.kb0; kb < im.kb1; ++kb, ++it) {
         const int s = it % kStages;
         const uint32_t ph = (it / kStages) & 1;
         if constexpr (!DENSE) mbar_wait(&full_a[s], ph);
         mbar_wait(&full_b[s], ph);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint64_t adesc = make_desc_sw128(smem_u32(sA + s * S::A_STAGE));
-          const uint64_t bdesc = make_desc_sw128(smem_u32(sB + s * S::B_STAGE));
+        const uint64_t adesc = make_desc_sw128(smem_u32(sA + s * S::A_STAGE + wg * 64 * 128));
+        const uint64_t bdesc = make_desc_sw128(smem_u32(sB + s * S::B_STAGE));
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)  // UMMA_K = 16: advance 32 bytes inside the 128-byte swizzle row
-            tc_mma_f16(tmem_d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, ((kb - im.kb0) | k) != 0);
-          tc_commit(&empty[s]);                              // frees the stage when these MMAs have read it
-          if (kb == im.kb1 - 1) tc_commit(&acc_full[buf]);   // accumulator complete
+        for (int k = 0; k < kBlockK / 16; ++k) {  // K = 16 per wgmma: advance 32 bytes inside the 128-byte swizzle row
+          const uint32_t accumulate = ((kb - im.kb0) | k) != 0;
+          if (im.un == kUN) wgmma_f16<T, kUN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), accumulate);
+          else wgmma_f16<T, kUN / 2>(*reinterpret_cast<float(*)[kUN / 4]>(&acc), adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), accumulate);
         }
-        __syncwarp();
+        wgmma_commit();
+        // the group of the previous k-block has retired: its stage may be refilled (one group stays in flight)
+        if (kb > im.kb0) {
+          wgmma_wait<1>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[(it - 1) % kStages]);
+        }
       }
-      ++q;
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[(it - 1) % kStages]);
+      // ---- epilogue: accumulators -> (bias) -> y, or the fp32 partial of this k-slice ----
+      const int prow0 = im.tile_n * PR;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = r0 + 8 * h;                 // tile row = weight row inside the tile
+        const int tf = t / PR, tp = t % PR;
+        const bool n_ok = (prow0 + tp) < a.step;
+        const int n = tf * a.step + prow0 + tp;
+        T bn = cvt_out<T>(0.0f);
+        if (has_bias && n_ok) bn = bias[n];
+#pragma unroll
+        for (int jj = 0; jj < kUN / 8; ++jj) {
+          if (8 * jj >= im.un) break;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * jj + c0 + e, m = im.m0 + col;
+            const float v = acc[4 * jj + 2 * h + e];
+            if (a.sched.ksplit > 1) {
+              // fp32 partial of this k-slice: [slice][tile][token][tile row]
+              if (m < a.M) a.ws[(((size_t)im.slice * (size_t)(a.sched.n_row * a.sched.n_tok) + (size_t)im.tile) * kUN + (size_t)col) * kTileRows + t] = v;
+            } else if (n_ok && m < a.M) {
+              T o = cvt_out<T>(v);
+              if (has_bias) o = __hadd(o, bn);  // out += bias: second rounding, as in the reference
+              y[(long long)m * a.N + n] = o;
+            }
+          }
+        }
+      }
     }
-  } else if (warp < 2 + kDequantThreads / 32) {
+  } else {
     if constexpr (!DENSE) {
-    // ================= dequant warps: packed bytes -> swizzled fp16/bf16 A tile =================
+    // ================= dequant warps: packed bytes -> swizzled fp16/bf16 A tile (+ the activation TMA) =================
     static_assert(kStages == 4, "the dequant loop is unrolled over the 4 ring stages");
-    const int td = threadIdx.x - 64;
+    const int td = threadIdx.x;
     const int pr = td / TPR, c = td % TPR;
     constexpr int GPQ = 256 / GS;  // quantisation groups per 4 k-blocks (4 or 2): one vector load per slab and array
     uint32_t soff[F];              // shared-memory offsets are tile invariant
@@ -443,6 +472,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
     // K % 256 == 0 (checked by the router) and k-slices are whole quads: every item starts at ring stage 0
     int j = next_valid((int)blockIdx.x);
     if (j < n_items) { tile_ptrs(decode_item(a, j)); load_quad(); }
+    if (td == 0) pdl_wait_primary();  // x may still be written by the predecessor; the weights are not
     uint32_t gq = 0;  // quads done so far (ring parity)
     while (j < n_items) {
       const int jn = next_valid(j + (int)gridDim.x);
@@ -475,6 +505,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
 #pragma unroll
         for (int d = 0; d < 4; ++d) {  // stage index == d because the ring has exactly four stages
           mbar_wait(&empty[d], parity);
+          if (td == 0) load_stage(cur, cur.kb0 + 4 * q + d, d);
           const uint32_t stage = sA_u32 + d * S::A_STAGE;
 #pragma unroll
           for (int f = 0; f < F; ++f) {
@@ -504,59 +535,6 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
       j = jn;
     }
     }  // !DENSE
-  } else {
-    // ================= epilogue warps: TMEM -> registers -> y, one tile behind the main loop =================
-    const int quarter = warp & 3;                 // TMEM lanes this warp may touch: 32*quarter .. +31
-    const int t = quarter * 32 + lane;            // tile row = weight row inside the tile
-    const int tf = t / PR, tp = t % PR;
-    T* y = reinterpret_cast<T*>(a.y);
-    const T* bias = reinterpret_cast<const T*>(a.bias);
-    const bool has_bias = bias != nullptr;
-    uint32_t q = 0;
-    for (int j = blockIdx.x; j < n_items; j += gridDim.x) {
-      const Item im = decode_item(a, j);
-      if (!im.valid) continue;
-      const uint32_t buf = q & 1, use = q >> 1;
-      const int prow0 = im.tile_n * PR;
-      const bool n_ok = (prow0 + tp) < a.step;
-      const int n = tf * a.step + prow0 + tp;
-      T bn = cvt_out<T>(0.0f);
-      if (has_bias && n_ok) bn = bias[n];
-      mbar_wait(&acc_full[buf], use & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int col = 0; col < im.un; col += 32) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * kUN + (uint32_t)col, v);
-        if (a.sched.ksplit > 1) {
-          // fp32 partial of this k-slice: [slice][tile][token][tile row] -- 32 lanes write 32 consecutive rows (128 bytes)
-          float* wsp = a.ws + (((size_t)im.slice * (size_t)(a.sched.n_row * a.sched.n_tok) + (size_t)im.tile) * kUN + (size_t)col) * kTileRows + t;
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj)
-            if (im.m0 + col + jj < a.M) wsp[(size_t)jj * kTileRows] = __uint_as_float(v[jj]);
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) {
-            const int m = im.m0 + col + jj;
-            if (n_ok && m < a.M) {
-              T o = cvt_out<T>(__uint_as_float(v[jj]));
-              if (has_bias) o = __hadd(o, bn);  // out += bias: second rounding, as in the reference
-              y[(long long)m * a.N + n] = o;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);  // every lane's tcgen05.ld has completed (wait::ld) before the syncwarp
-      ++q;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
   }
 }
 
@@ -698,17 +676,17 @@ static size_t splitk_ws_bytes(const Sched& s) {
 
 template <typename T, int NBITS, int GS>
 static int launch(const void* x, Args& a, cudaStream_t st, const void* dense_W = nullptr, void* ws = nullptr, size_t ws_bytes = 0) {
-  CUtensorMap xmap256, xmap128, amap;
+  CUtensorMap xmap_full, xmap_half, amap;
   const CUtensorMapDataType dt = std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  int rc = encode_map(&xmap256, x, a.M, a.K, dt, sizeof(T), kUN);
+  int rc = encode_map(&xmap_full, x, a.M, a.K, dt, sizeof(T), kUN);
   if (rc) return rc;
-  rc = encode_map(&xmap128, x, a.M, a.K, dt, sizeof(T), kUN / 2);
+  rc = encode_map(&xmap_half, x, a.M, a.K, dt, sizeof(T), kUN / 2);
   if (rc) return rc;
   if (NBITS == 16) {
     rc = encode_map(&amap, dense_W, a.N, a.K, dt, sizeof(T), kTileRows);
     if (rc) return rc;
   } else {
-    amap = xmap128;  // unused
+    amap = xmap_half;  // unused
   }
   constexpr int PR = NBITS == 16 ? kTileRows : kTileRows / (NBITS == 16 ? 1 : 8 / NBITS);
   const int P = persistent_ctas();
@@ -741,9 +719,9 @@ static int launch(const void* x, Args& a, cudaStream_t st, const void* dense_W =
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl_on() ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, k, xmap256, xmap128, amap, a);
+    cudaLaunchKernelEx(&cfg, k, xmap_full, xmap_half, amap, a);
   }
-  HQQ_LAUNCH_CHECK("hqq_b200_linear_fwd/tcgen05");
+  HQQ_LAUNCH_CHECK("hqq_b200_linear_fwd/wgmma");
   if (a.sched.ksplit > 1) {
     const long long total = (long long)a.M * a.N;
     const bool vec = a.step % 4 == 0 && PR % 4 == 0 && aligned(a.y, 8);
@@ -801,7 +779,7 @@ size_t gemm_workspace_bytes(int64_t M, int64_t N, int64_t K, int, int nbits, int
   return gemm::splitk_ws_bytes(gemm::make_sched(M, K, cdiv(N / F, PR), gemm::persistent_ctas(), true));
 }
 
-// y[M, N] = x[M, K] @ W[N, K]^T (+ bias), W an ordinary fp16/bf16 matrix: the same persistent tcgen05 kernel with both operands on TMA
+// y[M, N] = x[M, K] @ W[N, K]^T (+ bias), W an ordinary fp16/bf16 matrix: the same persistent wgmma kernel with both operands on TMA
 bool dense_route_ok(int64_t M, int64_t N, int64_t K, int dtype) {
   if (dtype != HQQ_F16 && dtype != HQQ_BF16) return false;
   return M >= 1 && N >= 1 && K >= 8 && K % 8 == 0 && N <= (1 << 28) && K <= (1 << 28) && M <= (1 << 28);  // 16-byte row pitch for the TMA

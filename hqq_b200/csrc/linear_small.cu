@@ -12,7 +12,7 @@
 // against x, a second MMA with an all-ones A tile yields sum_k x_k in the same fragment layout, and the
 // affine correction is applied once per group per accumulator (fp32).  mma.sync m16n8k16 with register A
 // fragments is used on purpose: at M <= 32 the kernel is bound by HBM and instruction issue, and a
-// register-operand MMA avoids the shared-memory round trip a tcgen05 operand would need.
+// register-operand MMA avoids the shared-memory round trip a wgmma operand would need.
 //
 // Scheduling: persistent CTAs walk the 16-row tiles of up to four weight matrices that share the activation (q/k/v,
 // gate/up) round-robin; the 8 warps of a CTA split K of a tile and stream their chunks through private cp.async rings
@@ -1019,7 +1019,7 @@ static int grid_for_kernel(int* grid_out) {
 static int balanced_grid(int tiles, int max_grid) {
   if (tiles <= max_grid) return tiles;
   HQQ_ENV_KNOB(mode, ([] { const char* e = getenv("HQQ_B200_BALANCED_GRID"); return (e && e[0] == '1') ? 1 : 0; })());
-  if (!mode) return max_grid;  // measured on B200: the kernel is bound per SM, so filling every CTA slot wins
+  if (!mode) return max_grid;  // the kernel is bound per SM, so filling every CTA slot wins
   int best = max_grid;
   double best_eff = 0.0;
   for (int g = max_grid; g >= max_grid / 2; --g) {
@@ -1099,8 +1099,8 @@ static int sk_mt(SKArgs& a, cudaStream_t st) {
   if (a.M == 1 && a.K <= 16384 && d1_enabled()) {
     if (NBITS == 8) return launch_d1<T, NBITS, GS, MAGIC, 2, 2>(a, st);
     // scale/zero ride the cp.async ring at the weights' distance (MR = 1) whenever the ring's aligned 16-byte copies are legal;
-    // measured on the B200 (round 2, profiles/r2_d1_variants.txt): 1.70 ms per token against 1.91 ms with register loads one
-    // unit ahead, bit-identical outputs.  evict-first hints, a third CTA per SM, L2 prefetch under the dependency wait and
+    // that keeps them off the critical path, where register loads one unit ahead expose their latency; the outputs are
+    // bit-identical.  evict-first hints, a third CTA per SM, L2 prefetch under the dependency wait and
     // cross-launch weight prefetch were measured in the same run, were not faster, and are gone.
     if constexpr (GS == 64 && NBITS != 8) {
       if (a.K % 512 == 0) {

@@ -1,4 +1,4 @@
-// Quantizer.quantize on sm_100a: min/max init -> proximal (half-quadratic) zero-point solver with the
+// Quantizer.quantize on sm_90a: min/max init -> proximal (half-quadratic) zero-point solver with the
 // reference's whole-tensor early stop -> round/clamp -> bit-pack.  Three launches, no host sync:
 //
 //   K1 solver_kernel     every group runs ALL `iters` iterations on-chip (weights stay in registers),
@@ -159,8 +159,8 @@ __device__ __forceinline__ void block_flush_errors(double (*err_w)[kMaxIters], i
 }
 
 // ---- K1, axis = 1: group = gs contiguous elements = L lanes x 8 elements, weights in registers -------------------------
-// Two exact shortcuts over the plain 20-iteration loop (solver_generic_kernel below is that plain loop; round 1 measured them
-// bit-identical on the B200 and ~3.2x faster, tests/test_quantize_gpu.py::test_register_solver_equals_plain_loop):
+// Two exact shortcuts over the plain 20-iteration loop (solver_generic_kernel below is that plain loop; the results are
+// bit-identical, tests/test_quantize_gpu.py::test_register_solver_equals_plain_loop):
 //  (1) shrink_lp_op(x) is exactly 0 wherever |x| - (1/beta)|x|^(p-1) <= 0, i.e. |x| <= beta^(-1/(2-p)) (0.170 for the
 //      default beta = 10, p = 0.7; optimize.py:96-108).  Quantisation errors of real weight matrices are far below that,
 //      so W_e = 0, `W_f - W_e` = W_f and the update collapses to z = mean(W_q - W_f*scale): no SFU work, and W_f*scale is

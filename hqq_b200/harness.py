@@ -63,7 +63,7 @@ class DecodeModel:
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
         # batch > 1 (BASELINE configs[4], bs = 32): `batch` sequences decode in lock-step at the same position; the linears then
-        # run the small-M kernel (M = batch <= 32; the tcgen05 kernel from 17 sequences on large matrices) between the batched glue
+        # run the small-M kernel (M = batch <= 32; the wgmma kernel from 17 sequences on large matrices) between the batched glue
         # kernels -- the one-token kernels and their NVLink exchange are M = 1 only, so tensor-parallel partials are summed by NCCL
         self.batch = int(batch)
         if self.batch < 1:
@@ -237,7 +237,7 @@ class DecodeModel:
 
     def _lin(self, x, layers, outs):
         """Matrices that share the activation x [B, K]: ONE launch of the small-M kernel when the router gives it all of them,
-        else one routed call per matrix (from 17 rows on, matrices above 2^24 weights take the tcgen05 kernel, csrc/linear.cu)."""
+        else one routed call per matrix (from 17 rows on, matrices above 2^24 weights take the wgmma kernel, csrc/linear.cu)."""
         if ops.linear_fwd_multi(x, layers, outs) is not None:
             return
         for l, y in zip(layers, outs):

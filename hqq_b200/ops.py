@@ -228,7 +228,7 @@ def linear_fwd(x2d: torch.Tensor, W_q: torch.Tensor, scale: torch.Tensor, zero: 
 
 
 def dense_gemm(x2d: torch.Tensor, W: torch.Tensor, bias=None, out: torch.Tensor | None = None) -> torch.Tensor | None:
-    """y = x2d @ W.T (+ bias) for an ordinary fp16/bf16 [N, K] matrix through the dense tcgen05 kernel (`hqq_b200_dense_gemm`);
+    """y = x2d @ W.T (+ bias) for an ordinary fp16/bf16 [N, K] matrix through the dense wgmma kernel (`hqq_b200_dense_gemm`);
     None when the shape / dtype is outside it (fp32, K not a multiple of 8)."""
     _lib.require_cuda(x2d, "the activation passed to dense_gemm")
     code = DTYPE_CODE.get(x2d.dtype, -1)

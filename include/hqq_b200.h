@@ -1,5 +1,5 @@
 /*
- * hqq_b200 -- C ABI of the B200 (sm_100a) HQQ quantize-and-infer hot path.
+ * hqq_b200 -- C ABI of the H100 (sm_90a) HQQ quantize-and-infer hot path.
  *
  * This is the drop-in boundary: plain pointers (device memory owned by the caller),
  * sizes and a cudaStream_t passed as void*.  No torch types, no allocation, no host
@@ -132,9 +132,9 @@ int hqq_b200_quantize_shard_finish(const void* W, int src_dtype, int64_t N, int6
  *   hqq/core/quantize.py:880-898 ; semantic template hqq/kernels/hqq_aten_torch.cpp:79-107
  *   x [M,K], y [M,N], bias [N] or NULL, scale/zero [N*K/gs], all of `dtype` (f16/bf16)
  *   Routes (hqq_b200_linear_fwd_route): 1 = small-M weight-streaming kernel (M <= 16; M <= 32 on matrices of up to 2^24 weights),
- *   2 = fused tcgen05 GEMM -- both axis 1,
+ *   2 = fused wgmma GEMM -- both axis 1,
  *   nbits 8/4/2/1, group_size 64/128, K % 256 == 0 -- and 3 = everything else hqq_b200_dequantize accepts (3-bit, axis 0, other
- *   group sizes, ragged K): the dequantize kernel writes W_r into `workspace`, the dense tcgen05 GEMM multiplies.  Returns
+ *   group sizes, ragged K): the dequantize kernel writes W_r into `workspace`, the dense wgmma GEMM multiplies.  Returns
  *   HQQ_E_UNSUPPORTED where none applies (fp32 compute).
  *   workspace: hqq_b200_linear_fwd_workspace_bytes() bytes, 256-byte aligned scratch owned by the caller: 0 for route 1
  *   (split-K partials of the small-M kernel meet in shared memory); route 2: 0 unless the problem has so few output tiles
@@ -147,7 +147,7 @@ int hqq_b200_linear_fwd(const void* x, const void* W_q, const void* scale, const
                         int group_size, int nbits, int axis, int dtype,
                         void* workspace, size_t workspace_bytes, void* stream);
 
-/* y[M,N] = x[M,K] @ W[N,K]^T (+ bias) for an ordinary fp16/bf16 matrix W: the persistent tcgen05 kernel of route 2 with both
+/* y[M,N] = x[M,K] @ W[N,K]^T (+ bias) for an ordinary fp16/bf16 matrix W: the persistent wgmma kernel of route 2 with both
  * operands on TMA.  Used by route 3 and by the backward pass of HQQMatmulNoCacheMul (grad_out @ W_r, hqq/core/quantize.py:322-352:
  * W = W_r^T).  K % 8 == 0 (16-byte row pitch), x / W 16-byte aligned.                                                        */
 int hqq_b200_dense_gemm(const void* x, const void* W, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
@@ -164,7 +164,7 @@ int hqq_b200_linear_fwd_multi(const void* x, int count, const void* const* W_q, 
                               void* workspace, size_t workspace_bytes, void* stream);
 
 /* Which kernels hqq_b200_linear_fwd would use: 0 none (unsupported), 1 small-M mma.sync weight-streaming kernel,
- * 2 fused tcgen05/TMA GEMM, 3 dequantize kernel + dense tcgen05 GEMM.                                         */
+ * 2 fused wgmma/TMA GEMM, 3 dequantize kernel + dense wgmma GEMM.                                         */
 int hqq_b200_linear_fwd_route(int64_t M, int64_t N, int64_t K, int group_size, int nbits,
                               int axis, int dtype);
 

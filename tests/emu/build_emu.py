@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE ONLY: build `libhqq_b200_emu.so` -- the kernels of hqq_b200/csrc (quantizer, bit-packing, small-M / one-token
-forward, tcgen05 GEMM, the decode glue kernels except the cluster argmax) compiled by g++ against tests/emu/include/cuda_runtime.h and
+forward, wgmma GEMM, the decode glue kernels except the cluster argmax) compiled by g++ against tests/emu/include/cuda_runtime.h and
 executed on the CPU by cooperative fibers.
 
 The .cu sources are used as they are, except for two textual rewrites CUDA syntax forces on a C++ compiler:

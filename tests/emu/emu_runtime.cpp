@@ -53,7 +53,8 @@ static bool fire_due(bool all) {
   return fired;
 }
 unsigned g_mma_a[64][32][4], g_mma_b[64][32][2];
-float g_tmem[128][512];
+std::vector<Wgmma> g_wg_open[2048];
+std::vector<std::vector<Wgmma>> g_wg_groups[2048];
 std::vector<Copy> g_cp_open[2048];
 std::vector<std::vector<Copy>> g_cp_groups[2048];
 Barrier g_named_bar[16];
@@ -73,7 +74,7 @@ void run_block(std::function<void()> body, dim3 block) {
   g_body = body;
   for (auto& b : g_warp_bar) b = Barrier();
   g_block_bar = Barrier();
-  for (int t = 0; t < 2048; ++t) { g_cp_open[t].clear(); g_cp_groups[t].clear(); }
+  for (int t = 0; t < 2048; ++t) { g_cp_open[t].clear(); g_cp_groups[t].clear(); g_wg_open[t].clear(); g_wg_groups[t].clear(); }
   for (auto& b : g_named_bar) b = Barrier();
   std::vector<Fiber> fibers(n);
   g_fibers = &fibers;

@@ -1,4 +1,4 @@
-// TEST INFRASTRUCTURE ONLY -- a stand-in for <cuda_runtime.h> that lets the *simple* kernels of hqq_b200/csrc (no tcgen05, TMA,
+// TEST INFRASTRUCTURE ONLY -- a stand-in for <cuda_runtime.h> that lets the *simple* kernels of hqq_b200/csrc (no wgmma, TMA,
 // cp.async, mma.sync or inline PTX on their path) be compiled by g++ and EXECUTED ON THE CPU by a cooperative-fiber emulator:
 // every CUDA thread of a block is a ucontext fiber, warp collectives (__shfl_xor_sync, __any_sync, __all_sync, __syncwarp) and
 // __syncthreads are rendezvous points between fibers.  It exists so that kernels written without access to a GPU can be executed
@@ -175,16 +175,14 @@ inline unsigned lop3(unsigned a, unsigned b, unsigned c, unsigned lut) {
 
 }  // namespace emu
 
-// ---- functional model of the Blackwell tensor-core path used by csrc/linear_gemm.cu ------------------------------------------
-// mbarrier (arrival count + transaction bytes + phase), TMA 2-D tile loads with SWIZZLE_128B, UMMA descriptors (K-major,
-// SWIZZLE_128B), tcgen05.mma kind::f16 (M = 128, N from the instruction descriptor) accumulating into a [128 lanes x 512 columns]
-// fp32 TMEM array, tcgen05.ld 32x32b.x32.  MMAs and copies complete at issue; what is modelled is the LOGIC (addresses,
-// swizzles, phases, who waits for whom) -- a protocol that deadlocks here is reported by the scheduler -- not timing, proxies
-// or memory ordering.
+// ---- functional model of the Hopper tensor-core path used by csrc/linear_gemm.cu --------------------------------------------
+// mbarrier (arrival count + transaction bytes + phase), TMA 2-D tile loads with SWIZZLE_128B, wgmma shared-memory descriptors
+// (K-major, SWIZZLE_128B), wgmma.mma_async m64nNk16 f32 += f16/bf16 into each thread's register fragment, commit_group /
+// wait_group.  What is modelled is the LOGIC (addresses, swizzles, fragment layouts, phases, who waits for whom) -- a protocol
+// that deadlocks here is reported by the scheduler -- not timing, proxies or memory ordering.
 namespace emu {
 struct Mbar { uint16_t init, pending; int32_t tx; };  // the 8 bytes of the kernel's uint64_t; phase in the sign of `init`'s top bit
 static_assert(sizeof(Mbar) == 8, "mbarrier model must fit the 64-bit object");
-extern float g_tmem[128][512];
 extern Barrier g_named_bar[16];
 inline uint32_t smem_offset(const void* p) { return (uint32_t)(reinterpret_cast<const char*>(p) - dyn_smem); }
 inline char* smem_ptr(uint32_t off) { return dyn_smem + off; }
@@ -259,38 +257,40 @@ inline float smem_half(uint32_t start, int row, int k, bool bf16) {  // K-major 
   memcpy(&h, dyn_smem + phys, 2);
   return bf16 ? half_bits_to_float<__nv_bfloat16>(h) : half_bits_to_float<__half>(h);
 }
-inline void umma_now(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  const int N = (int)((idesc >> 17) & 0x3Fu) << 3, M = (int)((idesc >> 24) & 0x1Fu) << 4;
-  const bool bf16 = ((idesc >> 7) & 7u) == 1u;
-  if (M != 128 || N < 8 || N > 256 || (adesc >> 61) != 2 || (bdesc >> 61) != 2) { fprintf(stderr, "emu: unsupported UMMA descriptor\n"); abort(); }
-  const uint32_t sa = (uint32_t)(adesc & 0x3FFFu) << 4, sb = (uint32_t)(bdesc & 0x3FFFu) << 4;
-  const int col0 = (int)(tmem_d & 0xFFFFu), lane0 = (int)(tmem_d >> 16);
-  if (col0 + N > 512 || lane0 != 0) { fprintf(stderr, "emu: accumulator outside TMEM\n"); abort(); }
-  static float Bt[256][16];
-  for (int n = 0; n < N; ++n)
-    for (int k = 0; k < 16; ++k) Bt[n][k] = smem_half(sb, n, k, bf16);
-  for (int r = 0; r < 128; ++r) {
-    float a[16];
-    for (int k = 0; k < 16; ++k) a[k] = smem_half(sa, r, k, bf16);
-    for (int n = 0; n < N; ++n) {
-      float acc = accumulate ? g_tmem[r][col0 + n] : 0.0f;
-      for (int k = 0; k < 16; ++k) acc += a[k] * Bt[n][k];
-      g_tmem[r][col0 + n] = acc;
-    }
-  }
+// wgmma.mma_async: operands are read when the operation EXECUTES.  The model runs a thread's wgmma groups at the latest moment
+// the program may rely on their results or on their operands no longer being needed -- its wgmma.wait_group -- so a kernel
+// that frees a stage before the group reading it has retired multiplies overwritten data.
+struct Wgmma { float* d; int N; uint32_t sa, sb; bool accumulate, bf16; };
+extern std::vector<Wgmma> g_wg_open[2048];               // per thread: wgmmas not yet committed
+extern std::vector<std::vector<Wgmma>> g_wg_groups[2048];  // per thread: committed groups, oldest first
+inline void wgmma_now(const Wgmma& w) {
+  // thread (warp ww, lane l) of the warpgroup owns rows 16 ww + l/4 (+ 8), columns 8 j + 2 (l % 4) (+ 1): d[4 j + 2 h + e]
+  const int tw = linear_tid() & 127, ww = tw >> 5, l = tw & 31;
+  for (int j = 0; j < w.N / 8; ++j)
+    for (int h = 0; h < 2; ++h)
+      for (int e = 0; e < 2; ++e) {
+        const int r = 16 * ww + (l >> 2) + 8 * h, n = 8 * j + 2 * (l & 3) + e;
+        float acc = w.accumulate ? w.d[4 * j + 2 * h + e] : 0.0f;
+        for (int k = 0; k < 16; ++k) acc += smem_half(w.sa, r, k, w.bf16) * smem_half(w.sb, n, k, w.bf16);
+        w.d[4 * j + 2 * h + e] = acc;
+      }
   ++g_progress;
 }
-// operands are read when the operation EXECUTES, which is when the deferred event fires
-inline void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  defer_ordered([=]() { umma_now(tmem_d, adesc, bdesc, idesc, accumulate); });
+inline void wgmma_f16(float* d, int N, uint64_t adesc, uint64_t bdesc, bool accumulate, bool bf16) {
+  if (N < 8 || N > 256 || N % 8 || (adesc >> 62) != 1 || (bdesc >> 62) != 1 || ((adesc >> 32) & 0x3FFFu) != 64 || ((bdesc >> 32) & 0x3FFFu) != 64) {
+    fprintf(stderr, "emu: unsupported wgmma descriptor\n");
+    abort();
+  }
+  const uint32_t sa = (uint32_t)(adesc & 0x3FFFu) << 4, sb = (uint32_t)(bdesc & 0x3FFFu) << 4;
+  g_wg_open[linear_tid()].push_back(Wgmma{d, N, sa, sb, accumulate, bf16});
 }
-// tcgen05.commit: the barrier is signalled once every tensor-core operation issued before it has executed
-inline void tc_commit(uint64_t* bar) { defer_ordered([=]() { mbar_arrive(bar); }); }
-inline void tmem_alloc(uint32_t* dst, int) { *dst = 0u; }
-inline void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  const int lane = (int)(taddr >> 16) + (linear_tid() & 31), col = (int)(taddr & 0xFFFFu);
-  if (lane >= 128 || col + 32 > 512) { fprintf(stderr, "emu: tcgen05.ld outside TMEM\n"); abort(); }
-  for (int j = 0; j < 32; ++j) memcpy(&v[j], &g_tmem[lane][col + j], 4);
+inline void wgmma_commit() { const int t = linear_tid(); g_wg_groups[t].push_back(std::move(g_wg_open[t])); g_wg_open[t].clear(); }
+inline void wgmma_wait(int allow_pending) {
+  auto& q = g_wg_groups[linear_tid()];
+  while ((int)q.size() > allow_pending) {
+    for (const Wgmma& w : q.front()) wgmma_now(w);
+    q.erase(q.begin());
+  }
 }
 inline void sts(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) { const uint32_t v[4] = {a, b, c, d}; memcpy(dyn_smem + addr, v, 16); }
 inline void sts(uint32_t addr, uint32_t a, uint32_t b) { const uint32_t v[2] = {a, b}; memcpy(dyn_smem + addr, v, 8); }

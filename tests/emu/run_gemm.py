@@ -1,5 +1,5 @@
-"""TEST INFRASTRUCTURE ONLY: run the emulated tcgen05 GEMM (csrc/linear_gemm.cu on the fiber emulator's functional model of
-mbarrier / TMA / tcgen05 / TMEM) over a fixed seeded case list under the HQQ_B200_* knobs of THIS process and save every output
+"""TEST INFRASTRUCTURE ONLY: run the emulated wgmma GEMM (csrc/linear_gemm.cu on the fiber emulator's functional model of
+mbarrier / TMA / wgmma) over a fixed seeded case list under the HQQ_B200_* knobs of THIS process and save every output
 plus the oracle's to an .npz (tests/test_emu_cpu.py compares)."""
 import ctypes
 import os
@@ -14,14 +14,14 @@ import build_emu  # noqa: E402
 import run_small as R  # noqa: E402
 from oracle import hqq_oracle as O  # noqa: E402
 
-# (nbits, gs, N, K, M, bias): ragged row tiles (N % 128 != 0), ragged token tiles, every UN (64/128/256), M > 256 and > 512 for the
+# (nbits, gs, N, K, M, bias): ragged row tiles (N % 128 != 0), ragged token tiles, both UN (64/128), M > 256 and > 512 for the
 # two-accumulator variant, few tiles x long K for split-K
 CASES = [(4, 64, 128, 256, 64, False), (4, 64, 256, 512, 200, True), (2, 128, 128, 256, 40, False), (8, 64, 128, 256, 300, False),
          (1, 64, 256, 256, 64, True), (4, 64, 200, 512, 600, False), (4, 128, 136, 1024, 257, True), (2, 64, 64, 768, 1030, False),
          (4, 64, 128, 2048, 128, False), (4, 64, 264, 1280, 100, True), (8, 128, 128, 512, 513, False), (4, 64, 128, 256, 33, False)]
 
 
-# route 3 (dequantize kernel -> dense tcgen05 GEMM, both operands on TMA): 3-bit, a group size the fused kernels do not take, ragged K
+# route 3 (dequantize kernel -> dense wgmma GEMM, both operands on TMA): 3-bit, a group size the fused kernels do not take, ragged K
 DENSE_CASES = [(3, 64, 130, 256, 40, True), (3, 64, 128, 512, 300, False), (4, 32, 128, 256, 64, False), (4, 64, 96, 320, 70, True),
                (2, 16, 64, 80, 33, False)]
 

@@ -59,17 +59,17 @@ def test_forward_routing_table(lib):
     assert r(1, 4096, 4096, 64, 4, 1, HQQ_F16) == 1      # decode: weight-streaming kernel
     assert r(16, 14336, 4096, 64, 4, 1, HQQ_BF16) == 1   # up to 16 tokens the weight-streaming kernel wins on every matrix
     assert r(32, 4096, 4096, 64, 4, 1, HQQ_BF16) == 1    # 17..32 tokens: still on matrices up to 4096 x 4096 ...
-    assert r(32, 14336, 4096, 64, 4, 1, HQQ_BF16) == 2   # ... larger ones go to the tcgen05 kernel (measured boundary, linear.cu)
+    assert r(32, 14336, 4096, 64, 4, 1, HQQ_BF16) == 2   # ... larger ones go to the wgmma kernel (boundary rule, linear.cu)
     assert r(17, 4096, 14336, 64, 4, 1, HQQ_F16) == 2
     assert r(32, 3584, 8192, 64, 4, 1, HQQ_F16) == 2 and r(32, 1280, 8192, 64, 4, 1, HQQ_F16) == 1   # the boundary: 2^24 weights
     assert r(32, 14336, 4096, 64, 4, 1, HQQ_F32) == 0
-    assert r(1, 4096, 4096, 64, 4, 0, HQQ_F16) == 3      # axis 0: dequantize kernel + dense tcgen05 GEMM
+    assert r(1, 4096, 4096, 64, 4, 0, HQQ_F16) == 3      # axis 0: dequantize kernel + dense wgmma GEMM
     assert r(1, 4096, 4096, 64, 4, 1, HQQ_F32) == 0      # float32 compute: no tensor-core route
     assert r(1, 4096, 4096, 64, 3, 1, HQQ_F16) == 3      # 3-bit (ten fields per int32, slabs cut rows): route 3
     assert r(1, 4096, 4000, 64, 4, 1, HQQ_F16) == 3      # the fused kernels need K % 256 == 0; the dense GEMM's TMA zero-fills ragged K
     assert r(1, 4096, 4096, 128, 2, 1, HQQ_BF16) == 1
     assert r(1, 4096, 4096, 32, 4, 1, HQQ_F16) == 3      # group sizes other than 64/128
-    assert r(4096, 4096, 4096, 64, 4, 1, HQQ_F16) == 2   # fused tcgen05 GEMM
+    assert r(4096, 4096, 4096, 64, 4, 1, HQQ_F16) == 2   # fused wgmma GEMM
     wsb = lib.hqq_b200_linear_fwd_workspace_bytes
     assert wsb(1, 4096, 4096, 64, 4, 1, HQQ_F16) == 0 and wsb(4096, 4096, 4096, 64, 4, 1, HQQ_F16) == 0
     assert wsb(128, 4096, 4096, 64, 4, 1, HQQ_F16) % (32 * 256 * 128 * 4) == 0 and wsb(128, 4096, 4096, 64, 4, 1, HQQ_F16) > 0  # few tiles: split-K partials

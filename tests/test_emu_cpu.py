@@ -1,5 +1,5 @@
 """CPU: the kernels of hqq_b200/csrc EXECUTED on the CPU by the cooperative-fiber emulator in tests/emu (every CUDA thread a fiber,
-warp collectives and __syncthreads as rendezvous; mbarrier / TMA / tcgen05 / TMEM / cp.async / mma.sync as functional models)
+warp collectives and __syncthreads as rendezvous; mbarrier / TMA / wgmma / cp.async / mma.sync as functional models)
 and compared with the oracle and the reference's fixtures.
 
 Why: kernels are written in a container without a GPU.  This executes the very same source text (two syntactic rewrites, see
@@ -95,7 +95,7 @@ def test_emulated_pack_unpack_dequantize_match_the_oracle(emu, oracle):
 
 @pytest.mark.parametrize("nbits,gs,shape,std", [(4, 64, (32, 256), 0.02), (2, 32, (16, 128), 0.5), (3, 64, (25, 128), 0.02)])
 def test_emulated_default_solver_matches_the_oracle(emu, oracle, nbits, gs, shape, std):
-    """Pins the emulator itself: the DEFAULT solver kernel, which has been validated on a B200 against the oracle, must agree with
+    """Pins the emulator itself: the DEFAULT solver kernel, which the GPU suite validates against the oracle, must agree with
     the oracle here to the same tolerances (tests/test_quantize_gpu.py)."""
     rng = np.random.default_rng(nbits)
     W = (rng.standard_normal(shape) * std).astype(np.float32)
@@ -254,8 +254,8 @@ def test_emulated_one_token_prologues_and_paired_epilogue(emu, oracle, tmp_path_
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-# csrc/linear_gemm.cu on the emulator's functional model of mbarrier / TMA (SWIZZLE_128B) / UMMA descriptors / tcgen05.mma /
-# TMEM / tcgen05.ld: addresses, swizzles, barrier phases and who-waits-for-whom are executed; timing, async proxies and memory
+# csrc/linear_gemm.cu on the emulator's functional model of mbarrier / TMA (SWIZZLE_128B) / wgmma descriptors / wgmma.mma_async
+# register fragments / wait_group: addresses, swizzles, barrier phases and who-waits-for-whom are executed; timing, async proxies and memory
 # ordering are not.  A barrier protocol that cannot make progress is reported as a deadlock by the scheduler.
 # ---------------------------------------------------------------------------------------------------------------------------
 GEMM_RUNNER = os.path.join(HERE, "emu", "run_gemm.py")
@@ -283,7 +283,7 @@ def test_emulated_tcgen05_gemm_matches_the_oracle(emu, tmp_path_factory):
     assert len(refs) == 12
     dense = [k for k in d if k.endswith("_ref") and k.startswith("dense")]
     assert len(dense) == 5
-    for k in dense:  # route 3: W_r from the dequantize kernel (the reference's two roundings), dense tcgen05 GEMM, fp32 accumulation
+    for k in dense:  # route 3: W_r from the dequantize kernel (the reference's two roundings), dense wgmma GEMM, fp32 accumulation
         assert rel(d[k[:-4]], d[k]) <= 1e-4, k
     for k in refs:
         # the A operand is dequantised with the reference's two roundings and accumulated in fp32: far inside the fp16 tolerance
@@ -294,7 +294,7 @@ def test_emulated_tcgen05_gemm_matches_the_oracle(emu, tmp_path_factory):
 
 @pytest.mark.parametrize("knob", [("HQQ_B200_GEMM_CTAS", "1"), ("HQQ_B200_GEMM_CTAS", "3"), ("HQQ_B200_GEMM_CTAS", "5"), ("HQQ_B200_GEMM_CTAS", "24")])
 def test_emulated_persistent_gemm_schedules_are_bit_identical(emu, tmp_path_factory, knob):
-    """The persistent kernel with its grid capped to 1 / 3 / 5 CTAs: every CTA then walks several tiles (both TMEM accumulators,
+    """The persistent kernel with its grid capped to 1 / 3 / 5 CTAs: every CTA then walks several tiles (accumulators reused,
     epilogue of tile i under the main loop of tile i + 1, rings running across tile boundaries, the half-tile round of the
     schedule) and issues the same MMAs in the same k order per output element as the one-tile-per-CTA run: identical outputs,
     and no barrier protocol that stalls."""
@@ -335,7 +335,7 @@ def test_emulated_tensor_parallel_exchange(emu, tmp_path, tp):
 
 def test_emulated_forward_random_shapes(emu, oracle):
     """Seeded sweep over what the router accepts (4/2/1/8-bit, gs 64/128, K a multiple of 256, M = 1..300, ragged N, bias or not):
-    whichever kernel hqq_b200_linear_fwd picks -- one-token, generic small-M or tcgen05 GEMM -- must agree with the oracle.  600
+    whichever kernel hqq_b200_linear_fwd picks -- one-token, generic small-M or wgmma GEMM -- must agree with the oracle.  600
     further configurations from other seeds were run while developing this; none exceeded 5.4e-4."""
     sys.path.insert(0, os.path.join(HERE, "emu"))
     import run_small as R

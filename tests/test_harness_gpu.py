@@ -230,7 +230,7 @@ def test_batched_glue_kernels_equal_the_one_sequence_kernels_row_by_row(dt):
                                          (32, harness.LlamaShape(hidden=4096, inter=14336, n_layers=1, n_heads=32, n_kv_heads=8, vocab=4096))])
 def test_batched_decode_graph_fused_equals_framework_ops(batch, shape):
     """Lock-step batch: the captured step on the batched glue kernels (add+RMSNorm rows, RoPE+attention per sequence, SiLU*mul; the
-    linears through `_lin`: small-M kernel, or the tcgen05 kernel for 17+ sequences on matrices above 2^24 weights -- the second
+    linears through `_lin`: small-M kernel, or the wgmma kernel for 17+ sequences on matrices above 2^24 weights -- the second
     case has such matrices) against the same step on framework ops, every sequence starting from its own token."""
     toks = []
     for f in (True, False):
@@ -251,7 +251,7 @@ def test_batched_decode_graph_fused_equals_framework_ops(batch, shape):
     assert len(set(a[0].tolist())) > 1                               # the sequences are really different
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (the fused NVLink exchange is exercised by tools/tp_check.py under gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (tools/tp_check.py exercises the fused NVLink exchange on a 2-GPU machine)")
 def test_tensor_parallel_peer_exchange_matches_nccl():
     """TP=2: the all-reduce fused into the row-parallel kernels over peer memory produces the same tokens as NCCL all-reduce."""
     import os

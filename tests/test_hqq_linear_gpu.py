@@ -125,7 +125,7 @@ def test_module_plumbing(lin):
 def test_layers_on_a_device_that_is_not_current():
     """BaseHQQModel.quantize_model(device=[...]) spreads layers over GPUs of one process: a layer on cuda:1 must launch on cuda:1 while
     cuda:0 is current (the C ABI launches on the calling thread's current device: ops.py guards it, the function-attribute and grid
-    caches of the kernels are per device) -- every route: one-token kernel, small-M kernel, tcgen05 GEMM, dequantize + dense GEMM."""
+    caches of the kernels are per device) -- every route: one-token kernel, small-M kernel, wgmma GEMM, dequantize + dense GEMM."""
     torch.manual_seed(21)
     assert torch.cuda.current_device() == 0
     for cfg in (dict(nbits=4, group_size=64, axis=1), dict(nbits=3, group_size=64, axis=1)):

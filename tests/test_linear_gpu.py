@@ -85,8 +85,8 @@ def test_small_m_kernel_vs_oracle(oracle, nbits, dtype, gs):
 @pytest.mark.parametrize("dtype", ["float16", "bfloat16"])
 @pytest.mark.parametrize("gs", [64, 128])
 def test_tcgen05_gemm_vs_oracle(oracle, nbits, dtype, gs):
-    """The tcgen05/TMA kernel (route 2): every bit width, both group sizes, token counts that exercise every UMMA N
-    (64/128/256), partial token tiles, ragged weight tiles, K not a multiple of 256, bias."""
+    """The wgmma/TMA kernel (route 2): every bit width, both group sizes, token counts that exercise both wgmma N
+    (64/128), partial token tiles, ragged weight tiles, K not a multiple of 256, bias."""
     rng = np.random.RandomState(7 * nbits + gs)
     f = 8 // nbits
     N, K = 40 * f, 512  # 40 packed rows: partial 128-row tile for every bit width; K = 8 k-blocks = 2 register quads
@@ -174,7 +174,7 @@ def test_forward_is_deterministic_and_batch_invariant():
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16, torch.float32])
 def test_every_config_has_a_forward(cfg, dt):
     """Configurations outside the fused kernels (axis=0, 3-bit, other group sizes) run route 3: our dequantize kernel + the dense
-    tcgen05 GEMM (float32 compute: dequantize kernel + library GEMM); results agree with the explicit dequantise-then-matmul
+    wgmma GEMM (float32 compute: dequantize kernel + library GEMM); results agree with the explicit dequantise-then-matmul
     definition (quantize.py:880-898)."""
     torch.manual_seed(9)
     lin = torch.nn.Linear(256, 128, bias=True)
@@ -216,7 +216,7 @@ def test_backward_matches_dequant_matmul():
 @pytest.mark.parametrize("M,N,K", [(1, 256, 512), (40, 384, 1000), (300, 130, 72), (1024, 4096, 4096), (257, 11008, 4096)])
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 def test_dense_tcgen05_gemm_vs_fp32_matmul(M, N, K, dt):
-    """hqq_b200_dense_gemm (the persistent tcgen05 kernel with both operands on TMA): ragged rows / tokens / K (K % 8 == 0 only),
+    """hqq_b200_dense_gemm (the persistent wgmma kernel with both operands on TMA): ragged rows / tokens / K (K % 8 == 0 only),
     bias, against an fp32 matmul of the same 16-bit operands."""
     torch.manual_seed(M + N + K)
     x = torch.randn(M, K, device=DEV).to(dt)
@@ -231,7 +231,7 @@ def test_dense_tcgen05_gemm_vs_fp32_matmul(M, N, K, dt):
 
 @pytest.mark.parametrize("cfg", [dict(nbits=3, group_size=64, axis=1), dict(nbits=4, group_size=64, axis=0), dict(nbits=2, group_size=32, axis=1)])
 def test_route3_full_size(cfg):
-    """3-bit / axis 0 / other group sizes at a BASELINE sweep size: route 3 (dequantize kernel -> dense tcgen05 GEMM) against an fp32
+    """3-bit / axis 0 / other group sizes at a BASELINE sweep size: route 3 (dequantize kernel -> dense wgmma GEMM) against an fp32
     GEMM over the (bit-exactly tested) dequantised matrix; the A operand IS that matrix, so only the accumulation order differs."""
     torch.manual_seed(11)
     N, K = 4096, 4096
@@ -246,7 +246,7 @@ def test_route3_full_size(cfg):
 
 
 def test_persistent_gemm_schedule_is_result_invariant(monkeypatch):
-    """HQQ_B200_GEMM_CTAS caps the persistent grid: 7 CTAs walk 32 x 5 tiles one after another (both TMEM accumulators, epilogue under
+    """HQQ_B200_GEMM_CTAS caps the persistent grid: 7 CTAs walk 32 x 5 tiles one after another (accumulators reused, epilogue under
     the next main loop, the half-tile round) and must reproduce the full-grid result bit for bit."""
     from hqq_b200 import _lib
     torch.manual_seed(12)

@@ -4,8 +4,8 @@ oracle.
 Stated tolerances (SURVEY.md 8c; the solver is a fixed-point iteration whose float32 rounding order decides
 round-half ties, so bit-exactness is only required where the arithmetic is order-free):
   * optimize=False (init, round-half-even, clamp, packing, 1/scale): BIT-EXACT.
-  * optimize=True, the reference's own fixtures: scale bit-exact, the SAME iteration count and EVERY level identical (what round 1's
-    B200 run demonstrated on all 14 configurations); zero-points to 2e-6; error trajectory to 5e-5.  Comparisons against the
+  * optimize=True, the reference's own fixtures: scale bit-exact, the SAME iteration count and EVERY level identical (on all 14
+    configurations); zero-points to 2e-6; error trajectory to 5e-5.  Comparisons against the
     oracle on other random matrices keep a +-1 iteration / <= 1 level / <= 5e-4 bound (the early stop compares float32 means that
     can tie to the last bit, and every implementation sums them in its own order).
 """

@@ -1,5 +1,5 @@
 """GPU: the model walker end to end (SURVEY.md 8 f-1) -- a tiny Llama is quantised through `AutoHQQHFModel.quantize_model` on the
-B200 and compared with the checkpoint the REAL reference produced from the same dense weights (tests/golden/models)."""
+GPU and compared with the checkpoint the REAL reference produced from the same dense weights (tests/golden/models)."""
 import os
 
 import pytest

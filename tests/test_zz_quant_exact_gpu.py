@@ -1,7 +1,7 @@
 """GPU: with the zero-point means accumulated in float64 the solver is expected to reproduce EVERY level of the reference's fixtures
 (it does when the kernels' source runs on the emulator, tests/test_emu_cpu.py).  Written after round 1's GPU budget was spent: the
 bound the validated suite asserts stays <= 5e-4 (tests/test_quantize_gpu.py); this stricter statement is a non-strict xfail until it
-has been seen on a B200 (the SFU's ex2/lg2 only matter for elements whose error survives the shrinkage -- none in these fixtures)."""
+has been seen on the GPU (the SFU's ex2/lg2 only matter for elements whose error survives the shrinkage -- none in these fixtures)."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Time the fused tcgen05 dequant-GEMM over the BASELINE sweep (and cuBLAS on the dequantised matrix for reference)."""
+"""Time the fused wgmma dequant-GEMM over the BASELINE sweep (and cuBLAS on the dequantised matrix for reference)."""
 import os
 import sys
 

@@ -1,7 +1,7 @@
 """Launch each of the four per-block launch groups of a decode step (q+k+v, o, gate+up, down; Llama-3-8B shapes, 4-bit gs=64)
 on cold weights -- the target of the `ncu --set full` capture whose dram bytes fill bench.py's roofline.traffic.
 
-    ncu --set full --clock-control none --import-source on -k regex:linear_decode1 -o gpurun_out/prof_groups python tools/prof_groups.py
+    ncu --set full --clock-control none --import-source on -k regex:linear_decode1 -o prof_groups python tools/prof_groups.py
 """
 import os
 import sys
@@ -21,7 +21,7 @@ for name, K, Ns in groups:
               for N in Ns]
     x = torch.randn(1, K, device="cuda").half()
     outs = [torch.empty(1, N, device="cuda", dtype=torch.float16) for N in Ns]
-    flush.fill_(1)  # evict the freshly written weights from the 126 MB L2
+    flush.fill_(1)  # evict the freshly written weights from the 50 MB L2
     torch.cuda.synchronize()
     assert ops.decode_linear_fwd(x, layers, outs, ops.YOP_SILU_MUL_PAIR if name == "gate_up" else 0)  # the MLP launch ships paired
     torch.cuda.synchronize()

@@ -1,4 +1,4 @@
-"""Mid-M (33..512) options on 4096x4096 4-bit: fused tcgen05 route, dequantize + dense tcgen05 (route 3's data flow), the small-M kernel in
+"""Mid-M (33..512) options on 4096x4096 4-bit: fused wgmma route, dequantize + dense wgmma (route 3's data flow), the small-M kernel in
 chunks of 32 tokens, and cuBLAS on the dequantised matrix -- to decide the router's boundaries."""
 import os
 import sys
@@ -41,5 +41,5 @@ for N, K in ((4096, 4096), (14336, 4096)):
                 ops.linear_fwd(x[i:i + 32], layer.W_q, m["scale"], m["zero"], None, N, K, 64, 4, 1, out=y[i:i + 32])
 
         t_chunk = timed(chunks)
-        print(f"N={N} K={K} M={M:4d}: fused {t_f:7.1f} us | dequantize {t_dq:6.1f} + dense tcgen05 {t_dense:6.1f} = {t_dq + t_dense:6.1f} | small-M x{(M + 31) // 32} {t_chunk:7.1f} | cuBLAS(dequantised) {t_cublas:6.1f}",
+        print(f"N={N} K={K} M={M:4d}: fused {t_f:7.1f} us | dequantize {t_dq:6.1f} + dense wgmma {t_dense:6.1f} = {t_dq + t_dense:6.1f} | small-M x{(M + 31) // 32} {t_chunk:7.1f} | cuBLAS(dequantised) {t_cublas:6.1f}",
               flush=True)

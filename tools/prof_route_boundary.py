@@ -1,5 +1,5 @@
-"""Where should the single-matrix forward hand over from the small-M kernel to the tcgen05 kernel?  GPU time (CUDA graph of 20 calls)
-of both for M = 8 ... 32 on Llama-3-8B-sized matrices, 4-bit gs 64: HQQ_B200_SMALL_M_MAX = 32 (small kernel) against = 1 (tcgen05)."""
+"""Where should the single-matrix forward hand over from the small-M kernel to the wgmma kernel?  GPU time (CUDA graph of 20 calls)
+of both for M = 8 ... 32 on Llama-3-8B-sized matrices, 4-bit gs 64: HQQ_B200_SMALL_M_MAX = 32 (small kernel) against = 1 (wgmma)."""
 import os
 import sys
 
@@ -58,4 +58,4 @@ for N, K in SHAPES:
             t[cap] = graph_us(lambda: ops.linear_fwd(x, layer.W_q, m["scale"], m["zero"], None, N, K, 64, 4, 1, out=y))
         del os.environ["HQQ_B200_SMALL_M_MAX"]
         lib.hqq_b200_reload_env()
-        print(f"N={N} K={K} M={M:3d}: small-M kernel {t[32]:6.1f} us | tcgen05 kernel {t[1]:6.1f} us", flush=True)
+        print(f"N={N} K={K} M={M:3d}: small-M kernel {t[32]:6.1f} us | wgmma kernel {t[1]:6.1f} us", flush=True)

@@ -1,4 +1,4 @@
-"""GPU time (CUDA graph of 20 calls, so no host launch overhead) of the fused tcgen05 route at mid M against the largest number of
+"""GPU time (CUDA graph of 20 calls, so no host launch overhead) of the fused wgmma route at mid M against the largest number of
 k-slices the schedule may use (HQQ_B200_GEMM_KSPLIT = 1 / 2 / 4 / 8), with the reference's flow (dequantize kernel + cuBLAS) and
 cuBLAS alone on the dequantised matrix beside it."""
 import os

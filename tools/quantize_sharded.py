@@ -1,4 +1,4 @@
-"""Quantise-only run, layers sharded across ranks (BASELINE configs[3]: Llama-2-70B-shaped, 1 -> 8 B200; SURVEY 8e: no collective).
+"""Quantise-only run, layers sharded across ranks (BASELINE configs[3]: Llama-2-70B-shaped, 1 -> 8 GPUs; SURVEY 8e: no collective).
 
     python tools/quantize_sharded.py [--model 70b|8b] [--blocks N]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 tools/quantize_sharded.py
