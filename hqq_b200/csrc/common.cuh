@@ -49,6 +49,43 @@ static inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 constexpr int kNumSMs = 132;  // H100 SXM
 
+// ---- host launch path ------------------------------------------------------------------------
+// Function attributes and SM counts belong to ONE device: the caches are indexed by the calling thread's current device, so
+// layers living on several GPUs of one process each get their own setup.
+constexpr int kMaxDevices = 64;
+int current_device();  // 0 when it cannot be queried or lies outside the caches
+int sm_count();        // of the current device, cached; kNumSMs when it cannot be queried
+bool pdl_enabled();    // HQQ_B200_PDL=0 (test hook) launches without the programmatic-dependency attribute
+
+// Opts KERNEL into `bytes` of dynamic shared memory on the current device (kept per device: the largest request so far).
+template <auto KERNEL>
+static int reserve_smem(int bytes) {
+  static int reserved[kMaxDevices] = {};
+  int& r = reserved[current_device()];
+  if (bytes > r) {
+    cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "hqq_b200_linear_fwd: cannot reserve %d bytes of shared memory: %s", bytes, cudaGetErrorString(e));
+    r = bytes;
+  }
+  return HQQ_OK;
+}
+
+// Launches with programmatic dependent launch (the kernel's prologue may overlap the tail of the previous kernel on the
+// stream; the kernel calls pdl_wait() before it reads what that kernel wrote) and counts the launch.
+template <typename K, typename... Args>
+static int launch_pdl(const char* name, K kernel, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, args...);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "%s: CUDA launch failed: %s", name, cudaGetErrorString(e));
+  return HQQ_OK;
+}
+
 static inline int fields_of(int nbits) { return nbits == 3 ? 10 : 8 / nbits; }
 static inline bool valid_nbits(int nbits) { return nbits == 8 || nbits == 4 || nbits == 3 || nbits == 2 || nbits == 1; }
 static inline size_t dtype_size(int dt) {
@@ -94,6 +131,29 @@ template <typename T, int N>
 struct alignas(sizeof(T) * N >= 16 ? 16 : sizeof(T) * N) Vec {
   T v[N];
 };
+
+// ---- device primitives ----------------------------------------------------------------------
+// Programmatic dependent launch.  Under the CPU emulator (tests/emu) kernels run one after another: nothing to wait for.
+#ifdef HQQ_EMU
+__device__ __forceinline__ void pdl_wait() {}
+__device__ __forceinline__ void pdl_launch_dependents() {}
+#else
+// blocks until the grids this one depends on have completed and their writes are visible
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+// lets the next kernel on the stream launch; it still waits for this grid in its own pdl_wait()
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+#endif
+
+// byte permute (prmt.b32, default mode): result byte i is byte ((s >> 4i) & 7) of the eight bytes {b, a}, a being bytes 0-3
+__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t s) {
+#ifdef HQQ_EMU
+  return ::emu::prmt(a, b, s);
+#else
+  uint32_t r;
+  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(s));
+  return r;
+#endif
+}
 
 // streaming 16-byte global load that does not pollute L1 (weights are read exactly once)
 __device__ __forceinline__ uint4 ldg_stream_v4(const void* p) {

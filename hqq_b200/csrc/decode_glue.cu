@@ -11,15 +11,11 @@
 namespace hqq {
 
 #ifdef HQQ_EMU
-// CPU emulation (tests/emu): kernels and blocks run one after another, so the dependency instructions, the L2 prefetch and the
-// system-scope accesses are plain code; the cluster argmax (DSMEM) is not emulated
-__device__ __forceinline__ void pdl_wait_g() {}
-__device__ __forceinline__ void pdl_launch_g() {}
+// CPU emulation (tests/emu): kernels and blocks run one after another, so the L2 prefetch and the system-scope accesses are
+// plain code; the cluster argmax (DSMEM) is not emulated
 __device__ __forceinline__ uint32_t ld_sys_u32(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
 __device__ __forceinline__ void prefetch_l2(const void*) {}
 #else
-__device__ __forceinline__ void pdl_wait_g() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_g() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ uint32_t ld_sys_u32(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -55,8 +51,8 @@ __global__ void __launch_bounds__(1024) add_rmsnorm_kernel(T* __restrict__ h, co
     y += row;
     if (delta) delta += row;
   }
-  pdl_launch_g();
-  pdl_wait_g();
+  pdl_launch_dependents();
+  pdl_wait();
   float v[8];
   int n = 0;
   float ss = 0.f;
@@ -82,8 +78,8 @@ template <typename T>
 __global__ void __launch_bounds__(1024) add_rmsnorm_tp_kernel(T* __restrict__ h, const uint32_t* red_data, int* step_ctr, int x_index, int x_per_step,
                                                               int tp, const T* __restrict__ w, T* __restrict__ y, int H, float eps) {
   __shared__ float red[32];
-  pdl_launch_g();
-  pdl_wait_g();
+  pdl_launch_dependents();
+  pdl_wait();
   const int step = *reinterpret_cast<volatile int*>(step_ctr);
   const uint32_t ex = (uint32_t)step * (uint32_t)x_per_step + (uint32_t)x_index;
   const uint32_t tag = ex & 0xFFFFu;
@@ -114,8 +110,8 @@ __global__ void __launch_bounds__(1024) add_rmsnorm_tp_kernel(T* __restrict__ h,
 // y = silu(g) * u
 template <typename T>
 __global__ void __launch_bounds__(256) silu_mul_kernel(const T* __restrict__ g, const T* __restrict__ u, T* __restrict__ y, int n) {
-  pdl_launch_g();
-  pdl_wait_g();
+  pdl_launch_dependents();
+  pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
     const float a = to_f32<T>(g[i]);
@@ -150,7 +146,7 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
     k_cache += b * n_kv * L * hd; v_cache += b * n_kv * L * hd;
   }
   const int pos = (int)pos_p[0];
-  pdl_launch_g();
+  pdl_launch_dependents();
   {
     // one 128-byte line per prefetch; pos rows of hd * sizeof(T) bytes each in both caches
     const char* kb = reinterpret_cast<const char*>(k_cache + (long long)kvh * L * hd);
@@ -161,7 +157,7 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
       prefetch_l2(vb + ((long long)i << 7));
     }
   }
-  pdl_wait_g();
+  pdl_wait();
   const int half = hd / 2;
   // rope: x*cos + rotate_half(x)*sin, computed in T like the framework ops
   if (d < hd) {
@@ -284,8 +280,8 @@ __global__ void __cluster_dims__(kArgmaxCtas, 1, 1) __launch_bounds__(1024) argm
   __shared__ unsigned long long xkey;
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
-  pdl_launch_g();
-  pdl_wait_g();
+  pdl_launch_dependents();
+  pdl_wait();
   float best = -INFINITY;
   int idx = 0;
   for (int i = (rank * 1024 + (int)threadIdx.x) * 8; i < n; i += kArgmaxCtas * 1024 * 8) {
@@ -353,20 +349,6 @@ __global__ void __cluster_dims__(kArgmaxCtas, 1, 1) __launch_bounds__(1024) argm
 }
 
 #endif  // !HQQ_EMU
-
-template <typename K, typename... Args>
-static int launch_pdl(const char* name, K kernel, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, args...);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "%s: CUDA launch failed: %s", name, cudaGetErrorString(e));
-  return HQQ_OK;
-}
 
 }  // namespace hqq
 

@@ -87,15 +87,6 @@ __host__ __device__ __forceinline__ Item decode_item(const Args& a, int j) {
   return it;
 }
 
-// programmatic dependent launch: the split-K second pass is a dependent of the GEMM grid
-#ifdef HQQ_EMU
-__device__ __forceinline__ void pdl_wait_primary() {}
-__device__ __forceinline__ void pdl_release_dependents() {}
-#else
-__device__ __forceinline__ void pdl_wait_primary() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_release_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-#endif
-
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------
 #ifdef HQQ_EMU
 // CPU emulation (tests/emu): the same entry points, backed by a functional model of mbarrier / TMA / wgmma
@@ -223,17 +214,6 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
 }
 
 // ---- level -> T with the reference's roundings -------------------------------------------------------------------
-// Two k-adjacent levels (bytes b0, b1 already masked to the field) -> T2 {fl(fl(q0 - z) * s), fl(fl(q1 - z) * s)}.
-__device__ __forceinline__ uint32_t prmt_b32(uint32_t a, uint32_t b, uint32_t sel) {
-#ifdef HQQ_EMU
-  return ::emu::prmt(a, b, sel);
-#else
-  uint32_t r;
-  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(sel));
-  return r;
-#endif
-}
-
 // Four k-adjacent levels (one per byte of `t`, already masked to the field) -> two packed T2
 //   {fl(fl(q0 - z) * s), fl(fl(q1 - z) * s)}, {.. q2, q3 ..}
 template <typename T> struct Pair;
@@ -243,7 +223,7 @@ template <> struct Pair<__half> {
     // byte | 0x6400 == 1024 + q exactly (one PRMT per pair); subtracting 1024 is exact, so (q - z) and (.. * s) round
     // exactly like the reference's two steps
     const __half2 k1024 = __half2half2(__ushort_as_half((unsigned short)0x6400));
-    uint32_t a = prmt_b32(t, 0x64646464u, 0x4140u), b = prmt_b32(t, 0x64646464u, 0x4342u);
+    uint32_t a = prmt(t, 0x64646464u, 0x4140u), b = prmt(t, 0x64646464u, 0x4342u);
     __half2 ha = __hmul2(__hsub2(__hsub2(*reinterpret_cast<__half2*>(&a), k1024), z2), s2);
     __half2 hb = __hmul2(__hsub2(__hsub2(*reinterpret_cast<__half2*>(&b), k1024), z2), s2);
     lo = *reinterpret_cast<uint32_t*>(&ha);
@@ -318,7 +298,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
   // waits before its first load, and nothing is written (y, split-K partials) before an accumulator fed by those loads is full.
   // Packed weights, scale, zero and bias are never produced by a kernel that releases its dependents early.
   if (threadIdx.x == 0) {
-    pdl_release_dependents();
+    pdl_launch_dependents();
     HQQ_PREFETCH_TENSORMAP(&xmap_full);
     HQQ_PREFETCH_TENSORMAP(&xmap_half);
     if constexpr (DENSE) HQQ_PREFETCH_TENSORMAP(&amap);
@@ -340,7 +320,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
     // ================= dense mode: TMA producer for both operands =================
     if (threadIdx.x == 0) {
       uint32_t it = 0;  // k-blocks issued so far (ring position)
-      pdl_wait_primary();
+      pdl_wait();
       for (int j = blockIdx.x; j < n_items; j += gridDim.x) {
         const Item im = decode_item(a, j);
         if (!im.valid) continue;
@@ -472,7 +452,7 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
     // K % 256 == 0 (checked by the router) and k-slices are whole quads: every item starts at ring stage 0
     int j = next_valid((int)blockIdx.x);
     if (j < n_items) { tile_ptrs(decode_item(a, j)); load_quad(); }
-    if (td == 0) pdl_wait_primary();  // x may still be written by the predecessor; the weights are not
+    if (td == 0) pdl_wait();  // x may still be written by the predecessor; the weights are not
     uint32_t gq = 0;  // quads done so far (ring parity)
     while (j < n_items) {
       const int jn = next_valid(j + (int)gridDim.x);
@@ -545,7 +525,7 @@ template <typename T, int V>
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ ws, T* __restrict__ y, const T* __restrict__ bias, int M, int N,
                                                             int step, int PR, int S, int n_row, int n_tok) {
   const long long idx = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * V;
-  pdl_wait_primary();  // launched as a programmatic dependent of the GEMM: resident early, reads only after that grid has completed
+  pdl_wait();  // launched as a programmatic dependent of the GEMM: resident early, reads only after that grid has completed
   if (idx >= (long long)M * N) return;
   const int m = (int)(idx / N), n = (int)(idx % N);
   const int f = n / step, prg = n % step;
@@ -617,12 +597,6 @@ static int encode_map(CUtensorMap* xmap, const void* x, int64_t rows, int64_t K,
   return HQQ_OK;
 }
 
-static int sm_count() {
-  int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kNumSMs;
-  return n;
-}
-
 // see `Sched`: full tiles first, the last partial round as half tiles when that shortens it
 // HQQ_B200_GEMM_CTAS=<n> (test hook): the number of persistent CTAs the schedule is built for instead of the SM count, so that
 // small problems exercise tile-after-tile execution, both accumulators, the half-tile round and split-K (the emulator tests and
@@ -630,12 +604,6 @@ static int sm_count() {
 static int persistent_ctas() {
   HQQ_ENV_KNOB(cta_cap, ([] { const char* e = getenv("HQQ_B200_GEMM_CTAS"); return e ? atoi(e) : 0; })());
   return cta_cap > 0 ? cta_cap : sm_count();
-}
-
-// HQQ_B200_PDL=0 (test hook, shared with the small-M kernels): launch without the programmatic-dependency attribute
-static bool pdl_on() {
-  HQQ_ENV_KNOB(on, ([] { const char* e = getenv("HQQ_B200_PDL"); return (e && e[0] == '0') ? 0 : 1; })());
-  return on == 1;
 }
 
 // HQQ_B200_GEMM_KSPLIT=<n> (test / measurement hook): the largest number of k-slices the schedule may use (1 = never split)
@@ -699,49 +667,19 @@ static int launch(const void* x, Args& a, cudaStream_t st, const void* dense_W =
     a.ws = reinterpret_cast<float*>(ws);
   }
   const int grid = a.sched.n_items < P ? a.sched.n_items : P;
-  auto k = linear_gemm_kernel<T, NBITS, GS>;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  static bool attr_set[64] = {};  // per device: the attribute belongs to the function on ONE device
-  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem::BYTES);
-    HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "hqq_b200_linear_fwd: cannot reserve %d bytes of shared memory: %s", Smem::BYTES, cudaGetErrorString(e));
-    if (dev >= 0 && dev < 64) attr_set[dev] = true;
-  }
-  {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Smem::BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_on() ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, k, xmap_full, xmap_half, amap, a);
-  }
-  HQQ_LAUNCH_CHECK("hqq_b200_linear_fwd/wgmma");
-  if (a.sched.ksplit > 1) {
-    const long long total = (long long)a.M * a.N;
-    const bool vec = a.step % 4 == 0 && PR % 4 == 0 && aligned(a.y, 8);
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)cdiv(vec ? total / 4 : total, 256));
-    cfg.blockDim = dim3(256);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_on() ? 1 : 0;
-    T* yt = reinterpret_cast<T*>(a.y);
-    const T* bt = reinterpret_cast<const T*>(a.bias);
-    const float* wsc = a.ws;
-    if (vec) cudaLaunchKernelEx(&cfg, splitk_reduce_kernel<T, 4>, wsc, yt, bt, a.M, a.N, a.step, (int)PR, a.sched.ksplit, a.sched.n_row, a.sched.n_tok);
-    else cudaLaunchKernelEx(&cfg, splitk_reduce_kernel<T, 1>, wsc, yt, bt, a.M, a.N, a.step, (int)PR, a.sched.ksplit, a.sched.n_row, a.sched.n_tok);
-    HQQ_LAUNCH_CHECK("hqq_b200_linear_fwd/splitk-reduce");
-  }
-  return HQQ_OK;
+  rc = reserve_smem<linear_gemm_kernel<T, NBITS, GS>>(Smem::BYTES);
+  if (rc) return rc;
+  rc = launch_pdl("hqq_b200_linear_fwd/wgmma", linear_gemm_kernel<T, NBITS, GS>, dim3((unsigned)grid), dim3(kThreads), Smem::BYTES, st, xmap_full,
+                  xmap_half, amap, a);
+  if (rc || a.sched.ksplit <= 1) return rc;
+  const long long total = (long long)a.M * a.N;
+  const bool vec = a.step % 4 == 0 && PR % 4 == 0 && aligned(a.y, 8);
+  const dim3 rgrid((unsigned)cdiv(vec ? total / 4 : total, 256));
+  T* yt = reinterpret_cast<T*>(a.y);
+  const T* bt = reinterpret_cast<const T*>(a.bias);
+  const float* wsc = a.ws;
+  return launch_pdl("hqq_b200_linear_fwd/splitk-reduce", vec ? splitk_reduce_kernel<T, 4> : splitk_reduce_kernel<T, 1>, rgrid, dim3(256), 0, st, wsc,
+                    yt, bt, a.M, a.N, a.step, (int)PR, a.sched.ksplit, a.sched.n_row, a.sched.n_tok);
 }
 
 template <typename T, int NBITS>

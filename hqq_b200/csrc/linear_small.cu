@@ -16,10 +16,9 @@
 //
 // Scheduling: persistent CTAs walk the 16-row tiles of up to four weight matrices that share the activation (q/k/v,
 // gate/up) round-robin; the 8 warps of a CTA split K of a tile and stream their chunks through private cp.async rings
-// in shared memory (3 x 2 KB in flight per warp, prefetching across tile boundaries), then reduce through shared
-// memory in a fixed order: deterministic, no atomics, no workspace.  Launched with programmatic dependent launch: the
-// weight prefetch starts before the producer of x has finished.
-#include <stdlib.h>
+// in shared memory (per warp ST stages of one 256-k unit, 2 KB, or 4 KB at 8 bits; ST - 1 of them in flight, prefetching
+// across tile boundaries), then reduce through shared memory in a fixed order: deterministic, no atomics, no workspace.
+// Launched with programmatic dependent launch: the weight prefetch starts before the producer of x has finished.
 #include <string.h>
 #include <type_traits>
 
@@ -147,15 +146,6 @@ template <> struct MT16<__nv_bfloat16> {
   __device__ __forceinline__ static void st(void* p, long long i, float v, const void* bias, int n) { reinterpret_cast<__nv_bfloat16*>(p)[i] = cvt(v, bias, n); }
 };
 
-__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t s) {
-#ifdef HQQ_EMU
-  return ::emu::prmt(a, b, s);
-#else
-  uint32_t r;
-  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(s));
-  return r;
-#endif
-}
 template <int LUT>
 __device__ __forceinline__ uint32_t lop3(uint32_t a, uint32_t b, uint32_t c) {
 #ifdef HQQ_EMU
@@ -170,29 +160,21 @@ __device__ __forceinline__ uint32_t lop3(uint32_t a, uint32_t b, uint32_t c) {
 __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t b, uint32_t c) { return lop3<0xEA>(a, b, c); }
 
 // How the integer levels are planted into 16-bit float lanes (lane value = OFF + q * V):
-//   MAGIC_OFFSET    fp16: bits | 0x6400 -> 1024 + q*2^sh          bf16: (bits >> sh) | 0x4300 -> 128 + q
-//   MAGIC_SUBNORMAL fp16 only: bits taken as a subnormal          -> q * 2^(sh-24)   (no offset, exact)
-enum { MAGIC_OFFSET = 0, MAGIC_SUBNORMAL = 1 };
-
-template <typename T, int NBITS, int MAGIC> struct Lanes;
+//   fp16: bits | 0x6400 -> 1024 + q*2^sh          bf16: (bits >> sh) | 0x4300 -> 128 + q
+template <typename T, int NBITS> struct Lanes;
 
 // fp16, sub-byte fields: mask in place, no shift (1 PRMT + 1 SHF + 4 LOP3 per 8 weights)
-template <int NBITS, int MAGIC>
-struct Lanes<__half, NBITS, MAGIC> {
-  static constexpr uint32_t OR = (MAGIC == MAGIC_OFFSET) ? 0x64006400u : 0u;
+template <int NBITS>
+struct Lanes<__half, NBITS> {
+  static constexpr uint32_t OR = 0x64006400u;
   uint32_t mask_a, mask_b;
   float invV_a, invV_b, offV_a, offV_b;
   __device__ __forceinline__ void init(int sh_a, int sh_b) {
     const uint32_t m = (1u << NBITS) - 1u;
     mask_a = (m << sh_a) * 0x00010001u;
     mask_b = (m << sh_b) * 0x00010001u;
-    if (MAGIC == MAGIC_OFFSET) {
-      invV_a = exp2f(-(float)sh_a); invV_b = exp2f(-(float)sh_b);
-      offV_a = 1024.0f * invV_a;    offV_b = 1024.0f * invV_b;
-    } else {
-      invV_a = exp2f(24.0f - (float)sh_a); invV_b = exp2f(24.0f - (float)sh_b);
-      offV_a = 0.0f; offV_b = 0.0f;
-    }
+    invV_a = exp2f(-(float)sh_a); invV_b = exp2f(-(float)sh_b);
+    offV_a = 1024.0f * invV_a;    offV_b = 1024.0f * invV_b;
   }
   // w: 4 consecutive k-bytes of one packed row.  a0/a2: field A for k{0,1} / k{2,3}; a1/a3: field B.
   __device__ __forceinline__ void extract(uint32_t w, uint32_t& a0, uint32_t& a1, uint32_t& a2, uint32_t& a3) const {
@@ -214,8 +196,8 @@ struct Lanes<__half, NBITS, MAGIC> {
 };
 
 // bf16, sub-byte fields: only 7 mantissa bits -> shift the field down to bit 0 first
-template <int NBITS, int MAGIC>
-struct Lanes<__nv_bfloat16, NBITS, MAGIC> {
+template <int NBITS>
+struct Lanes<__nv_bfloat16, NBITS> {
   int sh_a, sh_b;
   float invV_a, invV_b, offV_a, offV_b;
   __device__ __forceinline__ void init(int sa, int sb) {
@@ -241,14 +223,11 @@ struct Lanes<__nv_bfloat16, NBITS, MAGIC> {
 };
 
 // fp16, 8-bit: whole bytes, two packed rows per thread (rows r and r+8 of the tile)
-template <int MAGIC>
-struct Lanes<__half, 8, MAGIC> {
-  static constexpr uint32_t HB = (MAGIC == MAGIC_OFFSET) ? 0x64646464u : 0u;
+template <>
+struct Lanes<__half, 8> {
+  static constexpr uint32_t HB = 0x64646464u;
   float invV_a, invV_b, offV_a, offV_b;
-  __device__ __forceinline__ void init(int, int) {
-    if (MAGIC == MAGIC_OFFSET) { invV_a = invV_b = 1.0f; offV_a = offV_b = 1024.0f; }
-    else { invV_a = invV_b = 16777216.0f; offV_a = offV_b = 0.0f; }
-  }
+  __device__ __forceinline__ void init(int, int) { invV_a = invV_b = 1.0f; offV_a = offV_b = 1024.0f; }
   __device__ __forceinline__ void extract2(uint32_t wa, uint32_t wb, uint32_t& a0, uint32_t& a1, uint32_t& a2, uint32_t& a3) const {
     a0 = prmt(wa, HB, 0x4140u);  // lanes {k0, k1} of row r
     a2 = prmt(wa, HB, 0x4342u);  // lanes {k2, k3}
@@ -271,20 +250,9 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* g) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(g) : "memory");
 #endif
 }
-template <int BYTES>
-__device__ __forceinline__ void cp_async_small(void* smem, const void* g) {
-#ifdef HQQ_EMU
-  ::emu::cp_async(smem, g, BYTES);
-#else
-  const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(s), "l"(g), "n"(BYTES) : "memory");
-#endif
-}
 #ifdef HQQ_EMU
 __device__ __forceinline__ void cp_async_commit() { ::emu::cp_async_commit(); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { ::emu::cp_async_wait(N); }
-__device__ __forceinline__ void pdl_wait() {}
-__device__ __forceinline__ void pdl_launch_dependents() {}
 #else
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
@@ -295,41 +263,17 @@ template <typename T> __device__ __forceinline__ T from_f32_t(float v);
 template <> __device__ __forceinline__ __half from_f32_t<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_f32_t<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
-__device__ __forceinline__ int ld_acquire_sys(const int* p) {
-#ifdef HQQ_EMU
-  return *reinterpret_cast<const volatile int*>(p);
-#else
-  int v;
-  asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-#endif
-}
-__device__ __forceinline__ void st_release_sys(int* p, int v) {
-#ifdef HQQ_EMU
-  *reinterpret_cast<volatile int*>(p) = v;
-#else
-  asm volatile("st.release.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-#endif
-}
-
-#ifndef HQQ_EMU
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-#endif
-
-template <typename T, int NBITS, int GS, int MT, int MAGIC>
+template <typename T, int NBITS, int GS, int MT>
 struct SKCfg {
   static constexpr int F = 8 / NBITS;            // fields (slabs) per byte
   static constexpr int P = 16 / F;               // packed rows per 16-row MMA tile
   static constexpr int MPG = GS / 16;            // MMAs per quantisation group
   static constexpr int GPB = 256 / GS;           // quantisation groups per 256-k unit
-  static constexpr int MB = GPB * 2;             // bytes of scale (or zero) per unit and row
   static constexpr int NWV = (F == 1) ? 8 : 4;   // 16-byte weight vectors per thread and unit
   static constexpr int ST = (F == 1) ? 2 : 4;    // ring stages
   static constexpr int W_BYTES = ST * NWV * 256 * 16;
-  static constexpr int M_BYTES = 0;                     // scale/zero travel through registers
   static constexpr int P_BYTES = 2 * 8 * MT * 128 * 4;  // double-buffered split-K partials, one 16x8 tile per warp
-  static constexpr int SMEM = W_BYTES + M_BYTES + P_BYTES;
+  static constexpr int SMEM = W_BYTES + P_BYTES;
   static constexpr int MIN_CTAS = (SMEM <= 110 * 1024 && MT <= 2) ? 2 : 1;
 };
 
@@ -338,20 +282,20 @@ struct SKCfg {
 // per-thread cp.async rings (the ring keeps prefetching across tile boundaries, so HBM requests never drain).  Partials
 // meet in shared memory once per tile (one block barrier, double-buffered) and warp (tile % 8) adds them in warp order:
 // deterministic, no atomics, no global workspace.
-template <typename T, int NBITS, int GS, int MT, int MAGIC>
-__global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT, MAGIC>::MIN_CTAS) linear_small_kernel(const __grid_constant__ SKArgs a) {
-  using C = SKCfg<T, NBITS, GS, MT, MAGIC>;
+template <typename T, int NBITS, int GS, int MT>
+__global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT>::MIN_CTAS) linear_small_kernel(const __grid_constant__ SKArgs a) {
+  using C = SKCfg<T, NBITS, GS, MT>;
   constexpr int F = C::F, P = C::P, MPG = C::MPG, GPB = C::GPB, NWV = C::NWV, ST = C::ST;
   using MM = MT16<T>;
   extern __shared__ __align__(16) uint8_t smem[];
-  uint4* wring = reinterpret_cast<uint4*>(smem);                             // [ST][NWV][256] one 16-byte slot per thread
-  float* part_s = reinterpret_cast<float*>(smem + C::W_BYTES + C::M_BYTES);  // [2][8][MT][128]
+  uint4* wring = reinterpret_cast<uint4*>(smem);                  // [ST][NWV][256] one 16-byte slot per thread
+  float* part_s = reinterpret_cast<float*>(smem + C::W_BYTES);  // [2][8][MT][128]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int r = lane >> 2, c = lane & 3;
   const int p = (F == 1) ? r : (r % P);
   const int fa = (F == 1) ? 0 : (r / P), fb = (F == 1) ? 0 : (F / 2 + r / P);
-  Lanes<T, NBITS, MAGIC> lanes;
+  Lanes<T, NBITS> lanes;
   lanes.init(8 - NBITS * (fa + 1), 8 - NBITS * (fb + 1));
 
   // this warp's k-chunk of every tile (the same for all tiles: all matrices share K)
@@ -377,14 +321,18 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT, MAGIC>::MIN_CTAS)
     t.Wq = Wq; t.scale = reinterpret_cast<const T*>(sc); t.zero = reinterpret_cast<const T*>(ze);
     t.bias = reinterpret_cast<const T*>(bi); t.y = reinterpret_cast<T*>(y); t.N = N; t.step = step; t.tile0 = tile0;
   };
+  auto rows = [&](int gt, Tile& t, int& prow_a, int& prow_b) {
+    locate(gt, t);
+    prow_a = (gt - t.tile0) * P + p;
+    prow_b = (F == 1) ? prow_a + 8 : prow_a;
+  };
 
   // ---- issue cursor -------------------------------------------------------------------------------------------
   int i_tile = 0, i_k = 0;  // index into this CTA's tile list / unit within the warp's chunk
   const uint8_t *iw_a, *iw_b;
   auto issue_setup = [&]() {
-    Tile t; locate((int)blockIdx.x + i_tile * (int)gridDim.x, t);
-    const int gt = (int)blockIdx.x + i_tile * (int)gridDim.x;
-    const int prow_a = (gt - t.tile0) * P + p, prow_b = (F == 1) ? prow_a + 8 : prow_a;
+    Tile t; int prow_a, prow_b;
+    rows((int)blockIdx.x + i_tile * (int)gridDim.x, t, prow_a, prow_b);
     // rows past the ragged edge re-read row 0 (always mapped); their results are never stored
     const long long ra = prow_a < t.step ? prow_a : 0, rb = prow_b < t.step ? prow_b : 0;
     iw_a = t.Wq + ra * a.K + (long long)kb0 * 256 + 16 * c;
@@ -392,15 +340,14 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT, MAGIC>::MIN_CTAS)
   };
   int to_issue = n_tiles * upt;
   if (to_issue > 0) issue_setup();
-  // ---- meta cursor: scale/zero of the NEXT unit travel through registers (plain cached loads, one unit ahead).  They
-  // used to ride the cp.async ring, but 8-byte cp.async costs one shared-memory wavefront per lane (ncu: 60 % of all
-  // shared wavefronts of the kernel).
+  // ---- meta cursor: scale/zero of the NEXT unit travel through registers (plain cached loads, one unit ahead; an 8-byte
+  // cp.async per lane would cost one shared-memory wavefront each)
   int m_tile = 0, m_k = 0, m_left = n_tiles * upt;
   const T *ms_a = nullptr, *mz_a = nullptr, *ms_b = nullptr, *mz_b = nullptr;
   auto meta_setup = [&]() {
     const int gt = (int)blockIdx.x + m_tile * (int)gridDim.x;
-    Tile t; locate(gt, t);
-    const int prow_a = (gt - t.tile0) * P + p, prow_b = (F == 1) ? prow_a + 8 : prow_a;
+    Tile t; int prow_a, prow_b;
+    rows(gt, t, prow_a, prow_b);
     const long long na = prow_a < t.step ? fa * t.step + prow_a : 0, nb = prow_b < t.step ? fb * t.step + prow_b : 0;
     ms_a = t.scale + na * a.Gk + kb0 * GPB; mz_a = t.zero + na * a.Gk + kb0 * GPB;
     ms_b = t.scale + nb * a.Gk + kb0 * GPB; mz_b = t.zero + nb * a.Gk + kb0 * GPB;
@@ -542,9 +489,8 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT, MAGIC>::MIN_CTAS)
       *reinterpret_cast<float4*>(buf + (warp * MT + mt) * 128 + lane * 4) = make_float4(tot[mt][0], tot[mt][1], tot[mt][2], tot[mt][3]);
     __syncthreads();
     if (warp == (ti & 7)) {
-      const int gt = (int)blockIdx.x + ti * (int)gridDim.x;
-      Tile t; locate(gt, t);
-      const int prow_a = (gt - t.tile0) * P + p, prow_b = (F == 1) ? prow_a + 8 : prow_a;
+      Tile t; int prow_a, prow_b;
+      rows((int)blockIdx.x + ti * (int)gridDim.x, t, prow_a, prow_b);
       const bool ok_a = prow_a < t.step, ok_b = prow_b < t.step;
       const int n_a = fa * t.step + prow_a, n_b = fb * t.step + prow_b;
 #pragma unroll
@@ -575,12 +521,14 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT, MAGIC>::MIN_CTAS)
 // depends only on the activation is hoisted out of the per-tile loop: each warp stages ITS k-chunk of x once in shared
 // memory, already permuted to the lane pairing the bit-tricks produce ({k0,k2},{k1,k3}: no PRMT on the weights), and
 // sums it per quantisation group once (no all-ones MMA); the affine correction is applied to the single real column.
-// MR = 1 (experimental, HQQ_B200_D1_VARIANT=1042): scale/zero ride the cp.async ring at the same distance as the weights
-// (16-byte copies of the aligned block that holds this unit's 8 bytes) instead of register loads one unit ahead -- ncu showed
-// 18 % of all stall samples on the first use of those registers (DRAM latency under load exceeds one unit of work).
-template <typename T, int NBITS, int GS, int MAGIC, int ST, int MR = 0>
+// Scale/zero travel one of two ways, chosen by the host (sk_mt); the outputs are bit-identical:
+//   MR = 1  they ride the cp.async ring at the same distance as the weights, as 16-byte copies of the aligned block that holds
+//           this unit's bytes -- when K % 512 == 0 and every scale/zero row starts on 16 bytes.  Their DRAM latency then stays
+//           off the critical path, where one unit of work does not always hide it.
+//   MR = 0  register loads one unit ahead (the meta cursor below), otherwise.
+template <typename T, int NBITS, int GS, int ST, int MR = 0>
 struct D1Cfg {
-  static constexpr int F = 8 / NBITS, P = 16 / F, MPG = GS / 16, GPB = 256 / GS, MB = GPB * 2;
+  static constexpr int F = 8 / NBITS, P = 16 / F, MPG = GS / 16, GPB = 256 / GS;
   static constexpr int NWV = (F == 1) ? 8 : 4;
   static constexpr int W_BYTES = ST * NWV * 256 * 16;
   static constexpr int M_BYTES = (MR & 1) ? ST * 8 * 4 * 8 * 16 : 0;  // MR: [stage][warp][vector][row] 16-byte blocks; else registers
@@ -588,9 +536,9 @@ struct D1Cfg {
   static int smem(int K) { return W_BYTES + M_BYTES + P_BYTES + K * 2 + (K / GS) * 4; }
 };
 
-template <typename T, int NBITS, int GS, int MAGIC, int ST, int MC, int MR = 0>
+template <typename T, int NBITS, int GS, int ST, int MC, int MR = 0>
 __global__ void __launch_bounds__(256, MC) linear_decode1_kernel(const __grid_constant__ SKArgs a) {
-  using C = D1Cfg<T, NBITS, GS, MAGIC, ST, MR>;
+  using C = D1Cfg<T, NBITS, GS, ST, MR>;
   constexpr int F = C::F, P = C::P, MPG = C::MPG, GPB = C::GPB, NWV = C::NWV;
   using MM = MT16<T>;
   extern __shared__ __align__(16) uint8_t smem[];
@@ -604,7 +552,7 @@ __global__ void __launch_bounds__(256, MC) linear_decode1_kernel(const __grid_co
   const int r = lane >> 2, c = lane & 3;
   const int p = (F == 1) ? r : (r % P);
   const int fa = (F == 1) ? 0 : (r / P), fb = (F == 1) ? 0 : (F / 2 + r / P);
-  Lanes<T, NBITS, MAGIC> lanes;
+  Lanes<T, NBITS> lanes;
   lanes.init(8 - NBITS * (fa + 1), 8 - NBITS * (fb + 1));
 
   const int kb0 = a.KB * warp / 8, kb1 = a.KB * (warp + 1) / 8;
@@ -632,7 +580,7 @@ __global__ void __launch_bounds__(256, MC) linear_decode1_kernel(const __grid_co
   // paired epilogue (yop 1, F > 1): tile gt = packed rows [gt*PH, gt*PH + PH) of matrix 0 (fragment rows p < PH) and of matrix 1
   constexpr int PH = (P >= 2) ? P / 2 : 1;
   const bool paired = (F > 1) && a.yop == 1;
-  auto my_rows = [&](int gt, Tile& t, int& prow_a, int& prow_b) {
+  auto rows = [&](int gt, Tile& t, int& prow_a, int& prow_b) {
     if (paired) {
       pick(p >= PH ? 1 : 0, t);
       prow_a = prow_b = gt * PH + (p % PH);
@@ -647,9 +595,8 @@ __global__ void __launch_bounds__(256, MC) linear_decode1_kernel(const __grid_co
   const uint8_t *iw_a, *iw_b;
   const T* im = nullptr;  // MR: this lane's meta vector (c = 0: scale of row a, 1: zero of row a, 2: scale of row b, 3: zero of row b)
   auto issue_setup = [&]() {
-    const int gt = (int)blockIdx.x + i_tile * (int)gridDim.x;
     Tile t; int prow_a, prow_b;
-    my_rows(gt, t, prow_a, prow_b);
+    rows((int)blockIdx.x + i_tile * (int)gridDim.x, t, prow_a, prow_b);
     const long long ra = prow_a < t.step ? prow_a : 0, rb = prow_b < t.step ? prow_b : 0;
     iw_a = t.Wq + ra * a.K + (long long)kb0 * 256 + 16 * c;
     iw_b = t.Wq + rb * a.K + (long long)kb0 * 256 + 16 * c;
@@ -660,15 +607,13 @@ __global__ void __launch_bounds__(256, MC) linear_decode1_kernel(const __grid_co
   };
   int to_issue = n_tiles * upt;
   if (to_issue > 0) issue_setup();
-  // ---- meta cursor: scale/zero of the NEXT unit travel through registers (plain cached loads, one unit ahead).  They
-  // used to ride the cp.async ring, but 8-byte cp.async costs one shared-memory wavefront per lane (ncu: 60 % of all
-  // shared wavefronts of the kernel).
+  // ---- meta cursor (MR = 0): scale/zero of the NEXT unit travel through registers (plain cached loads, one unit ahead)
   int m_tile = 0, m_k = 0, m_left = (MR & 1) ? 0 : n_tiles * upt;
   const T *ms_a = nullptr, *mz_a = nullptr, *ms_b = nullptr, *mz_b = nullptr;
   auto meta_setup = [&]() {
     const int gt = (int)blockIdx.x + m_tile * (int)gridDim.x;
     Tile t; int prow_a, prow_b;
-    my_rows(gt, t, prow_a, prow_b);
+    rows(gt, t, prow_a, prow_b);
     const long long na = prow_a < t.step ? fa * t.step + prow_a : 0, nb = prow_b < t.step ? fb * t.step + prow_b : 0;
     ms_a = t.scale + na * a.Gk + kb0 * GPB; mz_a = t.zero + na * a.Gk + kb0 * GPB;
     ms_b = t.scale + nb * a.Gk + kb0 * GPB; mz_b = t.zero + nb * a.Gk + kb0 * GPB;
@@ -970,177 +915,78 @@ __global__ void __launch_bounds__(256, MC) linear_decode1_kernel(const __grid_co
 }
 
 // ---------------------------------------------------------------------------------------------------------
-static int magic_mode() {
-  HQQ_ENV_KNOB(mode, ([] { const char* e = getenv("HQQ_B200_GEMV_MAGIC"); return (e && !strcmp(e, "subnormal")) ? MAGIC_SUBNORMAL : MAGIC_OFFSET; })());
-  return mode;
-}
-
-// Function attributes (opt-in dynamic shared memory) and SM counts belong to ONE device: every cache below is indexed by the
-// calling thread's current device, so layers living on several GPUs of one process each get their own setup.
-constexpr int kMaxDevices = 64;
-static int cur_device() {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = 0;
-  return dev;
-}
-
-static int sm_count() {
-  static int n[kMaxDevices] = {};
-  const int dev = cur_device();
-  if (!n[dev]) {
-    if (cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n[dev] <= 0) n[dev] = kNumSMs;
-  }
-  return n[dev];
-}
-
-template <typename T, int NBITS, int GS, int MT, int MAGIC>
-static int grid_for_kernel(int* grid_out) {
-  using C = SKCfg<T, NBITS, GS, MT, MAGIC>;
-  static int grids[kMaxDevices] = {};
-  int& grid = grids[cur_device()];
-  if (!grid) {
-    auto k = linear_small_kernel<T, NBITS, GS, MT, MAGIC>;
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-    HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "hqq_b200_linear_fwd: cannot reserve %d bytes of shared memory: %s", C::SMEM, cudaGetErrorString(e));
-    int occ = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, 256, C::SMEM);
-    HQQ_REQUIRE(e == cudaSuccess && occ > 0, HQQ_E_CUDA, "hqq_b200_linear_fwd: occupancy query failed: %s", cudaGetErrorString(e));
-    if (occ > 2) occ = 2;
-    grid = sm_count() * occ;
-  }
-  *grid_out = grid;
-  return HQQ_OK;
-}
-
-// Persistent CTAs take tiles round-robin, so a grid that does not divide the tile count leaves most CTAs idle during the
-// last round (896 tiles on 296 CTAs = 3.03 -> 4 rounds, 76 %).  The kernel is bound by aggregate HBM bandwidth, not by
-// per-SM work, so it is better to launch fewer, equally loaded CTAs: pick g in [max_grid/2, max_grid] maximising
-// tiles / (ceil(tiles/g) * g); ties go to the larger grid.
-static int balanced_grid(int tiles, int max_grid) {
-  if (tiles <= max_grid) return tiles;
-  HQQ_ENV_KNOB(mode, ([] { const char* e = getenv("HQQ_B200_BALANCED_GRID"); return (e && e[0] == '1') ? 1 : 0; })());
-  if (!mode) return max_grid;  // the kernel is bound per SM, so filling every CTA slot wins
-  int best = max_grid;
-  double best_eff = 0.0;
-  for (int g = max_grid; g >= max_grid / 2; --g) {
-    const int rounds = (tiles + g - 1) / g;
-    const double eff = (double)tiles / ((double)rounds * g);
-    if (eff > best_eff + 1e-9) { best_eff = eff; best = g; }
-  }
-  return best;
-}
-
-static bool pdl_enabled() {
-  HQQ_ENV_KNOB(on, ([] { const char* e = getenv("HQQ_B200_PDL"); return (e && e[0] == '0') ? 0 : 1; })());
-  return on == 1;
-}
-
-template <typename T, int NBITS, int GS, int MT, int MAGIC>
+template <typename T, int NBITS, int GS, int MT>
 static int launch_sk(SKArgs& a, cudaStream_t st) {
-  using C = SKCfg<T, NBITS, GS, MT, MAGIC>;
-  int grid = 0;
-  int rc = grid_for_kernel<T, NBITS, GS, MT, MAGIC>(&grid);
+  using C = SKCfg<T, NBITS, GS, MT>;
+  int rc = reserve_smem<linear_small_kernel<T, NBITS, GS, MT>>(C::SMEM);
   if (rc) return rc;
-  grid = balanced_grid(a.total_tiles, grid);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(256);
-  cfg.dynamicSmemBytes = C::SMEM;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, linear_small_kernel<T, NBITS, GS, MT, MAGIC>, a);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "hqq_b200_linear_fwd/small: CUDA launch failed: %s", cudaGetErrorString(e));
-  return HQQ_OK;
+  static int per_sm[kMaxDevices] = {};  // resident CTAs per SM, at most 2
+  int& occ = per_sm[current_device()];
+  if (!occ) {
+    int n = 0;
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, linear_small_kernel<T, NBITS, GS, MT>, 256, C::SMEM);
+    HQQ_REQUIRE(e == cudaSuccess && n > 0, HQQ_E_CUDA, "hqq_b200_linear_fwd: occupancy query failed: %s", cudaGetErrorString(e));
+    occ = n > 2 ? 2 : n;
+  }
+  // one CTA per tile up to every resident slot: the kernel is bound per SM, so filling every slot wins over evening out rounds
+  const int max_grid = sm_count() * occ;
+  return launch_pdl("hqq_b200_linear_fwd/small", linear_small_kernel<T, NBITS, GS, MT>, dim3((unsigned)(a.total_tiles < max_grid ? a.total_tiles : max_grid)),
+                    dim3(256), C::SMEM, st, a);
 }
 
-template <typename T, int NBITS, int GS, int MAGIC, int ST, int MC, int MR = 0>
+template <typename T, int NBITS, int GS, int ST, int MC, int MR = 0>
 static int launch_d1(SKArgs& a, cudaStream_t st) {
-  using C = D1Cfg<T, NBITS, GS, MAGIC, ST, MR>;
-  static int max_smems[kMaxDevices] = {};
-  int& max_smem = max_smems[cur_device()];
-  const int smem = C::smem(a.K);
-  auto k = linear_decode1_kernel<T, NBITS, GS, MAGIC, ST, MC, MR>;
-  if (smem > max_smem) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "hqq_b200_linear_fwd: cannot reserve %d bytes of shared memory: %s", smem, cudaGetErrorString(e));
-    max_smem = smem;
-  }
+  const int smem = D1Cfg<T, NBITS, GS, ST, MR>::smem(a.K);
+  int rc = reserve_smem<linear_decode1_kernel<T, NBITS, GS, ST, MC, MR>>(smem);
+  if (rc) return rc;
   int per_sm = MC;
   while (per_sm > 1 && (smem + 1024) * per_sm > 227 * 1024) --per_sm;
-  int grid = balanced_grid(a.total_tiles, sm_count() * per_sm);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(256);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, k, a);
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  HQQ_REQUIRE(e == cudaSuccess, HQQ_E_CUDA, "hqq_b200_linear_fwd/decode1: CUDA launch failed: %s", cudaGetErrorString(e));
-  return HQQ_OK;
+  const int max_grid = sm_count() * per_sm;
+  return launch_pdl("hqq_b200_linear_fwd/decode1", linear_decode1_kernel<T, NBITS, GS, ST, MC, MR>,
+                    dim3((unsigned)(a.total_tiles < max_grid ? a.total_tiles : max_grid)), dim3(256), smem, st, a);
 }
 
-static bool d1_enabled() {
-  HQQ_ENV_KNOB(on, ([] { const char* e = getenv("HQQ_B200_DECODE1"); return (e && e[0] == '0') ? 0 : 1; })());
-  return on == 1;
-}
+bool small_xop_ok(int64_t M, int64_t K) { return M == 1 && K <= 16384; }  // the one-token kernel
 
-template <typename T, int NBITS, int GS, int MAGIC>
+template <typename T, int NBITS, int GS>
 static int sk_mt(SKArgs& a, cudaStream_t st) {
-  if (a.M == 1 && a.K <= 16384 && d1_enabled()) {
-    if (NBITS == 8) return launch_d1<T, NBITS, GS, MAGIC, 2, 2>(a, st);
-    // scale/zero ride the cp.async ring at the weights' distance (MR = 1) whenever the ring's aligned 16-byte copies are legal;
-    // that keeps them off the critical path, where register loads one unit ahead expose their latency; the outputs are
-    // bit-identical.  evict-first hints, a third CTA per SM, L2 prefetch under the dependency wait and
-    // cross-launch weight prefetch were measured in the same run, were not faster, and are gone.
-    if constexpr (GS == 64 && NBITS != 8) {
-      if (a.K % 512 == 0) {
-        bool ok = true;  // the ring copies aligned 16-byte blocks: every group row must start on one
-        for (int i = 0; i < a.nprob; ++i) ok = ok && aligned(a.p[i].scale, 16) && aligned(a.p[i].zero, 16);
-        if (ok) return launch_d1<T, NBITS, GS, MAGIC, 4, 2, 1>(a, st);
+  if (small_xop_ok(a.M, a.K)) {
+    if constexpr (NBITS == 8) {
+      return launch_d1<T, NBITS, GS, 2, 2>(a, st);
+    } else {
+      if constexpr (GS == 64) {  // MR = 1 when the ring's aligned 16-byte copies are legal (see D1Cfg)
+        if (a.K % 512 == 0) {
+          bool ok = true;  // every group row must start on a 16-byte boundary
+          for (int i = 0; i < a.nprob; ++i) ok = ok && aligned(a.p[i].scale, 16) && aligned(a.p[i].zero, 16);
+          if (ok) return launch_d1<T, NBITS, GS, 4, 2, 1>(a, st);
+        }
       }
+      return launch_d1<T, NBITS, GS, 4, 2>(a, st);
     }
-    return launch_d1<T, NBITS, GS, MAGIC, 4, 2>(a, st);
   }
-  if (a.M <= 8) return launch_sk<T, NBITS, GS, 1, MAGIC>(a, st);
-  if (a.M <= 16) return launch_sk<T, NBITS, GS, 2, MAGIC>(a, st);
-  return launch_sk<T, NBITS, GS, 4, MAGIC>(a, st);
+  if (a.M <= 8) return launch_sk<T, NBITS, GS, 1>(a, st);
+  if (a.M <= 16) return launch_sk<T, NBITS, GS, 2>(a, st);
+  return launch_sk<T, NBITS, GS, 4>(a, st);
 }
 
-template <typename T, int NBITS, int MAGIC>
+template <typename T, int NBITS>
 static int sk_gs(SKArgs& a, int gs, cudaStream_t st) {
   switch (gs) {
-    case 64: return sk_mt<T, NBITS, 64, MAGIC>(a, st);
-    case 128: return sk_mt<T, NBITS, 128, MAGIC>(a, st);
+    case 64: return sk_mt<T, NBITS, 64>(a, st);
+    case 128: return sk_mt<T, NBITS, 128>(a, st);
   }
   return HQQ_E_UNSUPPORTED;
 }
 
 template <typename T>
 static int sk_bits(SKArgs& a, int gs, int nbits, cudaStream_t st) {
-  const bool sub = std::is_same<T, __half>::value && magic_mode() == MAGIC_SUBNORMAL;
   switch (nbits) {
     case 8:
-      if constexpr (std::is_same<T, __half>::value) return sub ? sk_gs<T, 8, MAGIC_SUBNORMAL>(a, gs, st) : sk_gs<T, 8, MAGIC_OFFSET>(a, gs, st);
+      if constexpr (std::is_same<T, __half>::value) return sk_gs<T, 8>(a, gs, st);
       else return HQQ_E_UNSUPPORTED;
-    case 4:
-      if constexpr (std::is_same<T, __half>::value) return sub ? sk_gs<T, 4, MAGIC_SUBNORMAL>(a, gs, st) : sk_gs<T, 4, MAGIC_OFFSET>(a, gs, st);
-      else return sk_gs<T, 4, MAGIC_OFFSET>(a, gs, st);
-    case 2:
-      if constexpr (std::is_same<T, __half>::value) return sub ? sk_gs<T, 2, MAGIC_SUBNORMAL>(a, gs, st) : sk_gs<T, 2, MAGIC_OFFSET>(a, gs, st);
-      else return sk_gs<T, 2, MAGIC_OFFSET>(a, gs, st);
-    case 1:
-      if constexpr (std::is_same<T, __half>::value) return sub ? sk_gs<T, 1, MAGIC_SUBNORMAL>(a, gs, st) : sk_gs<T, 1, MAGIC_OFFSET>(a, gs, st);
-      else return sk_gs<T, 1, MAGIC_OFFSET>(a, gs, st);
+    case 4: return sk_gs<T, 4>(a, gs, st);
+    case 2: return sk_gs<T, 2>(a, gs, st);
+    case 1: return sk_gs<T, 1>(a, gs, st);
   }
   return HQQ_E_UNSUPPORTED;
 }
@@ -1159,8 +1005,6 @@ bool small_route_ok(int64_t M, int64_t N, int64_t K, int gs, int nbits, int axis
 }
 
 size_t small_workspace_bytes(int64_t) { return 0; }  // split-K partials meet in shared memory
-
-bool small_xop_ok(int64_t M, int64_t K) { return M == 1 && K <= 16384 && d1_enabled(); }
 
 int linear_small_multi(const void* x, int nprob, const void* const* Wq, const void* const* scale, const void* const* zero,
                        const void* const* bias, void* const* y, const int64_t* N, int64_t M, int64_t K, int gs, int nbits, int dtype,

@@ -256,9 +256,9 @@ int hqq_b200_glue_argmax_tp(const void* logits, int n, int64_t index_offset, voi
 int64_t hqq_b200_launch_count(void);
 void hqq_b200_launch_count_reset(void);
 
-/* The few HQQ_B200_* switches the library reads (test hooks: HQQ_B200_GEMM_CTAS, HQQ_B200_DECODE1, HQQ_B200_PDL,
- * HQQ_B200_PLAIN_SOLVER) are parsed once and cached; after changing one with setenv() call this to have the next launch parse
- * them again.  Not thread-safe against concurrent launches. */
+/* The few HQQ_B200_* switches the library reads (test / measurement hooks: HQQ_B200_GEMM_CTAS, HQQ_B200_GEMM_KSPLIT,
+ * HQQ_B200_SMALL_M_MAX, HQQ_B200_PDL, HQQ_B200_PLAIN_SOLVER) are parsed once and cached; after changing one with setenv() call
+ * this to have the next launch parse them again.  Not thread-safe against concurrent launches. */
 void hqq_b200_reload_env(void);
 
 #ifdef __cplusplus

@@ -366,16 +366,17 @@ def test_emulated_forward_random_shapes(emu, oracle):
     assert routes == {1, 2}
 
 
-def test_emulated_reload_env_switches_cached_knobs_in_one_process(emu):
-    """`hqq_b200_reload_env()`: a changed HQQ_B200_* switch is ignored until the reload and honoured after it."""
+def test_emulated_reload_env_rereads_gemm_ctas_in_one_process(emu):
+    """`hqq_b200_reload_env()`: a changed HQQ_B200_* switch (here HQQ_B200_GEMM_CTAS, seen through the split-K workspace size) is
+    ignored until the reload and honoured after it."""
     import json
     r = subprocess.run([sys.executable, os.path.join(HERE, "emu", "run_reload.py")], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-3000:]
     out = json.loads([ln for ln in r.stdout.splitlines() if ln.startswith("RELOAD ")][-1][7:])
-    assert out["default_rc"] == 0
-    assert out["cached_rc"] == 0 and out["cached_same"]          # no reload: the cached choice stands
-    assert out["reloaded_rc"] == -2                              # HQQ_E_UNSUPPORTED once HQQ_B200_DECODE1=0 is seen
-    assert out["restored_rc"] == 0 and out["restored_same"]
+    assert out["default_ws"] > 0                                 # 4 emulated SMs: the one output tile splits K
+    assert out["cached_ws"] == out["default_ws"]                 # no reload: the cached CTA count stands
+    assert out["reloaded_ws"] == 0                               # HQQ_B200_GEMM_CTAS=1 seen: one CTA, no split-K
+    assert out["restored_ws"] == out["default_ws"]
 
 
 @pytest.mark.parametrize("variant,cases", [(0, [(4, 0), (4, 1), (2, 0), (2, 1), (1, 0), (1, 1)]), (1, [(4, 1), (2, 0)])])
