@@ -5,6 +5,7 @@
 #ifndef HQQ_EMU
 #include <cooperative_groups.h>
 #endif
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -252,6 +253,318 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
   }
 }
 
+// Split-KV GQA attention for one decoded token at long context (DESIGN.md 3.5): RoPE + KV-cache append + attention over
+// cache[0..pos] with the cached positions split into S contiguous chunks, one CTA per (chunk, kv head, sequence).
+//
+// Each CTA handles all G = n_q / n_kv query heads of its group, so every K/V row crosses HBM once, not G times.  Both products
+// run on mma.sync m16n8k16 with the (at most 8) heads as the n = 8 dimension:
+//   scores^T [16 positions x 8 heads] = K tile [16 x 128] . Q^T       (K from shared memory through ldmatrix, Q^T in registers)
+//   O^T      [128 dims x 8 heads]    += V^T [128 x 16] . P^T           (V^T through ldmatrix.trans, P^T from the score fragments)
+// Each of the 8 warps streams the 16-position tiles w, w+8, ... of its CTA's chunk through a private 3-stage cp.async ring
+// (16 KB per warp: K then V, 16-byte chunks XOR-swizzled by row so ldmatrix is conflict-free) and keeps an online softmax in
+// fp32; P is rounded to T for the MMA and the row sum adds the rounded values.  The warps meet in shared memory in warp order,
+// the CTA publishes its partial (m, l, o[G][128]) to the workspace, and the last CTA of a (sequence, kv head) -- found with a
+// fence and a ticket -- combines the S partials in split order, writes out with one rounding to T and resets the ticket.
+//
+// S = max(1, min(SMs / n_kv, ceil(cache_len / 16))) is fixed at launch (graph replay advances *pos without re-capture); each CTA
+// derives its chunk from *pos: c = ceil((pos + 1) / S) rounded up to 16, split s covers [s c, min((s + 1) c, pos + 1)).
+namespace {
+
+constexpr int kSplitWarps = 8;
+constexpr int kSplitThreads = 32 * kSplitWarps;
+constexpr int kSplitStages = 3;
+constexpr int kSplitTile = 16;      // positions per tile: the m dimension of the score MMA
+constexpr int kSplitMaxGroup = 8;   // query heads per kv head: the n dimension of both MMAs
+constexpr int kSplitMaxLen = 131072;
+constexpr int kHd = 128;
+constexpr int kTileBytes = kSplitTile * kHd * 2;                          // one K or V tile, 4 KB
+constexpr int kStageBytes = 2 * kTileBytes;
+constexpr int kRingBytes = kSplitWarps * kSplitStages * kStageBytes;      // 192 KB
+constexpr int kSmemBytes = kRingBytes + (kSplitMaxGroup + 2) * kHd * 2 + 16;  // + rotated q [8][128], fresh k, v + the last-CTA flag
+constexpr int kPartFloats = kHd + 2;                                      // per head: m, l, o[128]
+static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kRingBytes, "the warp partials reuse the ring");
+
+template <typename T> __device__ __forceinline__ uint32_t bits16(T v) { return (uint32_t)*reinterpret_cast<const unsigned short*>(&v); }
+
+// byte offset of 16-byte chunk c of row r inside a [16][128] tile
+__device__ __forceinline__ int swz(int r, int c) { return r * 256 + ((c ^ (r & 7)) << 4); }
+
+__device__ __forceinline__ void split_cp16(void* smem, const void* g) {
+#ifdef HQQ_EMU
+  ::emu::cp_async(smem, g, 16);
+#else
+  const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(g) : "memory");
+#endif
+}
+#ifdef HQQ_EMU
+__device__ __forceinline__ void split_commit() { ::emu::cp_async_commit(); }
+template <int N> __device__ __forceinline__ void split_wait() { ::emu::cp_async_wait(N); }
+#else
+__device__ __forceinline__ void split_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void split_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+#endif
+
+// ldmatrix.x4 (TRANS: .trans): lane l supplies the row address p of row l % 8 of matrix l / 8 and receives r[j] of matrix j
+template <bool TRANS>
+__device__ __forceinline__ void ldsm4(uint32_t (&r)[4], const char* p) {
+#ifdef HQQ_EMU
+  const int l = threadIdx.x & 31;
+  for (int j = 0; j < 4; ++j) {
+    if (!TRANS) {
+      const char* src = __shfl_sync(0xffffffffu, p, j * 8 + (l >> 2));
+      r[j] = *reinterpret_cast<const uint32_t*>(src + 4 * (l & 3));
+    } else {  // element (row 2 (l % 4) + {0, 1}, column l / 4) of the stored matrix
+      const char* s0 = __shfl_sync(0xffffffffu, p, j * 8 + 2 * (l & 3));
+      const char* s1 = __shfl_sync(0xffffffffu, p, j * 8 + 2 * (l & 3) + 1);
+      r[j] = (uint32_t)*reinterpret_cast<const unsigned short*>(s0 + 2 * (l >> 2)) |
+             ((uint32_t)*reinterpret_cast<const unsigned short*>(s1 + 2 * (l >> 2)) << 16);
+    }
+  }
+#else
+  const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
+  if (TRANS)
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
+  else
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(a));
+#endif
+}
+
+// d += A[16x16] . B[16x8], fp32 accumulate
+template <typename T>
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+#ifdef HQQ_EMU
+  ::emu::mma_m16n8k16<T>(d, a[0], a[1], a[2], a[3], b0, b1, false);
+#else
+  if constexpr (std::is_same<T, __half>::value)
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+#endif
+}
+
+// grid = (S, n_kv, batch), block = 256.  q / out [batch, n_q * 128], k / v [batch, n_kv * 128], caches [batch, n_kv, L, 128].
+// part: [batch, n_kv, S, G, 2 + 128] floats (m, l, o per head), tickets: [batch, n_kv] uint32, zero between launches.
+template <typename T>
+__global__ void __launch_bounds__(kSplitThreads, 1)
+    rope_attn_decode_split_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
+                                  const T* __restrict__ sin_t, T* __restrict__ k_cache, T* __restrict__ v_cache, const long long* __restrict__ pos_p,
+                                  T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
+                                  float scale_log2) {
+  extern __shared__ __align__(16) char smem[];
+  constexpr int NW = kSplitWarps, ST = kSplitStages;
+  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
+  const int G = n_q / n_kv;
+  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  {
+    const long long kv = (long long)b * n_kv + kvh;
+    k_cache += kv * L * kHd; v_cache += kv * L * kHd;
+    k_in += kv * kHd; v_in += kv * kHd;
+    q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
+    part += kv * S * G * kPartFloats;
+    tickets += kv;
+  }
+  char* ring = smem + warp * ST * kStageBytes;
+  T* qs = reinterpret_cast<T*>(smem + kRingBytes);  // rotated q [8][128]
+  T* kf = qs + kSplitMaxGroup * kHd;                // rotated k and v of position pos
+  T* vf = kf + kHd;
+  int* last = reinterpret_cast<int*>(vf + kHd);
+
+  // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
+  const int pos = (int)pos_p[0], n_pos = pos + 1;
+  const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
+  const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
+  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
+  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;  // tiles warp, warp + NW, ... of the chunk
+  pdl_launch_dependents();
+
+  // Stage local tile i into its ring slot: rows < pos from the cache (cp.async), row pos from the rotated k / v of this step once
+  // `fresh` (the cache row is written by another CTA of this launch), rows past pos zero (finite: their probability is 0).
+  auto issue = [&](int i, bool fresh) {
+    if (i < my_tiles) {
+      const int t0 = c0 + (warp + i * NW) * kSplitTile;
+      char* st = ring + (i % ST) * kStageBytes;
+#pragma unroll 4
+      for (int j = lane; j < 2 * kSplitTile * 16; j += 32) {
+        const int isv = j >> 8, r = (j >> 4) & 15, c = j & 15, p = t0 + r;
+        char* dst = st + isv * kTileBytes + swz(r, c);
+        if (p < pos) {
+          split_cp16(dst, (isv ? v_cache : k_cache) + (long long)p * kHd + c * 8);
+        } else if (p > pos || fresh) {
+          uint4 val;
+          val.x = val.y = val.z = val.w = 0u;
+          if (p == pos) val = *reinterpret_cast<const uint4*>((isv ? vf : kf) + c * 8);
+          *reinterpret_cast<uint4*>(dst) = val;
+        }
+      }
+    }
+    split_commit();  // always (possibly empty): every iteration waits on the same group count
+  };
+  // cache rows < pos were written by earlier launches: the first ST - 1 tiles stream in under the previous kernel's tail
+#pragma unroll
+  for (int i = 0; i < ST - 1; ++i) issue(i, false);
+  pdl_wait();
+
+  // RoPE exactly as rope_attn_decode_kernel: x*cos + rotate_half(x)*sin, each product and the sum rounded to T
+  for (int i = tid; i < (G + 1) * kHd; i += kSplitThreads) {
+    const int h = i >> 7, d = i & (kHd - 1), half = kHd / 2;
+    const float c = to_f32<T>(cos_t[(long long)pos * kHd + d]), s = to_f32<T>(sin_t[(long long)pos * kHd + d]);
+    const T* x = h < G ? q_in + h * kHd : k_in;
+    const float xv = to_f32<T>(x[d]);
+    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
+    const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
+    if (h < G) {
+      qs[h * kHd + d] = r;
+    } else {
+      kf[d] = r;
+      vf[d] = v_in[d];
+      if (split == 0) {  // one writer per (sequence, kv head); no CTA of this launch reads cache row pos
+        k_cache[(long long)pos * kHd + d] = r;
+        v_cache[(long long)pos * kHd + d] = v_in[d];
+      }
+    }
+  }
+  __syncthreads();
+  if (pos >= c0 && pos < c1) {  // row pos in a tile staged before the wait: its owner fills it in now
+    const int ti = (pos - c0) / kSplitTile, i = ti / NW;
+    if (ti % NW == warp && i < ST - 1) {
+      const int r = pos - (c0 + ti * kSplitTile), c = lane & 15;
+      *reinterpret_cast<uint4*>(ring + (i % ST) * kStageBytes + (lane >> 4) * kTileBytes + swz(r, c)) =
+          *reinterpret_cast<const uint4*>((lane >> 4 ? vf : kf) + c * 8);
+    }
+  }
+  // Q^T fragments (B operand of the score MMA, n = head g): dims 16 kk + 2 qd + {0, 1} and + 8
+  uint32_t qb[8][2];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+    const T* qr = qs + g * kHd + kk * 16 + 2 * qd;
+    qb[kk][0] = g < G ? *reinterpret_cast<const uint32_t*>(qr) : 0u;
+    qb[kk][1] = g < G ? *reinterpret_cast<const uint32_t*>(qr + 8) : 0u;
+  }
+
+  // lane (g, qd) holds the running max / sum of heads 2 qd, 2 qd + 1 and O^T rows 16 mt + g (+ 8) of those heads
+  float o[8][4];
+#pragma unroll
+  for (int mt = 0; mt < 8; ++mt) o[mt][0] = o[mt][1] = o[mt][2] = o[mt][3] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  const int kr = (lane & 7) + ((lane >> 3) & 1) * 8, kc = lane >> 4;       // ldmatrix row / chunk, K (a0..a3: rows +8, then k +8)
+  const int vr = (lane & 7) + ((lane >> 4) & 1) * 8, vc = (lane >> 3) & 1;  // V^T (a0..a3: dims +8, then positions +8)
+  for (int i = 0; i < my_tiles; ++i) {
+    __syncwarp();  // every lane is done with the slot the next issue overwrites
+    issue(i + ST - 1, true);
+    split_wait<ST - 1>();
+    __syncwarp();  // this tile's copies and plain stores of every lane are visible to the warp
+    const char* kt = ring + (i % ST) * kStageBytes;
+    const char* vt = kt + kTileBytes;
+    float s[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t a[4];
+      ldsm4<false>(a, kt + swz(kr, 2 * kk + kc));
+      mma16816<T>(s, a, qb[kk][0], qb[kk][1]);
+    }
+    const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
+    const float x0 = p0 < c1 ? s[0] * scale_log2 : -INFINITY, x1 = p0 < c1 ? s[1] * scale_log2 : -INFINITY;
+    const float x2 = p0 + 8 < c1 ? s[2] * scale_log2 : -INFINITY, x3 = p0 + 8 < c1 ? s[3] * scale_log2 : -INFINITY;
+    float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
+#pragma unroll
+    for (int off = 4; off < 32; off <<= 1) {
+      t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
+      t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
+    }
+    const float n0 = fmaxf(m0, t0), n1 = fmaxf(m1, t1);  // finite: every tile holds position c0 + 16 j < c1
+    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
+    m0 = n0; m1 = n1;
+    const T p00 = from_f32<T>(exp2f(x0 - n0)), p01 = from_f32<T>(exp2f(x1 - n1));
+    const T p10 = from_f32<T>(exp2f(x2 - n0)), p11 = from_f32<T>(exp2f(x3 - n1));
+    l0 = l0 * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
+    l1 = l1 * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) { o[mt][0] *= a0; o[mt][1] *= a1; o[mt][2] *= a0; o[mt][3] *= a1; }
+    // P^T fragment (k = position, n = head g): positions 2 qd, 2 qd + 1 (+ 8) sit in lanes (2 qd, g / 2) and (2 qd + 1, g / 2)
+    const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
+    const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
+    const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
+    const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
+    const uint32_t b0 = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
+    const uint32_t b1 = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) {
+      uint32_t a[4];
+      ldsm4<true>(a, vt + swz(vr, 2 * mt + vc));
+      mma16816<T>(o[mt], a, b0, b1);
+    }
+  }
+  split_wait<0>();
+#pragma unroll
+  for (int off = 4; off < 32; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][8][m, l, o[128]]
+  float* wp = reinterpret_cast<float*>(smem);
+  {
+    float* w0 = wp + (warp * kSplitMaxGroup + 2 * qd) * kPartFloats;
+    float* w1 = w0 + kPartFloats;
+    if (g == 0) { w0[0] = m0; w0[1] = l0; w1[0] = m1; w1[1] = l1; }
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) {
+      w0[2 + 16 * mt + g] = o[mt][0]; w1[2 + 16 * mt + g] = o[mt][1];
+      w0[2 + 16 * mt + g + 8] = o[mt][2]; w1[2 + 16 * mt + g + 8] = o[mt][3];
+    }
+  }
+  __syncthreads();
+  // this CTA's partial, warps in order (an empty chunk publishes m = -inf, l = 0, o = 0)
+  for (int i = tid; i < G * kHd; i += kSplitThreads) {
+    const int h = i >> 7, d = i & (kHd - 1);
+    float M = -INFINITY;
+    for (int w = 0; w < NW; ++w) M = fmaxf(M, wp[(w * kSplitMaxGroup + h) * kPartFloats]);
+    float lsum = 0.f, osum = 0.f;
+    if (M != -INFINITY) {
+      for (int w = 0; w < NW; ++w) {
+        const float* e = wp + (w * kSplitMaxGroup + h) * kPartFloats;
+        const float f = exp2f(e[0] - M);
+        lsum += f * e[1];
+        osum += f * e[2 + d];
+      }
+    }
+    float* dst = part + ((long long)split * G + h) * kPartFloats;
+    if (d == 0) { dst[0] = M; dst[1] = lsum; }
+    dst[2 + d] = osum;
+  }
+  __threadfence();  // the partial is visible device-wide before the ticket counts it
+  __syncthreads();
+  if (tid == 0) *last = atomicAdd(tickets, 1u) == (unsigned)(S - 1);
+  __syncthreads();
+  if (!*last) return;
+  __threadfence();
+  // last CTA of the group: all S partials, split order, one rounding to T
+  for (int i = tid; i < G * kHd; i += kSplitThreads) {
+    const int h = i >> 7, d = i & (kHd - 1);
+    float M = -INFINITY;
+    for (int sp = 0; sp < S; ++sp) M = fmaxf(M, __ldcg(part + ((long long)sp * G + h) * kPartFloats));  // split 0 is never empty
+    float lsum = 0.f, osum = 0.f;
+    for (int sp = 0; sp < S; ++sp) {
+      const float* e = part + ((long long)sp * G + h) * kPartFloats;
+      const float f = exp2f(__ldcg(e) - M);
+      lsum += f * __ldcg(e + 1);
+      osum += f * __ldcg(e + 2 + d);
+    }
+    out[h * kHd + d] = from_f32<T>(osum / lsum);
+  }
+  if (tid == 0) *tickets = 0u;  // ready for the next launch (graph replay needs no memset)
+}
+
+int split_count(int n_kv, int cache_len) {
+  const int by_sm = sm_count() / n_kv;
+  const int by_len = (int)cdiv(cache_len, kSplitTile);
+  return max(1, min(by_sm, by_len));
+}
+
+}  // namespace
+
 #ifndef HQQ_EMU
 // argmax over n logits -> int64 index (first index on ties).  One thread-block cluster of 8 CTAs: each scans an
 // interleaved eighth of the row, the eight candidates meet in CTA 0's shared memory over DSMEM (no workspace, one launch).
@@ -422,6 +735,48 @@ extern "C" int hqq_b200_glue_rope_attn_decode(const void* q, const void* k, cons
                                               int cache_len, int head_dim, int dtype, void* stream) {
   return hqq_b200_glue_rope_attn_decode_batch(q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, n_q_heads, n_kv_heads, cache_len, head_dim, 1,
                                               dtype, stream);
+}
+
+extern "C" size_t hqq_b200_glue_rope_attn_decode_split_workspace_bytes(int n_q_heads, int n_kv_heads, int head_dim, int batch) {
+  if (n_kv_heads <= 0 || n_q_heads <= 0 || n_q_heads % n_kv_heads || head_dim <= 0 || batch <= 0) return 0;
+  const size_t s_max = (size_t)max(1, sm_count() / n_kv_heads);
+  const size_t groups = (size_t)batch * n_kv_heads;
+  return groups * s_max * (size_t)(n_q_heads / n_kv_heads) * (size_t)(head_dim + 2) * sizeof(float) + groups * sizeof(unsigned);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                    void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                    int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out && workspace, HQQ_E_INVALID,
+              "hqq_b200_glue_rope_attn_decode_split: null pointer");
+  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "hqq_b200_glue_rope_attn_decode_split: batch %d", batch);
+  HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0, HQQ_E_INVALID, "hqq_b200_glue_rope_attn_decode_split: workspace must be 4-byte aligned");
+  HQQ_REQUIRE(head_dim == kHd && n_kv_heads > 0 && n_kv_heads <= 65535 && n_q_heads % n_kv_heads == 0 && n_q_heads / n_kv_heads >= 1 &&
+                  n_q_heads / n_kv_heads <= kSplitMaxGroup && cache_len > 0 && cache_len <= kSplitMaxLen,
+              HQQ_E_UNSUPPORTED, "hqq_b200_glue_rope_attn_decode_split: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int S = split_count(n_kv_heads, cache_len);
+  const int G = n_q_heads / n_kv_heads;
+  const size_t part_bytes = (size_t)batch * n_kv_heads * max(1, sm_count() / n_kv_heads) * G * kPartFloats * sizeof(float);
+  float* part = (float*)workspace;
+  unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
+  const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
+  if (dtype == HQQ_F16) {
+    if (int rc = reserve_smem<rope_attn_decode_split_kernel<__half>>(kSmemBytes)) return rc;
+    return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<__half>, grid, dim3(kSplitThreads), kSmemBytes, st, (const __half*)q,
+                      (const __half*)k, (const __half*)v, (const __half*)cos_table, (const __half*)sin_table, (__half*)k_cache, (__half*)v_cache,
+                      (const long long*)pos, (__half*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2);
+  }
+  if (dtype == HQQ_BF16) {
+    if (int rc = reserve_smem<rope_attn_decode_split_kernel<__nv_bfloat16>>(kSmemBytes)) return rc;
+    return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<__nv_bfloat16>, grid, dim3(kSplitThreads), kSmemBytes, st,
+                      (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)cos_table,
+                      (const __nv_bfloat16*)sin_table, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, (const long long*)pos, (__nv_bfloat16*)out,
+                      part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2);
+  }
+  set_error("hqq_b200_glue_rope_attn_decode_split: dtype must be f16/bf16");
+  return HQQ_E_INVALID;
 }
 
 #ifndef HQQ_EMU

@@ -35,6 +35,8 @@ class LlamaShape:
     vocab: int = 128256
     rope_theta: float = 500000.0
     rms_eps: float = 1e-5
+    # None: plain RoPE frequencies.  {"rope_type": "llama3", ...}: the Llama-3.1 frequency scaling (transformers' "llama3" rope type)
+    rope_scaling: dict | None = None
 
     @property
     def head_dim(self) -> int:
@@ -44,6 +46,42 @@ class LlamaShape:
 LLAMA3_8B = LlamaShape()
 LLAMA3_70B = LlamaShape(hidden=8192, inter=28672, n_layers=80, n_heads=64, n_kv_heads=8)
 TINY = LlamaShape(hidden=512, inter=1024, n_layers=2, n_heads=8, n_kv_heads=2, vocab=1024)
+# Llama-3.1 / 3.3 (128k context): the Llama-3 shapes with the llama3 RoPE scaling
+LLAMA31_8B = LlamaShape(rope_scaling={"rope_type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
+                                      "original_max_position_embeddings": 8192})
+
+# Above this many cache positions the fused steps run the split-KV attention kernel (csrc/decode_glue.cu): the one-CTA-per-head
+# kernel keeps a score per position in shared memory and stops here.  At or below it they run that kernel as before.
+SINGLE_ATTN_MAX_LEN = 8192
+
+
+def rope_inv_freq(shape: LlamaShape, device) -> torch.Tensor:
+    """RoPE inverse frequencies [head_dim / 2] in fp32; with rope_scaling "llama3" scaled as transformers'
+    `_compute_llama3_parameters` does it (same fp32 operations in the same order)."""
+    hd = shape.head_dim
+    inv = 1.0 / (shape.rope_theta ** (torch.arange(0, hd, 2, device=device, dtype=torch.float32) / hd))
+    sc = shape.rope_scaling
+    if sc is None:
+        return inv
+    if sc.get("rope_type") != "llama3":
+        raise ValueError(f"unsupported rope_scaling {sc!r}: only rope_type 'llama3' is implemented")
+    factor, lf, hf = float(sc["factor"]), float(sc["low_freq_factor"]), float(sc["high_freq_factor"])
+    old = float(sc["original_max_position_embeddings"])
+    low_wl, high_wl = old / lf, old / hf
+    wavelen = 2 * math.pi / inv
+    inv_l = torch.where(wavelen > low_wl, inv / factor, inv)
+    smooth = (old / wavelen - lf) / (hf - lf)
+    smoothed = (1 - smooth) * inv_l / factor + smooth * inv_l
+    medium = ~(wavelen < high_wl) * ~(wavelen > low_wl)
+    return torch.where(medium, smoothed, inv_l)
+
+
+def rope_tables(shape: LlamaShape, cache_len: int, dtype, device):
+    """cos / sin tables [cache_len, head_dim] in `dtype` (the glue kernels read them by position)."""
+    inv = rope_inv_freq(shape, device)
+    t = torch.arange(cache_len, device=device, dtype=torch.float32)
+    fr = torch.outer(t, inv)
+    return torch.cat([fr.cos(), fr.cos()], dim=-1).to(dtype), torch.cat([fr.sin(), fr.sin()], dim=-1).to(dtype)
 
 
 def shard_dims(shape: LlamaShape, tp: int):
@@ -128,18 +166,25 @@ class DecodeModel:
             blk["k_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=dtype)
             blk["v_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=dtype)
             self.blocks.append(blk)
-        hd = shape.head_dim
-        inv = 1.0 / (shape.rope_theta ** (torch.arange(0, hd, 2, device=self.device, dtype=torch.float32) / hd))
-        t = torch.arange(cache_len, device=self.device, dtype=torch.float32)
-        fr = torch.outer(t, inv)
-        self.cos = torch.cat([fr.cos(), fr.cos()], dim=-1).to(dtype)  # [cache_len, hd]
-        self.sin = torch.cat([fr.sin(), fr.sin()], dim=-1).to(dtype)
+        self.cos, self.sin = rope_tables(shape, cache_len, dtype, self.device)  # [cache_len, hd]
         self.arange = torch.arange(cache_len, device=self.device)
         # static I/O for graph capture
         self.tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
         self.pos = torch.zeros(1, dtype=torch.long, device=self.device)
         self.next_tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
         self.graph = None
+
+    @property
+    def attn_kernel(self) -> str:
+        """Attention kernel of the fused steps: "single" (one CTA per query head, cache_len <= 8192) or "split" (split-KV)."""
+        return "split" if self.cache_len > SINGLE_ATTN_MAX_LEN else "single"
+
+    def _attn_split(self, lib, blk, hq, hkv, code, st):
+        from ._lib import check, ptr
+        b = self._bufs
+        check(lib.hqq_b200_glue_rope_attn_decode_split(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                       ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
+                                                       self.shape.head_dim, self.batch, code, st))
 
     # bytes one decode step must read from HBM (SURVEY.md 8d): packed weights + meta + fp16 lm_head row-major
     def bytes_per_token(self, nbits=None, group_size=None) -> float:
@@ -265,8 +310,12 @@ class DecodeModel:
         for blk in self.blocks:
             norm(delta, blk["norm1"])
             self._lin(b["x"], (blk["q"], blk["k"], blk["v"]), [b["q"], b["k"], b["v"]])
-            check(lib.hqq_b200_glue_rope_attn_decode_batch(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                           ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), hq, hkv, self.cache_len, hd, B, code, st))
+            if self.attn_kernel == "split":
+                self._attn_split(lib, blk, hq, hkv, code, st)
+            else:
+                check(lib.hqq_b200_glue_rope_attn_decode_batch(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                               ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), hq, hkv, self.cache_len, hd, B, code,
+                                                               st))
             self._lin(b["a"], (blk["o"],), [b["o"]])
             if self.tp > 1:
                 torch.distributed.all_reduce(b["o"], group=self.pg)
@@ -341,8 +390,11 @@ class DecodeModel:
             ok &= ops.decode_linear_fwd(h_cur, (blk["q"], blk["k"], blk["v"]), [b["q"], b["k"], b["v"]], 1, None if p2p else delta, blk["norm1"], h_nxt,
                                         s.rms_eps, tpx=(self._tpx(bi - 1, red_data=d_loc) if (p2p and bi > 0) else None))
             h_cur, h_nxt = h_nxt, h_cur
-            check(lib.hqq_b200_glue_rope_attn_decode(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                     ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), hq, hkv, self.cache_len, hd, code, st))
+            if self.attn_kernel == "split":
+                self._attn_split(lib, blk, hq, hkv, code, st)
+            else:
+                check(lib.hqq_b200_glue_rope_attn_decode(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                         ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), hq, hkv, self.cache_len, hd, code, st))
             ok &= ops.decode_linear_fwd(b["a"], (blk["o"],), [b["o"]], tpx=self._tpx(bi, peer_data=o_sc) if p2p else None)
             if self.tp > 1 and not p2p:
                 torch.distributed.all_reduce(b["o"], group=self.pg)
@@ -378,6 +430,11 @@ class DecodeModel:
                       "v": z(s.n_kv_heads // tp * s.head_dim), "a": z(s.n_heads // tp * s.head_dim), "o": z(s.hidden),
                       "gate": z(s.inter // tp), "up": z(s.inter // tp), "act": z(s.inter // tp), "down": z(s.hidden), "logits": z(self.vocab_shard),
                       "key": torch.zeros(1, dtype=torch.long, device=dev)}
+        if self.attn_kernel == "split":  # partials + tickets, zeroed once: every launch leaves the tickets at zero
+            from ._lib import load
+            with torch.cuda.device(dev):
+                nbytes = load().hqq_b200_glue_rope_attn_decode_split_workspace_bytes(s.n_heads // tp, s.n_kv_heads // tp, s.head_dim, self.batch)
+            self._bufs["attn_ws"] = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
 
     def capture(self, warmup: int = 3):
         """Warm up on a side stream, then capture one decode step into a CUDA graph."""

@@ -237,6 +237,25 @@ int hqq_b200_glue_rope_attn_decode_batch(const void* q, const void* k, const voi
                                          void* k_cache, void* v_cache, const int64_t* pos, void* out,
                                          int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                          int batch, int dtype, void* stream);
+/* Long-context form of hqq_b200_glue_rope_attn_decode_batch (same layouts, same RoPE and cache rows bit for bit, cache_len up to
+ * 131072 instead of 8192; the decode harness uses it above 8192).  The cached positions are split into S contiguous chunks,
+ * S = max(1, min(SMs / n_kv_heads, ceil(cache_len / 16))), one CTA per (chunk, kv head, sequence) serving all query heads of its
+ * group with tensor-core products; the last CTA of each (sequence, kv head) combines the partials in chunk order.  S does not
+ * depend on batch: a sequence of a batch gets bit for bit what it gets alone.  Like split-K, the result is a function of
+ * (inputs, *pos, SM count).
+ * workspace: hqq_b200_glue_rope_attn_decode_split_workspace_bytes(...) bytes on the device, 4-byte aligned: fp32 partials
+ * [batch, n_kv_heads, S, n_q_heads / n_kv_heads, 2 + head_dim] (laid out for S = max(1, SMs / n_kv_heads)) followed by
+ * batch * n_kv_heads uint32 tickets.  The caller zeroes it once after allocating it; every launch leaves the tickets at zero, so a
+ * captured graph replays without a memset.  One workspace serves any number of launches in stream order.
+ * Needs head_dim 128 and n_q_heads / n_kv_heads <= 8.  The precondition on *pos and cache rows [0, *pos) of
+ * hqq_b200_glue_rope_attn_decode applies. */
+int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const void* v,
+                                         const void* cos_table, const void* sin_table,
+                                         void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace,
+                                         int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                         int batch, int dtype, void* stream);
+/* Workspace bytes of hqq_b200_glue_rope_attn_decode_split on the current device (0 for invalid head counts). */
+size_t hqq_b200_glue_rope_attn_decode_split_workspace_bytes(int n_q_heads, int n_kv_heads, int head_dim, int batch);
 /* out[0] = argmax(logits[0..n)) (first index on ties) */
 int hqq_b200_glue_argmax(const void* logits, int n, int64_t* out, int dtype, void* stream);
 /* Vocabulary-sharded lm_head (tensor parallel decode): out_key[0] = a signed 64-bit key {ordered(max) : 0xFFFFFFFF - (index_offset +

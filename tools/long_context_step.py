@@ -1,0 +1,131 @@
+"""Long-context decode on one GPU: the Llama-3.1-8B-shaped model (4-bit, gs 64, fp16) with a 131072-position KV cache (17 GB),
+caches filled with random rows so no prompt has to be decoded.  For each position it prints one JSON line with
+  - the captured step: time and tok/s over >= 50 graph replays (CUDA events; *pos advances inside the graph),
+  - the attention launch alone: the 32 layers' split-KV launches captured in one graph, us per launch and GB/s, where
+    bytes = 2 n_kv (pos + 1) 128 * 2 (K and V rows read) + q / k / v / out, against the 3.35 TB/s data sheet,
+  - at pos 8191 also the one-CTA-per-head kernel on cache_len 8192 caches, the same way,
+  - the GPU name, power limit and median SM clock over the run (read-only nvidia-smi queries).
+
+    python tools/long_context_step.py [--steps 50] [--positions 1024,8191,...]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from bench import ClockSampler  # noqa: E402
+from hqq_b200 import harness  # noqa: E402
+from hqq_b200._lib import DTYPE_CODE, check, load, ptr, stream_ptr  # noqa: E402
+
+HBM_GBS = 3350.0  # H100 SXM data sheet
+
+
+def gpu_info():
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        name, plim, mx = [x.strip() for x in r.stdout.strip().split(",")[:3]]
+        return {"gpu": name, "power_limit_w": float(plim), "sm_max_mhz": float(mx)}
+    except Exception as e:  # noqa: BLE001
+        return {"gpu": torch.cuda.get_device_name(0), "power_limit_w": None, "error": str(e)[:100]}
+
+
+def time_graph(dev, fn, reps=20):
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream(dev).wait_stream(side)
+    torch.cuda.synchronize(dev)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        fn()
+    g.replay()
+    torch.cuda.synchronize(dev)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        g.replay()
+    e1.record()
+    torch.cuda.synchronize(dev)
+    return e0.elapsed_time(e1) / reps
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--positions", default="1024,8191,16384,32768,65536,131000")
+    ap.add_argument("--cache-len", type=int, default=131072)
+    args = ap.parse_args()
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    info = gpu_info()
+    shape = harness.LLAMA31_8B
+    model = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=args.cache_len, fused=5)
+    model.capture(warmup=2)
+    g = torch.Generator(device=dev).manual_seed(1)
+    for blk in model.blocks:
+        for name in ("k_cache", "v_cache"):
+            c = blk[name]
+            for i in range(0, c.shape[2], 16384):
+                c[:, :, i:i + 16384].copy_(torch.randn(c[:, :, i:i + 16384].shape, generator=g, device=dev) * 0.5)
+    lib, code = load(), DTYPE_CODE[model.dtype]
+    hd, hq, hkv = shape.head_dim, shape.n_heads, shape.n_kv_heads
+    b = model._bufs
+    for t in (b["q"], b["k"], b["v"]):
+        t.copy_(torch.randn(t.shape, generator=g, device=dev))
+    small = None
+    sampler = ClockSampler(0)
+    sampler.start()
+    for pos in [int(p) for p in args.positions.split(",")]:
+        pos = min(pos, args.cache_len - args.steps - 2)
+        model.tok.fill_(7)
+        model.pos.fill_(pos)
+        for _ in range(3):
+            model.decode()
+        model.pos.fill_(pos)
+        torch.cuda.synchronize(dev)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.steps):
+            model.decode()
+        e1.record()
+        torch.cuda.synchronize(dev)
+        step_ms = e0.elapsed_time(e1) / args.steps
+        # the attention launches of all 32 layers in one graph, at this position
+        model.pos.fill_(pos)
+        def split():  # the stream is read at call time: under capture it is the capturing stream
+            for blk in model.blocks:
+                model._attn_split(lib, blk, hq, hkv, code, stream_ptr(dev))
+        ms = time_graph(dev, split) / len(model.blocks)
+        nbytes = 2 * hkv * (pos + 1) * hd * 2 + (2 * hq + 2 * hkv) * hd * 2
+        line = {"pos": pos, "cache_len": args.cache_len, "step_ms": round(step_ms, 4), "tok_s": round(1e3 / step_ms, 2),
+                "steps_timed": args.steps, "attn_kernel": model.attn_kernel, "attn_us_per_launch": round(ms * 1e3, 2),
+                "attn_GBps": round(nbytes / ms / 1e6, 1), "attn_frac_of_3350": round(nbytes / ms / 1e6 / HBM_GBS, 3),
+                "attn_bytes_per_launch": nbytes, "kv_bytes_per_step": 32 * nbytes}
+        if pos == 8191:  # the one-CTA-per-head kernel on cache_len 8192 caches, same position, same graph timing
+            if small is None:
+                small = [(torch.randn(1, hkv, 8192, hd, generator=g, device=dev).half(), torch.randn(1, hkv, 8192, hd, generator=g, device=dev).half())
+                         for _ in model.blocks]
+            cos8, sin8 = model.cos[:8192].contiguous(), model.sin[:8192].contiguous()
+
+            def single():
+                for kc, vc in small:
+                    check(lib.hqq_b200_glue_rope_attn_decode(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(cos8), ptr(sin8), ptr(kc), ptr(vc),
+                                                             ptr(model.pos), ptr(b["a"]), hq, hkv, 8192, hd, code, stream_ptr(dev)))
+            ms1 = time_graph(dev, single) / len(small)
+            line["single_us_per_launch"] = round(ms1 * 1e3, 2)
+            line["single_GBps"] = round(nbytes / ms1 / 1e6, 1)
+            line["split_speedup"] = round(ms1 / ms, 2)
+        line.update(info)
+        print(json.dumps(line), flush=True)
+    clocks = sampler.stop()
+    print(json.dumps({"clocks": clocks, **info}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
