@@ -563,6 +563,232 @@ int split_count(int n_kv, int cache_len) {
   return max(1, min(by_sm, by_len));
 }
 
+// Prompt prefill (DESIGN.md 3.5): a chunk of T positions pos0 .. pos0 + T - 1 of every sequence.
+//
+// rope_append_rows_kernel writes rope(k) and v into cache rows [pos0, pos0 + T) and rope(q) into q_out, rounding exactly as
+// rope_attn_decode_kernel does, so a cache row is bit for bit the row a decode step writes from the same k and v.
+//
+// attn_prefill_kernel: causal GQA attention of the chunk's T queries over cache rows 0 .. pos0 + t (FlashAttention-2 style on
+// mma.sync m16n8k16).  A CTA owns 128 rows (t, h) = (row / G, row % G) of one (kv head, sequence), so each K/V tile is staged once
+// for all G <= 8 heads of the group; each of the 8 warps owns 16 rows for the whole key range:
+//   S [16 rows x 64 positions]  = Q [16 x 128] . K^T        (Q fragments in registers, K from shared memory through ldmatrix)
+//   O [16 rows x 128 dims]     += P [16 x 64]  . V           (P from the S accumulators, V through ldmatrix.trans, O in fp32)
+// K/V tiles of 64 positions, aligned to absolute positions, stream through a 3-stage cp.async ring shared by the CTA (16-byte
+// chunks XOR-swizzled by row).  Rows at or past pos0 + T are never loaded: their slots are zero.  Online softmax in fp32 with
+// exp2f; P is rounded to T for the second MMA and the row sum adds the rounded values; one rounding to T at the end.  A tile that
+// lies wholly past a row's position leaves its m, l and o bit for bit unchanged (scale 1, P = 0), and tile 0 -- which every row
+// sees -- comes first, so a row's output depends only on its q row and cache rows 0 .. p: not on pos0 / T chunking, batch or
+// which rows share its CTA.  No atomics, no workspace.  Query blocks with the longest key range are scheduled first.
+constexpr int kPreWarps = 8;
+constexpr int kPreThreads = 32 * kPreWarps;
+constexpr int kPreRows = 16 * kPreWarps;                  // (position, head) rows per CTA
+constexpr int kPreTile = 64;                              // key positions per tile
+constexpr int kPreStages = 3;
+constexpr int kPreTileBytes = kPreTile * kHd * 2;         // one K or V tile, 16 KB
+constexpr int kPreStageBytes = 2 * kPreTileBytes;
+constexpr int kPreSmemBytes = kPreStages * kPreStageBytes;  // 96 KB
+
+// grid = (T, batch), block = 256.  q / q_out [batch T, n_q 128], k / v [batch T, n_kv 128] (row b T + t), caches [batch, n_kv, L, 128].
+template <typename T>
+__global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
+                                                               const T* __restrict__ cos_t, const T* __restrict__ sin_t, T* __restrict__ k_cache,
+                                                               T* __restrict__ v_cache, T* __restrict__ q_out, int pos0, int n_tok, int n_q,
+                                                               int n_kv, int L) {
+  const int t = (int)blockIdx.x, b = (int)blockIdx.y, p = pos0 + t;
+  {
+    const long long row = (long long)b * n_tok + t;
+    q += row * n_q * kHd; q_out += row * n_q * kHd;
+    k += row * n_kv * kHd; v += row * n_kv * kHd;
+    k_cache += (long long)b * n_kv * L * kHd; v_cache += (long long)b * n_kv * L * kHd;
+  }
+  pdl_launch_dependents();
+  pdl_wait();
+  constexpr int half = kHd / 2;
+  for (int i = (int)threadIdx.x; i < (n_q + 2 * n_kv) * kHd; i += (int)blockDim.x) {
+    const int h = i >> 7, d = i & (kHd - 1);
+    if (h < n_q + n_kv) {  // x*cos + rotate_half(x)*sin, each product and the sum rounded to T (rope_attn_decode_kernel)
+      const float c = to_f32<T>(cos_t[(long long)p * kHd + d]), s = to_f32<T>(sin_t[(long long)p * kHd + d]);
+      const T* x = h < n_q ? q + h * kHd : k + (h - n_q) * kHd;
+      const float xv = to_f32<T>(x[d]);
+      const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
+      const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
+      if (h < n_q) q_out[h * kHd + d] = r;
+      else k_cache[((long long)(h - n_q) * L + p) * kHd + d] = r;
+    } else {
+      const int kvh = h - n_q - n_kv;
+      v_cache[((long long)kvh * L + p) * kHd + d] = v[kvh * kHd + d];
+    }
+  }
+}
+
+// grid = (n_kv, batch, ceil(T G / 128)), block = 256: the query block is the slowest grid index, so the blocks with the longest key
+// range are dispatched first across all kv heads and sequences.  q (rotated) / out [batch T, n_q 128] (row b T + t), caches
+// [batch, n_kv, L, 128].
+template <typename T>
+__global__ void __launch_bounds__(kPreThreads, 1)
+    attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k_cache, const T* __restrict__ v_cache, T* __restrict__ out, int pos0,
+                        int n_tok, int n_q, int n_kv, int L, float scale_log2) {
+  extern __shared__ __align__(16) char smem[];
+  constexpr int ST = kPreStages;
+  const int G = n_q / n_kv;
+  const int rb = (int)(gridDim.z - 1 - blockIdx.z), kvh = (int)blockIdx.x, b = (int)blockIdx.y;  // longest query blocks first
+  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  {
+    const long long kv = (long long)b * n_kv + kvh;
+    k_cache += kv * L * kHd; v_cache += kv * L * kHd;
+  }
+  const int n_rows = n_tok * G, row0 = rb * kPreRows;
+  const int n_tiles = (pos0 + (min(row0 + kPreRows, n_rows) - 1) / G) / kPreTile + 1;  // through the CTA's last position
+  const int lim = pos0 + n_tok;                                                          // rows >= lim are never loaded
+  const int wr0 = row0 + warp * 16;
+  const int w_end = wr0 < n_rows ? pos0 + (min(wr0 + 15, n_rows - 1)) / G : -1;          // the warp's last position
+  // the lane's rows g and g + 8 of the warp: position and q / out row (rows past the chunk compute on zero q and are not stored)
+  const int ra = wr0 + g, rb8 = wr0 + g + 8;
+  const bool va = ra < n_rows, vb = rb8 < n_rows;
+  const int pa = pos0 + (va ? ra / G : n_tok - 1), pb = pos0 + (vb ? rb8 / G : n_tok - 1);
+  const long long oa = ((long long)b * n_tok + (pa - pos0)) * n_q * kHd + (long long)(kvh * G + ra % G) * kHd;
+  const long long ob = ((long long)b * n_tok + (pb - pos0)) * n_q * kHd + (long long)(kvh * G + rb8 % G) * kHd;
+  pdl_launch_dependents();
+  pdl_wait();
+
+  auto issue = [&](int j) {
+    if (j < n_tiles) {
+      const int t0 = j * kPreTile;
+      char* st = smem + (j % ST) * kPreStageBytes;
+#pragma unroll 4
+      for (int c = tid; c < 2 * kPreTile * 16; c += kPreThreads) {
+        const int isv = c >> 10, r = (c >> 4) & (kPreTile - 1), ch = c & 15, p = t0 + r;
+        char* dst = st + isv * kPreTileBytes + swz(r, ch);
+        if (p < lim) {
+          split_cp16(dst, (isv ? v_cache : k_cache) + (long long)p * kHd + ch * 8);
+        } else {
+          uint4 z;
+          z.x = z.y = z.z = z.w = 0u;
+          *reinterpret_cast<uint4*>(dst) = z;
+        }
+      }
+    }
+    split_commit();  // always (possibly empty): every iteration waits on the same group count
+  };
+#pragma unroll
+  for (int i = 0; i < ST - 1; ++i) issue(i);
+
+  // Q fragments (A operand of the score MMA): rows g, g + 8; dims 16 kk + 2 qd + {0, 1} and + 8
+  uint32_t qf[8][4];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+    const int d = kk * 16 + 2 * qd;
+    qf[kk][0] = va ? *reinterpret_cast<const uint32_t*>(q + oa + d) : 0u;
+    qf[kk][1] = vb ? *reinterpret_cast<const uint32_t*>(q + ob + d) : 0u;
+    qf[kk][2] = va ? *reinterpret_cast<const uint32_t*>(q + oa + d + 8) : 0u;
+    qf[kk][3] = vb ? *reinterpret_cast<const uint32_t*>(q + ob + d + 8) : 0u;
+  }
+  // lane (g, qd) holds m, l (its share of the row sum) and O columns 8 dt + 2 qd + {0, 1} of rows g (index 0) and g + 8 (index 1)
+  float o[16][4];
+#pragma unroll
+  for (int dt = 0; dt < 16; ++dt) o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  const int kr = (lane & 7) + ((lane >> 4) & 1) * 8, kc = (lane >> 3) & 1;  // K as the B operand: n-tile pairs, then k + 8
+  const int vr = (lane & 7) + ((lane >> 3) & 1) * 8, vc = lane >> 4;         // V through .trans: positions + 8, then dims + 8
+  for (int j = 0; j < n_tiles; ++j) {
+    split_wait<ST - 2>();
+    __syncthreads();  // tile j is visible to every warp, and every warp is done with the slot the next issue overwrites
+    issue(j + ST - 1);
+    const int t0 = j * kPreTile;
+    if (t0 > w_end) continue;  // wholly past every row of this warp: it would change nothing
+    const char* kt = smem + (j % ST) * kPreStageBytes;
+    const char* vt = kt + kPreTileBytes;
+    float s[8][4];
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+#pragma unroll
+      for (int np = 0; np < 4; ++np) {
+        uint32_t kb[4];
+        ldsm4<false>(kb, kt + swz(16 * np + kr, 2 * kk + kc));
+        mma16816<T>(s[2 * np], qf[kk], kb[0], kb[1]);
+        mma16816<T>(s[2 * np + 1], qf[kk], kb[2], kb[3]);
+      }
+    }
+    float x0 = -INFINITY, x1 = -INFINITY;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const int kp = t0 + 8 * nt + 2 * qd;
+      s[nt][0] = kp <= pa ? s[nt][0] * scale_log2 : -INFINITY;
+      s[nt][1] = kp + 1 <= pa ? s[nt][1] * scale_log2 : -INFINITY;
+      s[nt][2] = kp <= pb ? s[nt][2] * scale_log2 : -INFINITY;
+      s[nt][3] = kp + 1 <= pb ? s[nt][3] * scale_log2 : -INFINITY;
+      x0 = fmaxf(x0, fmaxf(s[nt][0], s[nt][1]));
+      x1 = fmaxf(x1, fmaxf(s[nt][2], s[nt][3]));
+    }
+#pragma unroll
+    for (int off = 1; off < 4; off <<= 1) {
+      x0 = fmaxf(x0, __shfl_xor_sync(0xffffffffu, x0, off));
+      x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, off));
+    }
+    const float n0 = fmaxf(m0, x0), n1 = fmaxf(m1, x1);  // finite: tile 0 holds position 0, which every row sees
+    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
+    m0 = n0; m1 = n1;
+    uint32_t pf[8][2];  // P rounded to T, packed as the A operand of the second MMA
+    float r0 = 0.f, r1 = 0.f;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const T e0 = from_f32<T>(exp2f(s[nt][0] - n0)), e1 = from_f32<T>(exp2f(s[nt][1] - n0));
+      const T e2 = from_f32<T>(exp2f(s[nt][2] - n1)), e3 = from_f32<T>(exp2f(s[nt][3] - n1));
+      r0 += to_f32<T>(e0) + to_f32<T>(e1);
+      r1 += to_f32<T>(e2) + to_f32<T>(e3);
+      pf[nt][0] = bits16(e0) | (bits16(e1) << 16);
+      pf[nt][1] = bits16(e2) | (bits16(e3) << 16);
+    }
+    l0 = l0 * a0 + r0;
+    l1 = l1 * a1 + r1;
+#pragma unroll
+    for (int dt = 0; dt < 16; ++dt) { o[dt][0] *= a0; o[dt][1] *= a0; o[dt][2] *= a1; o[dt][3] *= a1; }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint32_t pa4[4] = {pf[2 * kk][0], pf[2 * kk][1], pf[2 * kk + 1][0], pf[2 * kk + 1][1]};
+#pragma unroll
+      for (int dp = 0; dp < 8; ++dp) {
+        uint32_t vb4[4];
+        ldsm4<true>(vb4, vt + swz(16 * kk + vr, 2 * dp + vc));
+        mma16816<T>(o[2 * dp], pa4, vb4[0], vb4[1]);
+        mma16816<T>(o[2 * dp + 1], pa4, vb4[2], vb4[3]);
+      }
+    }
+  }
+  split_wait<0>();
+#pragma unroll
+  for (int off = 1; off < 4; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+#pragma unroll
+  for (int dt = 0; dt < 16; ++dt) {
+    const int d = dt * 8 + 2 * qd;
+    if (va) {
+      const T y[2] = {from_f32<T>(o[dt][0] / l0), from_f32<T>(o[dt][1] / l0)};
+      *reinterpret_cast<uint32_t*>(out + oa + d) = bits16(y[0]) | (bits16(y[1]) << 16);
+    }
+    if (vb) {
+      const T y[2] = {from_f32<T>(o[dt][2] / l1), from_f32<T>(o[dt][3] / l1)};
+      *reinterpret_cast<uint32_t*>(out + ob + d) = bits16(y[0]) | (bits16(y[1]) << 16);
+    }
+  }
+}
+
+// The checks both prefill entry points share; returns HQQ_OK or the error code (message set).
+int prefill_args(const char* name, int pos0, int n_tok, int n_q, int n_kv, int L, int hd, int batch, int dtype) {
+  HQQ_REQUIRE(dtype == HQQ_F16 || dtype == HQQ_BF16, HQQ_E_INVALID, "%s: dtype must be f16/bf16", name);
+  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
+  HQQ_REQUIRE(hd == kHd && n_kv > 0 && n_kv <= 65535 && n_q > 0 && n_q % n_kv == 0 && n_q / n_kv <= kSplitMaxGroup && L > 0 && L <= kSplitMaxLen,
+              HQQ_E_UNSUPPORTED, "%s: needs head_dim 128, n_q_heads %% n_kv_heads == 0, n_q_heads / n_kv_heads <= 8, cache_len <= 131072 (got %d, %d/%d, %d)",
+              name, hd, n_q, n_kv, L);
+  HQQ_REQUIRE(n_tok >= 1 && pos0 >= 0 && n_tok <= L && pos0 <= L - n_tok, HQQ_E_INVALID, "%s: needs 1 <= T and pos0 + T <= cache_len (pos0=%d T=%d cache_len=%d)",
+              name, pos0, n_tok, L);
+  return HQQ_OK;
+}
+
 }  // namespace
 
 #ifndef HQQ_EMU
@@ -777,6 +1003,39 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k
   }
   set_error("hqq_b200_glue_rope_attn_decode_split: dtype must be f16/bf16");
   return HQQ_E_INVALID;
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache,
+                                              void* v_cache, void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                              int batch, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows";
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && q_out, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = prefill_args(name, pos0, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows", rope_append_rows_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k,
+                      (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, pos0, T, n_q_heads, n_kv_heads,
+                      cache_len);
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_attn_prefill(const void* q_rot, const void* k_cache, const void* v_cache, void* out, int pos0, int T, int n_q_heads,
+                                          int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_attn_prefill";
+  HQQ_REQUIRE(q_rot && k_cache && v_cache && out, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = prefill_args(name, pos0, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
+  const dim3 grid((unsigned)n_kv_heads, (unsigned)batch, (unsigned)cdiv((int64_t)T * (n_q_heads / n_kv_heads), kPreRows));  // z <= 8192
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    if (int rc = reserve_smem<attn_prefill_kernel<E>>(kPreSmemBytes)) return rc;
+    return launch_pdl("attn_prefill", attn_prefill_kernel<E>, grid, dim3(kPreThreads), kPreSmemBytes, st, (const E*)q_rot, (const E*)k_cache,
+                      (const E*)v_cache, (E*)out, pos0, T, n_q_heads, n_kv_heads, cache_len, scale_log2);
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
 
 #ifndef HQQ_EMU

@@ -173,6 +173,7 @@ class DecodeModel:
         self.pos = torch.zeros(1, dtype=torch.long, device=self.device)
         self.next_tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
         self.graph = None
+        self.last_logits = None  # set by prefill(): logits of the last prompt position of each sequence
 
     @property
     def attn_kernel(self) -> str:
@@ -421,6 +422,147 @@ class DecodeModel:
             check(lib.hqq_b200_glue_add_rmsnorm(ptr(h_cur), ptr(delta), ptr(self.final_norm), ptr(b["x"]), s.hidden, s.rms_eps, code, st))
         self._head(lib, b["x"], code, st)
         self.pos.add_(1).remainder_(self.cache_len)
+
+    def prefill(self, tokens: torch.Tensor, start: int = 0, chunk: int = 2048) -> torch.Tensor:
+        """Take in a prompt: `tokens` [batch, T] (or [T] when batch is 1) at positions start .. start + T - 1 of every sequence.
+        The prompt runs in chunks of at most `chunk` tokens (batch * chunk <= 65535, the row limit of the rows kernels); each
+        chunk goes through every block, writing its rotated k and v into the caches.  Only the last position of each sequence
+        goes through the final norm, the lm_head and the argmax; self.last_logits [batch, vocab / tp] keeps those logits (this
+        rank's vocabulary shard).  Afterwards self.pos = (start + T) mod cache_len -- the steps' own wrap, so a prompt that fills
+        the cache leaves the next step at position 0 as a step at the last position does -- and self.tok [batch] holds the greedy
+        next token, which is returned: a captured decode step continues from there.
+
+        fused (any value but False): the package's kernels -- add+RMSNorm rows, the routed q/k/v linears at M = batch * chunk,
+        RoPE + cache append, causal GQA attention over the cache (csrc/decode_glue.cu), o, add+RMSNorm rows, gate/up, SiLU*mul,
+        down.  fused=False: the same walk on framework ops (F.rms_norm, the layers, torch RoPE, F.scaled_dot_product_attention
+        with a causal mask over the cache), the correctness reference as step() is for decode.  With tensor parallelism the two
+        row-parallel outputs and the head's argmax keys meet in NCCL all-reduces; the peer-memory exchange of fused=5 decode and
+        its step counter are not touched."""
+        s, B = self.shape, self.batch
+        tokens = torch.as_tensor(tokens, device=self.device)
+        if tokens.dim() == 1 and B == 1:
+            tokens = tokens.view(1, -1)
+        if tokens.dim() != 2 or tokens.shape[0] != B:
+            raise ValueError(f"tokens must be [batch={B}, T] (or [T] when batch is 1), got {tuple(tokens.shape)}")
+        T = int(tokens.shape[1])
+        if T < 1 or start < 0 or start + T > self.cache_len:
+            raise ValueError(f"prompt positions [{start}, {start + T}) must lie in the cache [0, {self.cache_len})")
+        chunk = min(int(chunk), 65535 // B)
+        if chunk < 1:
+            raise ValueError("chunk must be >= 1")
+        tokens = tokens.to(torch.long)
+        hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
+        h_last = d_last = None
+        with torch.no_grad():
+            for c0 in range(0, T, chunk):
+                n = min(chunk, T - c0)
+                h, delta = (self._prefill_chunk_fused if self.fused else self._prefill_chunk_ref)(tokens[:, c0:c0 + n], start + c0, hd, hq, hkv)
+                if c0 + n == T:
+                    h_last, d_last = h.view(B, n, s.hidden)[:, -1].contiguous(), delta.view(B, n, s.hidden)[:, -1].contiguous()
+            tok = self._prefill_head(h_last, d_last)
+        self.tok.copy_(tok)
+        self.pos.fill_((start + T) % self.cache_len)
+        return self.tok.clone()
+
+    def _prefill_chunk_fused(self, ids, p0, hd, hq, hkv):
+        """One chunk on the package's kernels; returns the residual stream h [M, hidden] before the last block's MLP delta, and
+        that delta (the final norm adds them for the rows it needs)."""
+        from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
+        lib, s = load(), self.shape
+        st = stream_ptr(self.device)
+        code = DTYPE_CODE[self.dtype]
+        B, n = ids.shape
+        M = B * n
+        e = lambda w: torch.empty(M, w, device=self.device, dtype=self.dtype)
+        h = self.embed.index_select(0, ids.reshape(-1))  # [M, hidden], row b * n + t
+        x, q, k, v, qr, a, o = e(s.hidden), e(hq * hd), e(hkv * hd), e(hkv * hd), e(hq * hd), e(hq * hd), e(s.hidden)
+        inter = s.inter // self.tp
+        gate, up, act, down = e(inter), e(inter), e(inter), e(s.hidden)
+        norm = lambda d, w: check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(d), ptr(w), ptr(x), M, s.hidden, s.rms_eps, code, st))
+        delta = None
+        for blk in self.blocks:
+            norm(delta, blk["norm1"])
+            self._lin(x, (blk["q"], blk["k"], blk["v"]), [q, k, v])
+            check(lib.hqq_b200_glue_rope_append_rows(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
+                                                     ptr(qr), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
+            check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(blk["k_cache"]), ptr(blk["v_cache"]), ptr(a), p0, n, hq, hkv, self.cache_len, hd, B,
+                                                 code, st))
+            self._lin(a, (blk["o"],), [o])
+            if self.tp > 1:
+                torch.distributed.all_reduce(o, group=self.pg)
+            norm(o, blk["norm2"])
+            self._lin(x, (blk["gate"], blk["up"]), [gate, up])
+            check(lib.hqq_b200_glue_silu_mul(ptr(gate), ptr(up), ptr(act), M * inter, code, st))
+            self._lin(act, (blk["down"],), [down])
+            if self.tp > 1:
+                torch.distributed.all_reduce(down, group=self.pg)
+            delta = down
+        return h, delta
+
+    def _prefill_chunk_ref(self, ids, p0, hd, hq, hkv):
+        """The same chunk on framework ops (fused=False)."""
+        s = self.shape
+        B, n = ids.shape
+        M = B * n
+        h = self.embed.index_select(0, ids.reshape(-1))
+        cos, sin = self.cos[p0:p0 + n].view(1, n, 1, hd), self.sin[p0:p0 + n].view(1, n, 1, hd)
+        end = p0 + n
+        mask = torch.arange(end, device=self.device).view(1, end) <= torch.arange(p0, end, device=self.device).view(n, 1)  # [n, end]
+        delta = None
+        for blk in self.blocks:
+            if delta is not None:
+                h = h + delta
+            x = F.rms_norm(h, (s.hidden,), blk["norm1"], s.rms_eps)
+            q, k, v = self._multi(x, (blk["q"], blk["k"], blk["v"]))
+            q = self._rope(q.view(B, n, hq, hd), cos, sin)
+            k = self._rope(k.view(B, n, hkv, hd), cos, sin)
+            blk["k_cache"][:, :, p0:end] = k.transpose(1, 2)
+            blk["v_cache"][:, :, p0:end] = v.view(B, n, hkv, hd).transpose(1, 2)
+            a = F.scaled_dot_product_attention(q.transpose(1, 2), blk["k_cache"][:, :, :end], blk["v_cache"][:, :, :end], attn_mask=mask,
+                                               enable_gqa=True)
+            o = blk["o"](a.transpose(1, 2).reshape(M, hq * hd))
+            if self.tp > 1:
+                torch.distributed.all_reduce(o, group=self.pg)
+            h = h + o
+            x = F.rms_norm(h, (s.hidden,), blk["norm2"], s.rms_eps)
+            g, u = self._multi(x, (blk["gate"], blk["up"]))
+            delta = blk["down"](F.silu(g) * u)
+            if self.tp > 1:
+                torch.distributed.all_reduce(delta, group=self.pg)
+        return h, delta
+
+    def _prefill_head(self, h, delta):
+        """Final norm, lm_head and greedy pick for the last position of each sequence: h, delta [batch, hidden]."""
+        s, B = self.shape, self.batch
+        if not self.fused:
+            x = F.rms_norm(h + delta, (s.hidden,), self.final_norm, s.rms_eps)
+            logits = torch.matmul(x, self.lm_head.t())
+            self.last_logits = logits
+            if self.tp == 1:
+                return torch.argmax(logits, dim=-1)
+            val, idx = torch.max(logits.float(), dim=-1)
+            gmax = val.clone()
+            torch.distributed.all_reduce(gmax, op=torch.distributed.ReduceOp.MAX, group=self.pg)
+            cand = torch.where(val == gmax, idx + self.rank * self.vocab_shard, torch.full_like(idx, s.vocab))
+            torch.distributed.all_reduce(cand, op=torch.distributed.ReduceOp.MIN, group=self.pg)
+            return cand
+        from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
+        lib = load()
+        st = stream_ptr(self.device)
+        code = DTYPE_CODE[self.dtype]
+        x = torch.empty_like(h)
+        check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(delta), ptr(self.final_norm), ptr(x), B, s.hidden, s.rms_eps, code, st))
+        self.last_logits = torch.matmul(x, self.lm_head.t())
+        # the argmax kernel reads 16-byte vectors: every row starts on a 16-byte boundary whatever the vocabulary shard's length
+        n = self.vocab_shard
+        rows = torch.empty(B, -(-n // 8) * 8, dtype=self.dtype, device=self.device)
+        rows[:, :n].copy_(self.last_logits)
+        key = torch.empty(B, dtype=torch.long, device=self.device)
+        for b in range(B):  # {value : 0xFFFFFFFF - global index} keys: their MAX over the vocabulary shards is the first global argmax
+            check(lib.hqq_b200_glue_argmax_key(ptr(rows[b]), n, self.rank * n, ptr(key[b:]), code, st))
+        if self.tp > 1:
+            torch.distributed.all_reduce(key, op=torch.distributed.ReduceOp.MAX, group=self.pg)
+        return 0xFFFFFFFF - torch.bitwise_and(key, 0xFFFFFFFF)
 
     def _alloc_bufs(self):
         s, dev, dt = self.shape, self.device, self.dtype

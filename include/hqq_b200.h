@@ -256,6 +256,26 @@ int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const voi
                                          int batch, int dtype, void* stream);
 /* Workspace bytes of hqq_b200_glue_rope_attn_decode_split on the current device (0 for invalid head counts). */
 size_t hqq_b200_glue_rope_attn_decode_split_workspace_bytes(int n_q_heads, int n_kv_heads, int head_dim, int batch);
+/* Prompt prefill, step 1: a chunk of T positions pos0 .. pos0 + T - 1 of `batch` sequences.  q [batch*T, n_q_heads*head_dim],
+ * k / v [batch*T, n_kv_heads*head_dim] as the q/k/v linears produce them (token row b*T + t); caches [batch, n_kv_heads, cache_len,
+ * head_dim].  Writes rope(k) and v into cache rows [pos0, pos0 + T) and rope(q) into q_out (same layout as q).  RoPE rounds as
+ * hqq_b200_glue_rope_attn_decode does (each product and the sum rounded to dtype), so a cache row written here is bit for bit the
+ * row a decode step writes at the same position from the same k and v.
+ * Needs head_dim 128, n_q_heads % n_kv_heads == 0, n_q_heads / n_kv_heads <= 8, 1 <= T, pos0 + T <= cache_len <= 131072,
+ * batch <= 65535. */
+int hqq_b200_glue_rope_append_rows(const void* q, const void* k, const void* v,
+                                   const void* cos_table, const void* sin_table,
+                                   void* k_cache, void* v_cache, void* q_out, int pos0, int T,
+                                   int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                   int batch, int dtype, void* stream);
+/* Prompt prefill, step 2: causal GQA attention of the chunk's queries over the cache.  Query t (row b*T + t of q_rot, rotated as
+ * hqq_b200_glue_rope_append_rows leaves it) sits at position pos0 + t and attends to cache rows 0 .. pos0 + t; out has the layout
+ * of q_rot, ready for o_proj.  Cache rows at or past pos0 + T are never read.  A row's output depends only on its q row and cache
+ * rows 0 .. pos0 + t: it is bit for bit the same whatever pos0 / T chunking or batch produced it.  No workspace, no atomics.
+ * Same argument limits as hqq_b200_glue_rope_append_rows. */
+int hqq_b200_glue_attn_prefill(const void* q_rot, const void* k_cache, const void* v_cache, void* out,
+                               int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                               int batch, int dtype, void* stream);
 /* out[0] = argmax(logits[0..n)) (first index on ties) */
 int hqq_b200_glue_argmax(const void* logits, int n, int64_t* out, int dtype, void* stream);
 /* Vocabulary-sharded lm_head (tensor parallel decode): out_key[0] = a signed 64-bit key {ordered(max) : 0xFFFFFFFF - (index_offset +
