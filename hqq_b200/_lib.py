@@ -62,6 +62,8 @@ SIGNATURES = {
     "hqq_b200_glue_rope_attn_decode_split_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "hqq_b200_glue_rope_append_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                                c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_kv8": (c_int, [c_void_p] * 14 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv8": (c_int, [c_void_p] * 14 + [c_int] * 9 + [c_void_p]),
     "hqq_b200_glue_attn_prefill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "hqq_b200_glue_argmax": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_key": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),

@@ -126,6 +126,36 @@ template <> __device__ __forceinline__ __nv_bfloat16 dequant_one<__nv_bfloat16>(
   return __hmul(__hsub(level_to<__nv_bfloat16>(q), z), s);
 }
 
+// ---- quantisation of one group (csrc/quantize.cu and the 8-bit KV cache of csrc/decode_glue.cu) ----------------------------
+__device__ __forceinline__ float rint_magic(float t) {
+  // round-half-even for |t| < 2^22; beyond that the result is still >= 2^22-ish in magnitude with the
+  // right sign, so the clamp that always follows yields the same level as rintf would.
+  return __fsub_rn(__fadd_rn(t, 12582912.0f), 12582912.0f);
+}
+
+struct GroupState {
+  float s, rs, z;
+};
+
+__device__ __forceinline__ void init_group(float mn, float mx, int maxv, int round_zero, GroupState& st) {
+  // quantize.py:126-134 ; `max_v / denom` is reciprocal(denom) * max_v in torch (two roundings)
+  float denom = __fsub_rn(mx, mn);
+  float s = __fmul_rn(__frcp_rn(denom), (float)maxv);
+  if (fabsf(denom) <= 1e-4f) s = 1.0f;
+  s = fminf(s, 2e4f);
+  float z = __fmul_rn(-mn, s);
+  if (round_zero) z = rintf(z);
+  st.s = s;
+  st.rs = __frcp_rn(s);
+  st.z = z;
+}
+
+// optimize.py:254 / quantize.py:147: round(W*scale + zero).clamp(min,max); mul and add round separately
+__device__ __forceinline__ float quant_level(float w, float s, float z, float fmaxv) {
+  const float t = rint_magic(__fadd_rn(__fmul_rn(w, s), z));
+  return fminf(fmaxf(t, 0.0f), fmaxv);
+}
+
 // ---- vector of N elements of T with 16/8/4-byte aligned storage ------------------------
 template <typename T, int N>
 struct alignas(sizeof(T) * N >= 16 ? 16 : sizeof(T) * N) Vec {

@@ -345,6 +345,10 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], 
 #endif
 }
 
+template <typename T>
+__device__ __forceinline__ void split_merge(const float* wp, float* __restrict__ part, unsigned* __restrict__ tickets, T* __restrict__ out, int* last,
+                                           int S, int split, int G, int tid);
+
 // grid = (S, n_kv, batch), block = 256.  q / out [batch, n_q * 128], k / v [batch, n_kv * 128], caches [batch, n_kv, L, 128].
 // part: [batch, n_kv, S, G, 2 + 128] floats (m, l, o per head), tickets: [batch, n_kv] uint32, zero between launches.
 template <typename T>
@@ -516,6 +520,15 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
     }
   }
   __syncthreads();
+  split_merge<T>(wp, part, tickets, out, last, S, split, G, tid);
+}
+
+// The end of both split kernels, once the warp partials wp [NW][8][m, l, o[128]] are in shared memory: this CTA's partial to the
+// workspace, the ticket, and in the last CTA of the (sequence, kv head) the merge of all S partials into out.
+template <typename T>
+__device__ __forceinline__ void split_merge(const float* wp, float* __restrict__ part, unsigned* __restrict__ tickets, T* __restrict__ out, int* last,
+                                           int S, int split, int G, int tid) {
+  constexpr int NW = kSplitWarps;
   // this CTA's partial, warps in order (an empty chunk publishes m = -inf, l = 0, o = 0)
   for (int i = tid; i < G * kHd; i += kSplitThreads) {
     const int h = i >> 7, d = i & (kHd - 1);
@@ -555,6 +568,324 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
     out[h * kHd + d] = from_f32<T>(osum / lsum);
   }
   if (tid == 0) *tickets = 0u;  // ready for the next launch (graph replay needs no memset)
+}
+
+// 8-bit HQQ KV cache (DESIGN.md 3.5).  A cache row of one kv head is Quantizer.quantize(row, nbits=8, group_size=gs, axis=1,
+// optimize=False): levels uint8 [128] and per-group scale / zero [128 / gs] in T; the attended row is T(T(q - z) * s), what
+// hqq_b200_dequantize gives.
+//
+// kv8_quant4: a 128-element row held four per lane (lane l: elements 4 l .. 4 l + 3).  Group min / max over gs / 4 lanes, then
+// init_group (maxv 255, zero not rounded) and quant_level as quantize.cu does for an 8-bit layer without the solver.  Returns the
+// four levels (byte j: element 4 l + j) and the scale (1 / s) and zero of the lane's group rounded to T.
+template <typename T>
+__device__ __forceinline__ uint32_t kv8_quant4(const float (&x)[4], int gs, T& scale, T& zero) {
+  float mn = fminf(fminf(x[0], x[1]), fminf(x[2], x[3])), mx = fmaxf(fmaxf(x[0], x[1]), fmaxf(x[2], x[3]));
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    if (o < gs / 4) {
+      mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    }
+  }
+  GroupState st;
+  init_group(mn, mx, 255, 0, st);
+  uint32_t q = 0;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) q |= (uint32_t)quant_level(x[j], st.s, st.z, 255.0f) << (8 * j);
+  scale = from_f32<T>(__frcp_rn(st.s));  // quantize.py:154 scale = 1.0 / scale, then the meta cast to T
+  zero = from_f32<T>(st.z);
+  return q;
+}
+
+template <typename T> struct Pair;
+template <> struct Pair<__half> { using type = __half2; };
+template <> struct Pair<__nv_bfloat16> { using type = __nv_bfloat162; };
+
+// The two levels in bytes 2 HI, 2 HI + 1 of w -> T(T(q - z) * s) each, packed as a T2 (byte 2 HI in the low half): T(q) exactly,
+// then one rounded T subtraction and one rounded T product per element (z, s: T2 of the two elements' zero and scale).
+// fp16: half2(1024 + q) by bit pattern (0x64qq; one prmt for both), minus 1024 exactly.  bf16 (8 significant bits cannot hold
+// 1024 + q): float 2^23 + q by bit pattern, minus 2^23, packed to bf16x2 exactly.
+template <typename T, int HI>
+__device__ __forceinline__ uint32_t kv8_deq2(uint32_t w, typename Pair<T>::type z, typename Pair<T>::type s) {
+  typename Pair<T>::type q;
+  if constexpr (std::is_same<T, __half>::value) {
+    const uint32_t h = prmt(w, 0x64646464u, HI ? 0x4342u : 0x4140u);
+    q = __hsub2(*reinterpret_cast<const __half2*>(&h), __half2half2(__ushort_as_half((unsigned short)0x6400u)));
+  } else {
+    const float a = __fsub_rn(__uint_as_float(prmt(w, 0x4B000000u, 0x7540u | (2 * HI))), 8388608.0f);
+    const float b = __fsub_rn(__uint_as_float(prmt(w, 0x4B000000u, 0x7540u | (2 * HI + 1))), 8388608.0f);
+    q = __floats2bfloat162_rn(a, b);
+  }
+  const typename Pair<T>::type r = __hmul2(__hsub2(q, z), s);
+  return *reinterpret_cast<const uint32_t*>(&r);
+}
+
+// Split-KV decode attention over an 8-bit cache: rope_attn_decode_split_kernel's grid, chunks, ticket, merge and RoPE.  Each warp
+// streams levels and meta of its 16-position tiles through a 4-stage cp.async ring (4352 bytes a stage: K and V levels [16][128],
+// 16-byte chunks XOR-swizzled by row, then k scale | k zero | v scale | v zero [16][128 / gs]) and dequantises straight into the MMA
+// fragments.  The head dim is permuted, the same way for both operands of a product (so the products are unchanged): lane
+// (g, qd) takes K dims 32 qd .. 32 qd + 31 of positions g, g + 8 (k slot 2 qd + {0, 1, 8, 9} of step kk is dim 32 qd + 4 kk + {0..3})
+// and V dims 16 g .. 16 g + 15 of positions 2 qd + {0, 1, 8, 9} (O^T row g / g + 8 of step mt is dim 16 g + 2 mt / + 1): two
+// 16-byte loads a row, one group each.  Row pos is this launch's quantisation of the fresh k / v in every CTA that holds it; split
+// 0 writes it to the cache.
+constexpr int kKv8Stages = 4;
+constexpr int kKv8LvlBytes = kSplitTile * kHd;                                    // one K or V level tile, 2 KB
+constexpr int kKv8MetaBytes = kSplitTile * 2 * 2;                                 // one meta array of a tile: [16][<= 2] T
+constexpr int kKv8StageBytes = 2 * kKv8LvlBytes + 4 * kKv8MetaBytes;
+constexpr int kKv8RingBytes = kSplitWarps * kKv8Stages * kKv8StageBytes;           // 136 KB
+// + rotated q [8][128] T, fresh k, v [128] T, their levels [2][128] and meta [4][2] T, the last-CTA flag
+constexpr int kKv8SmemBytes = kKv8RingBytes + (kSplitMaxGroup + 2) * kHd * 2 + 2 * kHd + 16 + 16;
+static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kKv8RingBytes, "the warp partials reuse the ring");
+
+__device__ __forceinline__ int swz8(int r, int c) { return r * kHd + ((c ^ (r & 7)) << 4); }  // 16-byte chunk c of level row r
+
+// grid = (S, n_kv, batch), block = 256.  q / out, k / v as rope_attn_decode_split_kernel; levels [batch, n_kv, L, 128] uint8, meta
+// [batch, n_kv, L, 128 / gs] T; part / tickets as there.
+template <typename T>
+__global__ void __launch_bounds__(kSplitThreads, 1)
+    rope_attn_decode_split_kv8_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
+                                      const T* __restrict__ sin_t, uint8_t* __restrict__ k_q, T* __restrict__ k_s, T* __restrict__ k_z,
+                                      uint8_t* __restrict__ v_q, T* __restrict__ v_s, T* __restrict__ v_z, const long long* __restrict__ pos_p,
+                                      T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
+                                      int gs, float scale_log2) {
+  extern __shared__ __align__(16) char smem[];
+  constexpr int NW = kSplitWarps, ST = kKv8Stages;
+  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
+  const int G = n_q / n_kv, ng = kHd / gs;
+  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  {
+    const long long kv = (long long)b * n_kv + kvh;
+    k_q += kv * L * kHd; v_q += kv * L * kHd;
+    k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+    k_in += kv * kHd; v_in += kv * kHd;
+    q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
+    part += kv * S * G * kPartFloats;
+    tickets += kv;
+  }
+  char* ring = smem + warp * ST * kKv8StageBytes;
+  T* qs = reinterpret_cast<T*>(smem + kKv8RingBytes);  // rotated q [8][128]
+  T* kf = qs + kSplitMaxGroup * kHd;                   // rotated k and v of position pos
+  T* vf = kf + kHd;
+  uint8_t* fq = reinterpret_cast<uint8_t*>(vf + kHd);  // their levels: k [128], v [128]
+  T* fm = reinterpret_cast<T*>(fq + 2 * kHd);          // their meta: k scale, k zero, v scale, v zero [2] each
+  int* last = reinterpret_cast<int*>(fm + 8);
+
+  // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
+  const int pos = (int)pos_p[0], n_pos = pos + 1;
+  const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
+  const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
+  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
+  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;
+  pdl_launch_dependents();
+
+  // Stage local tile i as rope_attn_decode_split_kernel does: rows < pos from the cache, row pos from this launch's quantisation
+  // once `fresh`, rows past pos zero (levels and meta: they dequantise to 0).  A meta chunk of 16 bytes spans 8 / ng rows; one that
+  // reaches row pos (or sits on a misaligned address) is staged row by row.
+  auto issue = [&](int i, bool fresh) {
+    if (i < my_tiles) {
+      const int t0 = c0 + (warp + i * NW) * kSplitTile;
+      char* st = ring + (i % ST) * kKv8StageBytes;
+#pragma unroll 4
+      for (int j = lane; j < 2 * kSplitTile * 8; j += 32) {
+        const int isv = j >> 7, r = (j >> 3) & 15, c = j & 7, p = t0 + r;
+        char* dst = st + isv * kKv8LvlBytes + swz8(r, c);
+        if (p < pos) {
+          split_cp16(dst, (isv ? v_q : k_q) + (long long)p * kHd + c * 16);
+        } else if (p > pos || fresh) {
+          uint4 val;
+          val.x = val.y = val.z = val.w = 0u;
+          if (p == pos) val = *reinterpret_cast<const uint4*>(fq + isv * kHd + c * 16);
+          *reinterpret_cast<uint4*>(dst) = val;
+        }
+      }
+      if (lane < 8 * ng) {  // 4 arrays x 2 ng chunks
+        const int a = lane / (2 * ng), j = lane % (2 * ng), rows = 8 / ng, r0 = j * rows;
+        const T* src = (a == 0 ? k_s : a == 1 ? k_z : a == 2 ? v_s : v_z) + (long long)(t0 + r0) * ng;
+        char* dst = st + 2 * kKv8LvlBytes + a * kKv8MetaBytes + j * 16;
+        if (t0 + r0 + rows <= pos && ((uintptr_t)src & 15) == 0) {
+          split_cp16(dst, src);
+        } else {
+          for (int e = 0; e < 8; ++e) {
+            const int p = t0 + r0 + e / ng;
+            if (p < pos) reinterpret_cast<T*>(dst)[e] = src[e];
+            else if (p > pos) reinterpret_cast<T*>(dst)[e] = from_f32<T>(0.f);
+            else if (fresh) reinterpret_cast<T*>(dst)[e] = fm[2 * a + e % ng];
+          }
+        }
+      }
+    }
+    split_commit();  // always (possibly empty): every iteration waits on the same group count
+  };
+#pragma unroll
+  for (int i = 0; i < ST - 1; ++i) issue(i, false);
+  pdl_wait();
+
+  // RoPE exactly as rope_attn_decode_kernel: x*cos + rotate_half(x)*sin, each product and the sum rounded to T
+  for (int i = tid; i < (G + 1) * kHd; i += kSplitThreads) {
+    const int h = i >> 7, d = i & (kHd - 1), half = kHd / 2;
+    const float c = to_f32<T>(cos_t[(long long)pos * kHd + d]), s = to_f32<T>(sin_t[(long long)pos * kHd + d]);
+    const T* x = h < G ? q_in + h * kHd : k_in;
+    const float xv = to_f32<T>(x[d]);
+    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
+    const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
+    if (h < G) {
+      qs[h * kHd + d] = r;
+    } else {
+      kf[d] = r;
+      vf[d] = v_in[d];
+    }
+  }
+  __syncthreads();
+  if (warp < 2) {  // warp 0 quantises the rotated k row, warp 1 the v row; split 0 writes them to the cache
+    const T* src = warp ? vf : kf;
+    float x[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) x[j] = to_f32<T>(src[4 * lane + j]);
+    T sc, ze;
+    const uint32_t q = kv8_quant4<T>(x, gs, sc, ze);
+    *reinterpret_cast<uint32_t*>(fq + warp * kHd + 4 * lane) = q;
+    const int grp = 4 * lane / gs;
+    if ((4 * lane) % gs == 0) { fm[4 * warp + grp] = sc; fm[4 * warp + 2 + grp] = ze; }
+    if (split == 0) {
+      *reinterpret_cast<uint32_t*>((warp ? v_q : k_q) + (long long)pos * kHd + 4 * lane) = q;
+      if ((4 * lane) % gs == 0) {
+        (warp ? v_s : k_s)[(long long)pos * ng + grp] = sc;
+        (warp ? v_z : k_z)[(long long)pos * ng + grp] = ze;
+      }
+    }
+  }
+  __syncthreads();
+  if (pos >= c0 && pos < c1) {  // row pos in a tile staged before the wait: its owner fills it in now
+    const int ti = (pos - c0) / kSplitTile, i = ti / NW;
+    if (ti % NW == warp && i < ST - 1) {
+      const int r = pos - (c0 + ti * kSplitTile);
+      char* st = ring + (i % ST) * kKv8StageBytes;
+      if (lane < 16) {
+        const int isv = lane >> 3, c = lane & 7;
+        *reinterpret_cast<uint4*>(st + isv * kKv8LvlBytes + swz8(r, c)) = *reinterpret_cast<const uint4*>(fq + isv * kHd + c * 16);
+      } else if (lane < 16 + 4 * ng) {
+        const int a = (lane - 16) / ng, e = (lane - 16) % ng;
+        reinterpret_cast<T*>(st + 2 * kKv8LvlBytes + a * kKv8MetaBytes)[r * ng + e] = fm[2 * a + e];
+      }
+    }
+  }
+  // Q^T fragments in the permuted dims: k slots 2 qd + {0, 1} / + {8, 9} of step kk are dims 32 qd + 4 kk + {0, 1} / + {2, 3}
+  uint32_t qb[8][2];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+    const T* qr = qs + g * kHd + 32 * qd + 4 * kk;
+    qb[kk][0] = g < G ? *reinterpret_cast<const uint32_t*>(qr) : 0u;
+    qb[kk][1] = g < G ? *reinterpret_cast<const uint32_t*>(qr + 2) : 0u;
+  }
+
+  float o[8][4];
+#pragma unroll
+  for (int mt = 0; mt < 8; ++mt) o[mt][0] = o[mt][1] = o[mt][2] = o[mt][3] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  const int gk = 32 * qd / gs, gv = 16 * g / gs;  // the group of the lane's K dims and of its V dims
+  for (int i = 0; i < my_tiles; ++i) {
+    __syncwarp();  // every lane is done with the slot the next issue overwrites
+    issue(i + ST - 1, true);
+    split_wait<ST - 1>();
+    __syncwarp();  // this tile's copies and plain stores of every lane are visible to the warp
+    const char* st = ring + (i % ST) * kKv8StageBytes;
+    const T* ms = reinterpret_cast<const T*>(st + 2 * kKv8LvlBytes);
+    constexpr int MA = kKv8MetaBytes / 2;  // T elements per meta array
+    float s[4] = {0.f, 0.f, 0.f, 0.f};
+    {
+      const uint4 ka0 = *reinterpret_cast<const uint4*>(st + swz8(g, 2 * qd)), ka1 = *reinterpret_cast<const uint4*>(st + swz8(g, 2 * qd + 1));
+      const uint4 kb0 = *reinterpret_cast<const uint4*>(st + swz8(g + 8, 2 * qd)), kb1 = *reinterpret_cast<const uint4*>(st + swz8(g + 8, 2 * qd + 1));
+      typename Pair<T>::type sa, sb, za, zb;  // rows g and g + 8, both halves alike
+      sa.x = sa.y = ms[g * ng + gk]; sb.x = sb.y = ms[(g + 8) * ng + gk];
+      za.x = za.y = ms[MA + g * ng + gk]; zb.x = zb.y = ms[MA + (g + 8) * ng + gk];
+      const uint32_t wa[8] = {ka0.x, ka0.y, ka0.z, ka0.w, ka1.x, ka1.y, ka1.z, ka1.w};
+      const uint32_t wb[8] = {kb0.x, kb0.y, kb0.z, kb0.w, kb1.x, kb1.y, kb1.z, kb1.w};
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        uint32_t a[4];
+        a[0] = kv8_deq2<T, 0>(wa[kk], za, sa);
+        a[2] = kv8_deq2<T, 1>(wa[kk], za, sa);
+        a[1] = kv8_deq2<T, 0>(wb[kk], zb, sb);
+        a[3] = kv8_deq2<T, 1>(wb[kk], zb, sb);
+        mma16816<T>(s, a, qb[kk][0], qb[kk][1]);
+      }
+    }
+    const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
+    const float x0 = p0 < c1 ? s[0] * scale_log2 : -INFINITY, x1 = p0 < c1 ? s[1] * scale_log2 : -INFINITY;
+    const float x2 = p0 + 8 < c1 ? s[2] * scale_log2 : -INFINITY, x3 = p0 + 8 < c1 ? s[3] * scale_log2 : -INFINITY;
+    float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
+#pragma unroll
+    for (int off = 4; off < 32; off <<= 1) {
+      t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
+      t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
+    }
+    const float n0 = fmaxf(m0, t0), n1 = fmaxf(m1, t1);  // finite: every tile holds position c0 + 16 j < c1
+    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
+    m0 = n0; m1 = n1;
+    const T p00 = from_f32<T>(exp2f(x0 - n0)), p01 = from_f32<T>(exp2f(x1 - n1));
+    const T p10 = from_f32<T>(exp2f(x2 - n0)), p11 = from_f32<T>(exp2f(x3 - n1));
+    l0 = l0 * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
+    l1 = l1 * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) { o[mt][0] *= a0; o[mt][1] *= a1; o[mt][2] *= a0; o[mt][3] *= a1; }
+    // P^T fragment (k = position, n = head g), as in rope_attn_decode_split_kernel
+    const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
+    const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
+    const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
+    const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
+    const uint32_t b0 = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
+    const uint32_t b1 = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
+    {
+      // V^T: positions r = 2 qd + {0, 1, 8, 9}, dims 16 g .. 16 g + 15 (one 16-byte chunk each)
+      const char* vt = st + kKv8LvlBytes;
+      const int r0 = 2 * qd;
+      const uint4 v0 = *reinterpret_cast<const uint4*>(vt + swz8(r0, g)), v1 = *reinterpret_cast<const uint4*>(vt + swz8(r0 + 1, g));
+      const uint4 v8 = *reinterpret_cast<const uint4*>(vt + swz8(r0 + 8, g)), v9 = *reinterpret_cast<const uint4*>(vt + swz8(r0 + 9, g));
+      const T* vs = ms + 2 * MA;
+      const T* vz = ms + 3 * MA;
+      typename Pair<T>::type s01, s89, z01, z89;  // positions r0, r0 + 1 and r0 + 8, r0 + 9
+      s01.x = vs[r0 * ng + gv]; s01.y = vs[(r0 + 1) * ng + gv];
+      s89.x = vs[(r0 + 8) * ng + gv]; s89.y = vs[(r0 + 9) * ng + gv];
+      z01.x = vz[r0 * ng + gv]; z01.y = vz[(r0 + 1) * ng + gv];
+      z89.x = vz[(r0 + 8) * ng + gv]; z89.y = vz[(r0 + 9) * ng + gv];
+      const uint32_t w0[4] = {v0.x, v0.y, v0.z, v0.w}, w1[4] = {v1.x, v1.y, v1.z, v1.w};
+      const uint32_t w8[4] = {v8.x, v8.y, v8.z, v8.w}, w9[4] = {v9.x, v9.y, v9.z, v9.w};
+#pragma unroll
+      for (int wi = 0; wi < 4; ++wi) {
+        // dims 16 g + 4 wi .. + 3 are bytes 0..3 of word wi; interleave the two positions of each pair: [p.b, p'.b, p.b+1, p'.b+1]
+        const uint32_t lo01 = prmt(w0[wi], w1[wi], 0x5140u), hi01 = prmt(w0[wi], w1[wi], 0x7362u);
+        const uint32_t lo89 = prmt(w8[wi], w9[wi], 0x5140u), hi89 = prmt(w8[wi], w9[wi], 0x7362u);
+        uint32_t a[4];
+        // step mt = 2 wi: dims 16 g + 4 wi (+ 1); step 2 wi + 1: dims 16 g + 4 wi + 2 (+ 3)
+        a[0] = kv8_deq2<T, 0>(lo01, z01, s01); a[1] = kv8_deq2<T, 1>(lo01, z01, s01);
+        a[2] = kv8_deq2<T, 0>(lo89, z89, s89); a[3] = kv8_deq2<T, 1>(lo89, z89, s89);
+        mma16816<T>(o[2 * wi], a, b0, b1);
+        a[0] = kv8_deq2<T, 0>(hi01, z01, s01); a[1] = kv8_deq2<T, 1>(hi01, z01, s01);
+        a[2] = kv8_deq2<T, 0>(hi89, z89, s89); a[3] = kv8_deq2<T, 1>(hi89, z89, s89);
+        mma16816<T>(o[2 * wi + 1], a, b0, b1);
+      }
+    }
+  }
+  split_wait<0>();
+#pragma unroll
+  for (int off = 4; off < 32; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][8][m, l, o[128]]
+  float* wp = reinterpret_cast<float*>(smem);
+  {
+    float* w0 = wp + (warp * kSplitMaxGroup + 2 * qd) * kPartFloats;
+    float* w1 = w0 + kPartFloats;
+    if (g == 0) { w0[0] = m0; w0[1] = l0; w1[0] = m1; w1[1] = l1; }
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) {  // O^T rows g, g + 8 of step mt are dims 16 g + 2 mt, 16 g + 2 mt + 1
+      w0[2 + 16 * g + 2 * mt] = o[mt][0]; w1[2 + 16 * g + 2 * mt] = o[mt][1];
+      w0[2 + 16 * g + 2 * mt + 1] = o[mt][2]; w1[2 + 16 * g + 2 * mt + 1] = o[mt][3];
+    }
+  }
+  __syncthreads();
+  split_merge<T>(wp, part, tickets, out, last, S, split, G, tid);
 }
 
 int split_count(int n_kv, int cache_len) {
@@ -618,6 +949,70 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
       const int kvh = h - n_q - n_kv;
       v_cache[((long long)kvh * L + p) * kHd + d] = v[kvh * kHd + d];
     }
+  }
+}
+
+// Prefill into an 8-bit cache: rope_append_rows_kernel's RoPE, then every k and v row quantised as the kv8 decode kernel quantises
+// row pos (the same levels and meta bit for bit), and its dequantisation written to the staging caches at the same row.
+// grid = (T, batch), block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position (k and v of each kv head).
+// Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.
+template <typename T>
+__global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
+                                                                   const T* __restrict__ cos_t, const T* __restrict__ sin_t, uint8_t* __restrict__ k_q,
+                                                                   T* __restrict__ k_s, T* __restrict__ k_z, uint8_t* __restrict__ v_q,
+                                                                   T* __restrict__ v_s, T* __restrict__ v_z, T* __restrict__ k_st, T* __restrict__ v_st,
+                                                                   T* __restrict__ q_out, int pos0, int n_tok, int n_q, int n_kv, int L, int gs) {
+  const int t = (int)blockIdx.x, b = (int)blockIdx.y, p = pos0 + t, ng = kHd / gs;
+  {
+    const long long row = (long long)b * n_tok + t, kv = (long long)b * n_kv;
+    q += row * n_q * kHd; q_out += row * n_q * kHd;
+    k += row * n_kv * kHd; v += row * n_kv * kHd;
+    k_q += kv * L * kHd; v_q += kv * L * kHd; k_st += kv * L * kHd; v_st += kv * L * kHd;
+    k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+  }
+  pdl_launch_dependents();
+  pdl_wait();
+  constexpr int half = kHd / 2;
+  for (int i = (int)threadIdx.x; i < n_q * kHd; i += (int)blockDim.x) {  // rope(q) as rope_append_rows_kernel
+    const int h = i >> 7, d = i & (kHd - 1);
+    const float c = to_f32<T>(cos_t[(long long)p * kHd + d]), s = to_f32<T>(sin_t[(long long)p * kHd + d]);
+    const T* x = q + h * kHd;
+    const float xv = to_f32<T>(x[d]);
+    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
+    q_out[h * kHd + d] = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
+  }
+  const int warp = (int)threadIdx.x >> 5, lane = (int)threadIdx.x & 31;
+  for (int r = warp; r < 2 * n_kv; r += (int)blockDim.x >> 5) {
+    const int kvh = r >> 1, isv = r & 1;
+    float x[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int d = 4 * lane + j;
+      if (isv) {
+        x[j] = to_f32<T>(v[kvh * kHd + d]);
+      } else {
+        const float c = to_f32<T>(cos_t[(long long)p * kHd + d]), s = to_f32<T>(sin_t[(long long)p * kHd + d]);
+        const T* xk = k + kvh * kHd;
+        const float xv = to_f32<T>(xk[d]);
+        const float xr = (d < half) ? -to_f32<T>(xk[d + half]) : to_f32<T>(xk[d - half]);
+        x[j] = to_f32<T>(from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s))));
+      }
+    }
+    T sc, ze;
+    const uint32_t lv = kv8_quant4<T>(x, gs, sc, ze);
+    const long long row = (long long)kvh * L + p;
+    *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + row * kHd + 4 * lane) = lv;
+    if ((4 * lane) % gs == 0) {
+      (isv ? v_s : k_s)[row * ng + 4 * lane / gs] = sc;
+      (isv ? v_z : k_z)[row * ng + 4 * lane / gs] = ze;
+    }
+    typename Pair<T>::type s2, z2;
+    s2.x = s2.y = sc;
+    z2.x = z2.y = ze;
+    uint2 y;
+    y.x = kv8_deq2<T, 0>(lv, z2, s2);
+    y.y = kv8_deq2<T, 1>(lv, z2, s2);
+    *reinterpret_cast<uint2*>((isv ? v_st : k_st) + row * kHd + 4 * lane) = y;
   }
 }
 
@@ -1003,6 +1398,59 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k
   }
   set_error("hqq_b200_glue_rope_attn_decode_split: dtype must be f16/bf16");
   return HQQ_E_INVALID;
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                        const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
+                                                        int head_dim, int group_size, int batch, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_attn_decode_split_kv8";
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && pos && out && workspace, HQQ_E_INVALID,
+              "%s: null pointer", name);
+  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
+  HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0 && ((uintptr_t)k_q & 15) == 0 && ((uintptr_t)v_q & 15) == 0, HQQ_E_INVALID,
+              "%s: workspace must be 4-byte and the level caches 16-byte aligned", name);
+  HQQ_REQUIRE(head_dim == kHd && n_kv_heads > 0 && n_kv_heads <= 65535 && n_q_heads % n_kv_heads == 0 && n_q_heads / n_kv_heads >= 1 &&
+                  n_q_heads / n_kv_heads <= kSplitMaxGroup && cache_len > 0 && cache_len <= kSplitMaxLen && (group_size == 64 || group_size == 128),
+              HQQ_E_UNSUPPORTED, "%s: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072, group_size 64 or 128", name);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int S = split_count(n_kv_heads, cache_len);
+  const int G = n_q_heads / n_kv_heads;
+  const size_t part_bytes = (size_t)batch * n_kv_heads * max(1, sm_count() / n_kv_heads) * G * kPartFloats * sizeof(float);
+  float* part = (float*)workspace;
+  unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
+  const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    if (int rc = reserve_smem<rope_attn_decode_split_kv8_kernel<E>>(kKv8SmemBytes)) return rc;
+    return launch_pdl("rope_attn_decode_split_kv8", rope_attn_decode_split_kv8_kernel<E>, grid, dim3(kSplitThreads), kKv8SmemBytes, st, (const E*)q,
+                      (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q,
+                      (E*)v_scale, (E*)v_zero, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, group_size, scale_log2);
+  };
+  if (dtype == HQQ_F16) return go(__half());
+  if (dtype == HQQ_BF16) return go(__nv_bfloat16());
+  set_error("%s: dtype must be f16/bf16", name);
+  return HQQ_E_INVALID;
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_q,
+                                                  void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage, void* v_stage,
+                                                  void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                  int group_size, int batch, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_kv8";
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
+              HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = prefill_args(name, pos0, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
+  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows_kv8", rope_append_rows_kv8_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q,
+                      (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q,
+                      (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0, T, n_q_heads, n_kv_heads, cache_len, group_size);
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache,

@@ -37,34 +37,11 @@ struct SolverArgs {
   double* partial;  // [gridDim.x][iters]
 };
 
-__device__ __forceinline__ float rint_magic(float t) {
-  // round-half-even for |t| < 2^22; beyond that the result is still >= 2^22-ish in magnitude with the
-  // right sign, so the clamp that always follows yields the same level as rintf would.
-  return __fsub_rn(__fadd_rn(t, 12582912.0f), 12582912.0f);
-}
-
-struct GroupState {
-  float s, rs, z;
-};
-
 __device__ __forceinline__ void init_group_ext(const SolverArgs& a, long long g, bool valid, GroupState& st) {
   const float s = valid ? a.s_init[g] : 1.0f;
   st.s = s;
   st.rs = __frcp_rn(s);
   st.z = valid ? a.z_init[g] : 0.0f;
-}
-
-__device__ __forceinline__ void init_group(float mn, float mx, int maxv, int round_zero, GroupState& st) {
-  // quantize.py:126-134 ; `max_v / denom` is reciprocal(denom) * max_v in torch (two roundings)
-  float denom = __fsub_rn(mx, mn);
-  float s = __fmul_rn(__frcp_rn(denom), (float)maxv);
-  if (fabsf(denom) <= 1e-4f) s = 1.0f;
-  s = fminf(s, 2e4f);
-  float z = __fmul_rn(-mn, s);
-  if (round_zero) z = rintf(z);
-  st.s = s;
-  st.rs = __frcp_rn(s);
-  st.z = z;
 }
 
 // Group mean of the zero-point terms: float64 accumulation (the terms are float32 values of magnitude <= 2^nbits, so the sum of a
@@ -459,8 +436,7 @@ __global__ void __launch_bounds__(256) quant_pack_kernel(const TIn* __restrict__
           // optimize.py:254 / quantize.py:147: round(W*scale + zero).clamp(min,max); mul and add round separately
           // rint and the float -> int conversion as float adds (ncu: this kernel was bound by the conversion pipe): below 2^22
           // rint_magic is rintf, beyond it the clamp decides alike; a clamped level (0 .. 255) + 1.5 * 2^23 carries it in its low bits
-          float t = rint_magic(__fadd_rn(__fmul_rn(to_f32<TIn>(w.v[j]), s[j]), z[j]));
-          t = fminf(fmaxf(t, 0.0f), (float)maxv);
+          const float t = quant_level(to_f32<TIn>(w.v[j]), s[j], z[j], (float)maxv);
           const uint32_t q = __float_as_uint(__fadd_rn(t, 12582912.0f)) & 0xFFu;
           o.v[j] = (typename P::T)((uint32_t)o.v[j] | (q << P::shift(f)));
         }

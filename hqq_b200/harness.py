@@ -84,6 +84,34 @@ def rope_tables(shape: LlamaShape, cache_len: int, dtype, device):
     return torch.cat([fr.cos(), fr.cos()], dim=-1).to(dtype), torch.cat([fr.sin(), fr.sin()], dim=-1).to(dtype)
 
 
+def kv8_quantize_rows(x: torch.Tensor, group_size: int):
+    """The 8-bit KV cache format on framework ops: rows x [..., 128] in T -> levels uint8 [..., 128] and scale, zero
+    [..., 128 / group_size] in T.  HQQ's Quantizer.quantize(row, nbits=8, group_size, axis=1, optimize=False) (round_zero off, as for
+    8-bit layers) in fp32 -- inverse scale reciprocal(max - min) * 255 (1 where max - min <= 1e-4, at most 2e4), zero -min * s,
+    levels round(x * s + z) clamped to [0, 255] with the product and the sum rounded separately -- then scale = 1 / s and the zero
+    cast to T.  The solver is not run: its early stop compares a mean over the whole tensor, so a row's levels would depend on
+    which rows were quantised with it."""
+    shape = x.shape
+    w = x.float().reshape(-1, group_size)
+    mn, mx = w.amin(dim=1, keepdim=True), w.amax(dim=1, keepdim=True)
+    denom = mx - mn
+    s = torch.reciprocal(denom) * 255.0
+    s = torch.where(denom.abs() <= 1e-4, torch.ones_like(s), s)
+    s = torch.clamp(s, max=2e4)
+    z = -mn * s
+    q = torch.clamp(torch.round(w * s + z), 0, 255).to(torch.uint8)
+    meta = shape[:-1] + (shape[-1] // group_size,)
+    return q.reshape(shape), torch.reciprocal(s).to(x.dtype).reshape(meta), z.to(x.dtype).reshape(meta)
+
+
+def kv8_dequantize(q: torch.Tensor, scale: torch.Tensor, zero: torch.Tensor) -> torch.Tensor:
+    """Rows of the 8-bit KV cache back in T: (T(q) - zero) * scale with one rounding to T per operation (hqq_b200_dequantize,
+    Quantizer.dequantize).  q [..., 128] uint8, scale / zero [..., 128 / group_size] in T."""
+    ng = scale.shape[-1]
+    qs = q.reshape(q.shape[:-1] + (ng, q.shape[-1] // ng)).to(scale.dtype)
+    return ((qs - zero.unsqueeze(-1)) * scale.unsqueeze(-1)).reshape(q.shape)
+
+
 def shard_dims(shape: LlamaShape, tp: int):
     """Per-rank sizes of the sharded projections (pure host logic, unit-tested on CPU)."""
     if shape.n_heads % tp or shape.n_kv_heads % tp or shape.inter % tp:
@@ -98,8 +126,17 @@ def shard_dims(shape: LlamaShape, tp: int):
 class DecodeModel:
     def __init__(self, shape: LlamaShape = LLAMA3_8B, nbits: int = 4, group_size: int = 64, dtype=torch.float16,
                  device="cuda", cache_len: int = 256, tp: int = 1, rank: int = 0, seed: int = 0, process_group=None,
-                 n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False):
+                 n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
+                 kv_bits: int = 16, kv_group_size: int = 64):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
+        # kv_bits 8: every layer's K and V cache in HQQ's 8-bit format (kv8_quantize_rows), groups of kv_group_size along the head dim
+        if kv_bits not in (16, 8):
+            raise ValueError(f"kv_bits must be 16 or 8 (got {kv_bits!r})")
+        if kv_group_size not in (64, 128):
+            raise ValueError(f"kv_group_size must be 64 or 128 (got {kv_group_size!r})")
+        if kv_bits == 8 and shape.head_dim != 128:
+            raise ValueError("kv_bits=8 needs head_dim 128")
+        self.kv_bits, self.kv_group_size = int(kv_bits), int(kv_group_size)
         # batch > 1 (BASELINE configs[4], bs = 32): `batch` sequences decode in lock-step at the same position; the linears then
         # run the small-M kernel (M = batch <= 32; the wgmma kernel from 17 sequences on large matrices) between the batched glue
         # kernels -- the one-token kernels and their NVLink exchange are M = 1 only, so tensor-parallel partials are summed by NCCL
@@ -163,9 +200,14 @@ class DecodeModel:
             blk["norm1"] = torch.ones(shape.hidden, device=self.device, dtype=dtype)
             blk["norm2"] = torch.ones(shape.hidden, device=self.device, dtype=dtype)
             hkv = shape.n_kv_heads // tp
-            blk["k_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=dtype)
-            blk["v_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=dtype)
+            cdt = torch.uint8 if self.kv_bits == 8 else dtype
+            blk["k_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=cdt)
+            blk["v_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=cdt)
+            if self.kv_bits == 8:
+                for name in ("k_scale", "k_zero", "v_scale", "v_zero"):
+                    blk[name] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim // kv_group_size, device=self.device, dtype=dtype)
             self.blocks.append(blk)
+        self._kv8_stage = None  # kv_bits 8: dequantised fp16 / bf16 K and V for the prefill attention, allocated by the first fused prefill
         self.cos, self.sin = rope_tables(shape, cache_len, dtype, self.device)  # [cache_len, hd]
         self.arange = torch.arange(cache_len, device=self.device)
         # static I/O for graph capture
@@ -177,12 +219,26 @@ class DecodeModel:
 
     @property
     def attn_kernel(self) -> str:
-        """Attention kernel of the fused steps: "single" (one CTA per query head, cache_len <= 8192) or "split" (split-KV)."""
+        """Attention kernel of the fused steps: "single" (one CTA per query head, cache_len <= 8192), "split" (split-KV) or
+        "split_kv8" (split-KV over the 8-bit cache, at every cache_len)."""
+        if self.kv_bits == 8:
+            return "split_kv8"
         return "split" if self.cache_len > SINGLE_ATTN_MAX_LEN else "single"
+
+    def kv_cache_bytes(self) -> int:
+        """Bytes of every layer's KV cache on this rank: fp16 / bf16 rows, or levels plus scale and zero with kv_bits 8."""
+        names = ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero")
+        return sum(blk[n].numel() * blk[n].element_size() for blk in self.blocks for n in names if n in blk)
 
     def _attn_split(self, lib, blk, hq, hkv, code, st):
         from ._lib import check, ptr
         b = self._bufs
+        if self.kv_bits == 8:
+            check(lib.hqq_b200_glue_rope_attn_decode_split_kv8(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                               ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
+                                                               ptr(blk["v_zero"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
+                                                               self.shape.head_dim, self.kv_group_size, self.batch, code, st))
+            return
         check(lib.hqq_b200_glue_rope_attn_decode_split(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
                                                        ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
                                                        self.shape.head_dim, self.batch, code, st))
@@ -223,9 +279,14 @@ class DecodeModel:
             q, k, v = q.view(B, hq, hd), k.view(B, hkv, hd), v.view(B, hkv, hd)
             q = self._rope(q, cos, sin)
             k = self._rope(k, cos, sin)
-            blk["k_cache"].index_copy_(2, self.pos, k.view(B, hkv, 1, hd))
-            blk["v_cache"].index_copy_(2, self.pos, v.view(B, hkv, 1, hd))
-            a = F.scaled_dot_product_attention(q.view(B, hq, 1, hd), blk["k_cache"], blk["v_cache"], attn_mask=mask, enable_gqa=True)
+            if self.kv_bits == 8:  # the rotated rows quantised into the cache; attention over the dequantised cache
+                self._kv8_write(blk, k.view(B, hkv, 1, hd), v.view(B, hkv, 1, hd), self.pos)
+                kc, vc = self._kv8_read(blk, self.cache_len)
+            else:
+                blk["k_cache"].index_copy_(2, self.pos, k.view(B, hkv, 1, hd))
+                blk["v_cache"].index_copy_(2, self.pos, v.view(B, hkv, 1, hd))
+                kc, vc = blk["k_cache"], blk["v_cache"]
+            a = F.scaled_dot_product_attention(q.view(B, hq, 1, hd), kc, vc, attn_mask=mask, enable_gqa=True)
             o = blk["o"](a.reshape(B, hq * hd))
             if self.tp > 1:
                 torch.distributed.all_reduce(o, group=self.pg)
@@ -248,6 +309,18 @@ class DecodeModel:
         else:
             self.next_tok.copy_(torch.argmax(logits, dim=-1))
         self.pos.add_(1).remainder_(self.cache_len)
+
+    def _kv8_write(self, blk, k, v, idx):
+        """kv_bits 8 on framework ops: rows k, v [batch, n_kv, n, 128] quantised into cache positions idx [n]."""
+        for name, x in (("k", k), ("v", v)):
+            lv, sc, ze = kv8_quantize_rows(x, self.kv_group_size)
+            blk[name + "_cache"].index_copy_(2, idx, lv)
+            blk[name + "_scale"].index_copy_(2, idx, sc)
+            blk[name + "_zero"].index_copy_(2, idx, ze)
+
+    def _kv8_read(self, blk, end):
+        """kv_bits 8 on framework ops: the dequantised K and V cache rows [0, end)."""
+        return tuple(kv8_dequantize(blk[n + "_cache"][:, :, :end], blk[n + "_scale"][:, :, :end], blk[n + "_zero"][:, :, :end]) for n in ("k", "v"))
 
     def _head(self, lib, x, code, st):
         """Final projection + greedy pick inside the captured step: fp16 lm_head through the library GEMV (it is not an HQQ
@@ -311,7 +384,7 @@ class DecodeModel:
         for blk in self.blocks:
             norm(delta, blk["norm1"])
             self._lin(b["x"], (blk["q"], blk["k"], blk["v"]), [b["q"], b["k"], b["v"]])
-            if self.attn_kernel == "split":
+            if self.attn_kernel != "single":
                 self._attn_split(lib, blk, hq, hkv, code, st)
             else:
                 check(lib.hqq_b200_glue_rope_attn_decode_batch(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
@@ -391,7 +464,7 @@ class DecodeModel:
             ok &= ops.decode_linear_fwd(h_cur, (blk["q"], blk["k"], blk["v"]), [b["q"], b["k"], b["v"]], 1, None if p2p else delta, blk["norm1"], h_nxt,
                                         s.rms_eps, tpx=(self._tpx(bi - 1, red_data=d_loc) if (p2p and bi > 0) else None))
             h_cur, h_nxt = h_nxt, h_cur
-            if self.attn_kernel == "split":
+            if self.attn_kernel != "single":
                 self._attn_split(lib, blk, hq, hkv, code, st)
             else:
                 check(lib.hqq_b200_glue_rope_attn_decode(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
@@ -437,7 +510,12 @@ class DecodeModel:
         down.  fused=False: the same walk on framework ops (F.rms_norm, the layers, torch RoPE, F.scaled_dot_product_attention
         with a causal mask over the cache), the correctness reference as step() is for decode.  With tensor parallelism the two
         row-parallel outputs and the head's argmax keys meet in NCCL all-reduces; the peer-memory exchange of fused=5 decode and
-        its step counter are not touched."""
+        its step counter are not touched.
+
+        kv_bits 8: the rows kernel quantises k and v into the 8-bit cache as the decode kernel does and writes their dequantisation
+        into a staging pair [batch, n_kv, cache_len, 128] in T (allocated once, shared by all layers); staging rows [0, start of the
+        chunk) are dequantised from the cache per layer and chunk (hqq_b200_dequantize), and the attention kernel reads the staging
+        pair.  fused=False quantises into the cache and attends over its dequantisation."""
         s, B = self.shape, self.batch
         tokens = torch.as_tensor(tokens, device=self.device)
         if tokens.dim() == 1 and B == 1:
@@ -480,13 +558,31 @@ class DecodeModel:
         gate, up, act, down = e(inter), e(inter), e(inter), e(s.hidden)
         norm = lambda d, w: check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(d), ptr(w), ptr(x), M, s.hidden, s.rms_eps, code, st))
         delta = None
+        kv8 = self.kv_bits == 8
+        if kv8 and self._kv8_stage is None:  # one staging pair for all layers: [batch, n_kv, cache_len, 128] each
+            self._kv8_stage = tuple(torch.zeros(B, hkv, self.cache_len, hd, device=self.device, dtype=self.dtype) for _ in range(2))
         for blk in self.blocks:
             norm(delta, blk["norm1"])
             self._lin(x, (blk["q"], blk["k"], blk["v"]), [q, k, v])
-            check(lib.hqq_b200_glue_rope_append_rows(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
-                                                     ptr(qr), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
-            check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(blk["k_cache"]), ptr(blk["v_cache"]), ptr(a), p0, n, hq, hkv, self.cache_len, hd, B,
-                                                 code, st))
+            if kv8:
+                # staging rows [0, p0) dequantised from the 8-bit cache, rows [p0, p0 + n) written by the rows kernel; the attention
+                # kernel is the one of the fp16 cache, reading the staging pair
+                kst, vst = self._kv8_stage
+                for bi in range(B):
+                    for hh in range(hkv):
+                        for c, dst in (("k", kst), ("v", vst)):
+                            if p0 > 0:
+                                check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][bi, hh]), ptr(blk[c + "_scale"][bi, hh]), ptr(blk[c + "_zero"][bi, hh]),
+                                                              ptr(dst[bi, hh]), p0, hd, self.kv_group_size, 8, 1, code, st))
+                check(lib.hqq_b200_glue_rope_append_rows_kv8(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]),
+                                                             ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(kst),
+                                                             ptr(vst), ptr(qr), p0, n, hq, hkv, self.cache_len, hd, self.kv_group_size, B, code, st))
+                kc, vc = kst, vst
+            else:
+                check(lib.hqq_b200_glue_rope_append_rows(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
+                                                         ptr(qr), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
+                kc, vc = blk["k_cache"], blk["v_cache"]
+            check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(kc), ptr(vc), ptr(a), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
             self._lin(a, (blk["o"],), [o])
             if self.tp > 1:
                 torch.distributed.all_reduce(o, group=self.pg)
@@ -516,10 +612,14 @@ class DecodeModel:
             q, k, v = self._multi(x, (blk["q"], blk["k"], blk["v"]))
             q = self._rope(q.view(B, n, hq, hd), cos, sin)
             k = self._rope(k.view(B, n, hkv, hd), cos, sin)
-            blk["k_cache"][:, :, p0:end] = k.transpose(1, 2)
-            blk["v_cache"][:, :, p0:end] = v.view(B, n, hkv, hd).transpose(1, 2)
-            a = F.scaled_dot_product_attention(q.transpose(1, 2), blk["k_cache"][:, :, :end], blk["v_cache"][:, :, :end], attn_mask=mask,
-                                               enable_gqa=True)
+            if self.kv_bits == 8:
+                self._kv8_write(blk, k.transpose(1, 2), v.view(B, n, hkv, hd).transpose(1, 2), torch.arange(p0, end, device=self.device))
+                kc, vc = self._kv8_read(blk, end)
+            else:
+                blk["k_cache"][:, :, p0:end] = k.transpose(1, 2)
+                blk["v_cache"][:, :, p0:end] = v.view(B, n, hkv, hd).transpose(1, 2)
+                kc, vc = blk["k_cache"][:, :, :end], blk["v_cache"][:, :, :end]
+            a = F.scaled_dot_product_attention(q.transpose(1, 2), kc, vc, attn_mask=mask, enable_gqa=True)
             o = blk["o"](a.transpose(1, 2).reshape(M, hq * hd))
             if self.tp > 1:
                 torch.distributed.all_reduce(o, group=self.pg)
@@ -572,7 +672,7 @@ class DecodeModel:
                       "v": z(s.n_kv_heads // tp * s.head_dim), "a": z(s.n_heads // tp * s.head_dim), "o": z(s.hidden),
                       "gate": z(s.inter // tp), "up": z(s.inter // tp), "act": z(s.inter // tp), "down": z(s.hidden), "logits": z(self.vocab_shard),
                       "key": torch.zeros(1, dtype=torch.long, device=dev)}
-        if self.attn_kernel == "split":  # partials + tickets, zeroed once: every launch leaves the tickets at zero
+        if self.attn_kernel != "single":  # partials + tickets, zeroed once: every launch leaves the tickets at zero
             from ._lib import load
             with torch.cuda.device(dev):
                 nbytes = load().hqq_b200_glue_rope_attn_decode_split_workspace_bytes(s.n_heads // tp, s.n_kv_heads // tp, s.head_dim, self.batch)
@@ -604,8 +704,9 @@ class DecodeModel:
         self.tok.fill_(token)
         self.pos.zero_()
         for blk in self.blocks:
-            blk["k_cache"].zero_()
-            blk["v_cache"].zero_()
+            for name in ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero"):
+                if name in blk:
+                    blk[name].zero_()
         if hasattr(self, "_bufs"):
             for t in self._bufs.values():
                 t.zero_()

@@ -254,8 +254,22 @@ int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const voi
                                          void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace,
                                          int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                          int batch, int dtype, void* stream);
-/* Workspace bytes of hqq_b200_glue_rope_attn_decode_split on the current device (0 for invalid head counts). */
+/* Workspace bytes of hqq_b200_glue_rope_attn_decode_split on the current device (0 for invalid head counts).  The same
+ * workspace serves hqq_b200_glue_rope_attn_decode_split_kv8. */
 size_t hqq_b200_glue_rope_attn_decode_split_workspace_bytes(int n_q_heads, int n_kv_heads, int head_dim, int batch);
+/* hqq_b200_glue_rope_attn_decode_split over an 8-bit HQQ KV cache: the same grid, split count, merge order, workspace and RoPE
+ * rounding.  A cache row of one kv head is Quantizer.quantize(row, nbits=8, group_size, axis=1, optimize=False) with the meta cast to
+ * dtype: k_q / v_q uint8 [batch, n_kv_heads, cache_len, head_dim] (16-byte aligned), k_scale / k_zero / v_scale / v_zero
+ * [batch, n_kv_heads, cache_len, head_dim / group_size] in dtype, and the attended row is (q - zero) * scale with one rounding to
+ * dtype per operation, as hqq_b200_dequantize computes it.  Row *pos is quantised from rope(k) and v in this launch and written
+ * there; every attended row, row *pos included, is the dequantised row, so the output is attention over exactly the cache the next
+ * step reads.  group_size 64 or 128; the other limits and the precondition on *pos are those of hqq_b200_glue_rope_attn_decode_split. */
+int hqq_b200_glue_rope_attn_decode_split_kv8(const void* q, const void* k, const void* v,
+                                             const void* cos_table, const void* sin_table,
+                                             void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                             const int64_t* pos, void* out, void* workspace,
+                                             int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                             int batch, int dtype, void* stream);
 /* Prompt prefill, step 1: a chunk of T positions pos0 .. pos0 + T - 1 of `batch` sequences.  q [batch*T, n_q_heads*head_dim],
  * k / v [batch*T, n_kv_heads*head_dim] as the q/k/v linears produce them (token row b*T + t); caches [batch, n_kv_heads, cache_len,
  * head_dim].  Writes rope(k) and v into cache rows [pos0, pos0 + T) and rope(q) into q_out (same layout as q).  RoPE rounds as
@@ -268,6 +282,17 @@ int hqq_b200_glue_rope_append_rows(const void* q, const void* k, const void* v,
                                    void* k_cache, void* v_cache, void* q_out, int pos0, int T,
                                    int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                    int batch, int dtype, void* stream);
+/* hqq_b200_glue_rope_append_rows for an 8-bit cache (see hqq_b200_glue_rope_attn_decode_split_kv8 for the format): q_out as
+ * hqq_b200_glue_rope_append_rows writes it, bit for bit; rope(k) and v of rows [pos0, pos0 + T) quantised into the levels and meta
+ * exactly as the decode kernel quantises row *pos; and their dequantised rows written to k_stage / v_stage
+ * [batch, n_kv_heads, cache_len, head_dim] in dtype at the same rows, for hqq_b200_glue_attn_prefill to read.  group_size 64 or 128;
+ * other limits as hqq_b200_glue_rope_append_rows. */
+int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, const void* v,
+                                       const void* cos_table, const void* sin_table,
+                                       void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                       void* k_stage, void* v_stage, void* q_out, int pos0, int T,
+                                       int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                       int batch, int dtype, void* stream);
 /* Prompt prefill, step 2: causal GQA attention of the chunk's queries over the cache.  Query t (row b*T + t of q_rot, rotated as
  * hqq_b200_glue_rope_append_rows leaves it) sits at position pos0 + t and attends to cache rows 0 .. pos0 + t; out has the layout
  * of q_rot, ready for o_proj.  Cache rows at or past pos0 + T are never read.  A row's output depends only on its q row and cache

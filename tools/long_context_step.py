@@ -5,8 +5,11 @@ caches filled with random rows so no prompt has to be decoded.  For each positio
     bytes = 2 n_kv (pos + 1) 128 * 2 (K and V rows read) + q / k / v / out, against the 3.35 TB/s data sheet,
   - at pos 8191 also the one-CTA-per-head kernel on cache_len 8192 caches, the same way,
   - the GPU name, power limit and median SM clock over the run (read-only nvidia-smi queries).
+With --kv-bits 16,8 one model per cache kind is built in the same process and the kinds alternate at every position; for the 8-bit
+cache (HQQ 8-bit rows, groups of --kv-group-size) the attention bytes are levels plus scale and zero.  kv_cache_bytes() of each
+model is printed first.
 
-    python tools/long_context_step.py [--steps 50] [--positions 1024,8191,...]"""
+    python tools/long_context_step.py [--steps 50] [--positions 1024,8191,...] [--kv-bits 16,8]"""
 import argparse
 import json
 import os
@@ -60,69 +63,89 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--positions", default="1024,8191,16384,32768,65536,131000")
     ap.add_argument("--cache-len", type=int, default=131072)
+    ap.add_argument("--kv-bits", default="16")
+    ap.add_argument("--kv-group-size", type=int, default=64)
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     info = gpu_info()
     shape = harness.LLAMA31_8B
-    model = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=args.cache_len, fused=5)
-    model.capture(warmup=2)
-    g = torch.Generator(device=dev).manual_seed(1)
-    for blk in model.blocks:
-        for name in ("k_cache", "v_cache"):
-            c = blk[name]
-            for i in range(0, c.shape[2], 16384):
-                c[:, :, i:i + 16384].copy_(torch.randn(c[:, :, i:i + 16384].shape, generator=g, device=dev) * 0.5)
-    lib, code = load(), DTYPE_CODE[model.dtype]
+    lib = load()
     hd, hq, hkv = shape.head_dim, shape.n_heads, shape.n_kv_heads
-    b = model._bufs
-    for t in (b["q"], b["k"], b["v"]):
-        t.copy_(torch.randn(t.shape, generator=g, device=dev))
+    g = torch.Generator(device=dev).manual_seed(1)
+    models = {}
+    for kb in [int(x) for x in args.kv_bits.split(",")]:
+        model = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=args.cache_len, fused=5, kv_bits=kb,
+                                    kv_group_size=args.kv_group_size)
+        model.capture(warmup=2)
+        for blk in model.blocks:
+            for n in ("k", "v"):
+                c = blk[n + "_cache"]
+                for i in range(0, c.shape[2], 16384):
+                    rows = torch.randn(c[:, :, i:i + 16384].shape, generator=g, device=dev, dtype=torch.float32).mul_(0.5).half()
+                    if kb == 8:
+                        lv, sc, ze = harness.kv8_quantize_rows(rows, args.kv_group_size)
+                        c[:, :, i:i + 16384].copy_(lv)
+                        blk[n + "_scale"][:, :, i:i + 16384].copy_(sc)
+                        blk[n + "_zero"][:, :, i:i + 16384].copy_(ze)
+                    else:
+                        c[:, :, i:i + 16384].copy_(rows)
+                    del rows
+        for t in (model._bufs["q"], model._bufs["k"], model._bufs["v"]):
+            t.copy_(torch.randn(t.shape, generator=g, device=dev))
+        models[kb] = model
+        print(json.dumps({"kv_bits": kb, "kv_group_size": args.kv_group_size if kb == 8 else None, "kv_cache_bytes": model.kv_cache_bytes(), **info}),
+              flush=True)
+    code = DTYPE_CODE[torch.float16]
     small = None
     sampler = ClockSampler(0)
     sampler.start()
     for pos in [int(p) for p in args.positions.split(",")]:
         pos = min(pos, args.cache_len - args.steps - 2)
-        model.tok.fill_(7)
-        model.pos.fill_(pos)
-        for _ in range(3):
-            model.decode()
-        model.pos.fill_(pos)
-        torch.cuda.synchronize(dev)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(args.steps):
-            model.decode()
-        e1.record()
-        torch.cuda.synchronize(dev)
-        step_ms = e0.elapsed_time(e1) / args.steps
-        # the attention launches of all 32 layers in one graph, at this position
-        model.pos.fill_(pos)
-        def split():  # the stream is read at call time: under capture it is the capturing stream
-            for blk in model.blocks:
-                model._attn_split(lib, blk, hq, hkv, code, stream_ptr(dev))
-        ms = time_graph(dev, split) / len(model.blocks)
-        nbytes = 2 * hkv * (pos + 1) * hd * 2 + (2 * hq + 2 * hkv) * hd * 2
-        line = {"pos": pos, "cache_len": args.cache_len, "step_ms": round(step_ms, 4), "tok_s": round(1e3 / step_ms, 2),
-                "steps_timed": args.steps, "attn_kernel": model.attn_kernel, "attn_us_per_launch": round(ms * 1e3, 2),
-                "attn_GBps": round(nbytes / ms / 1e6, 1), "attn_frac_of_3350": round(nbytes / ms / 1e6 / HBM_GBS, 3),
-                "attn_bytes_per_launch": nbytes, "kv_bytes_per_step": 32 * nbytes}
-        if pos == 8191:  # the one-CTA-per-head kernel on cache_len 8192 caches, same position, same graph timing
-            if small is None:
-                small = [(torch.randn(1, hkv, 8192, hd, generator=g, device=dev).half(), torch.randn(1, hkv, 8192, hd, generator=g, device=dev).half())
-                         for _ in model.blocks]
-            cos8, sin8 = model.cos[:8192].contiguous(), model.sin[:8192].contiguous()
+        for kb, model in models.items():
+            b = model._bufs
+            model.tok.fill_(7)
+            model.pos.fill_(pos)
+            for _ in range(3):
+                model.decode()
+            model.pos.fill_(pos)
+            torch.cuda.synchronize(dev)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(args.steps):
+                model.decode()
+            e1.record()
+            torch.cuda.synchronize(dev)
+            step_ms = e0.elapsed_time(e1) / args.steps
+            # the attention launches of all 32 layers in one graph, at this position
+            model.pos.fill_(pos)
 
-            def single():
-                for kc, vc in small:
-                    check(lib.hqq_b200_glue_rope_attn_decode(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(cos8), ptr(sin8), ptr(kc), ptr(vc),
-                                                             ptr(model.pos), ptr(b["a"]), hq, hkv, 8192, hd, code, stream_ptr(dev)))
-            ms1 = time_graph(dev, single) / len(small)
-            line["single_us_per_launch"] = round(ms1 * 1e3, 2)
-            line["single_GBps"] = round(nbytes / ms1 / 1e6, 1)
-            line["split_speedup"] = round(ms1 / ms, 2)
-        line.update(info)
-        print(json.dumps(line), flush=True)
+            def split(model=model):  # the stream is read at call time: under capture it is the capturing stream
+                for blk in model.blocks:
+                    model._attn_split(lib, blk, hq, hkv, code, stream_ptr(dev))
+            ms = time_graph(dev, split) / len(model.blocks)
+            row = hd * 2 if kb == 16 else hd + 4 * (hd // args.kv_group_size)  # bytes of one cached row of one kv head
+            nbytes = 2 * hkv * (pos + 1) * row + (2 * hq + 2 * hkv) * hd * 2
+            line = {"pos": pos, "kv_bits": kb, "cache_len": args.cache_len, "step_ms": round(step_ms, 4), "tok_s": round(1e3 / step_ms, 2),
+                    "steps_timed": args.steps, "attn_kernel": model.attn_kernel, "attn_us_per_launch": round(ms * 1e3, 2),
+                    "attn_GBps": round(nbytes / ms / 1e6, 1), "attn_frac_of_3350": round(nbytes / ms / 1e6 / HBM_GBS, 3),
+                    "attn_bytes_per_launch": nbytes, "kv_bytes_per_step": 32 * nbytes}
+            if pos == 8191 and kb == 16 and model.attn_kernel == "split":  # the one-CTA-per-head kernel on cache_len 8192 caches
+                if small is None:
+                    small = [(torch.randn(1, hkv, 8192, hd, generator=g, device=dev).half(), torch.randn(1, hkv, 8192, hd, generator=g, device=dev).half())
+                             for _ in model.blocks]
+                cos8, sin8 = model.cos[:8192].contiguous(), model.sin[:8192].contiguous()
+
+                def single(model=model, b=b, cos8=cos8, sin8=sin8):
+                    for kc, vc in small:
+                        check(lib.hqq_b200_glue_rope_attn_decode(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(cos8), ptr(sin8), ptr(kc), ptr(vc),
+                                                                 ptr(model.pos), ptr(b["a"]), hq, hkv, 8192, hd, code, stream_ptr(dev)))
+                ms1 = time_graph(dev, single) / len(small)
+                line["single_us_per_launch"] = round(ms1 * 1e3, 2)
+                line["single_GBps"] = round(nbytes / ms1 / 1e6, 1)
+                line["split_speedup"] = round(ms1 / ms, 2)
+            line.update(info)
+            print(json.dumps(line), flush=True)
     clocks = sampler.stop()
     print(json.dumps({"clocks": clocks, **info}), flush=True)
 

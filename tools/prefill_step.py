@@ -7,8 +7,12 @@ prompt length it prints one JSON line with
     T, 128], k / v expanded to 32 heads; the same positions attended, so the same FLOPs),
   - the GPU name, power limit and median SM clock over the run (read-only nvidia-smi queries).
 A last line times 8192 one-token decode steps from position 0 (the captured step), the other way to take in an 8192-token prompt.
+With --kv-bits 16,8 one model per cache kind is built in the same process and the kinds alternate at every prompt length; for the
+8-bit cache the attention launches read the staging pair, and the staging dequantisation (rows [0, pos0) of every layer and chunk,
+hqq_b200_dequantize) is timed the same way and reported as its share of the prefill.  kv_cache_bytes() of each model is printed, and
+at the end the relative L2 of the two kinds' last-position logits after one --logits-prompt-token prompt, in fp16 and in bf16.
 
-    python tools/prefill_step.py [--lengths 512,2048,...] [--chunk 4096] [--sdpa-max 131072]"""
+    python tools/prefill_step.py [--lengths 512,2048,...] [--chunk 4096] [--sdpa-max 131072] [--kv-bits 16,8]"""
 import argparse
 import json
 import os
@@ -45,52 +49,73 @@ def main():
     ap.add_argument("--cache-len", type=int, default=131072)
     ap.add_argument("--sdpa-max", type=int, default=131072, help="longest prompt the SDPA comparison runs on")
     ap.add_argument("--decode-steps", type=int, default=8192)
+    ap.add_argument("--kv-bits", default="16")
+    ap.add_argument("--logits-prompt", type=int, default=4096, help="with two cache kinds: their last-position logits after a prompt this long")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     info = gpu_info()
     shape = harness.LLAMA31_8B
-    model = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=args.cache_len, fused=5)
-    model.capture(warmup=2)
+    models = {}
+    for kb in [int(x) for x in args.kv_bits.split(",")]:
+        models[kb] = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=args.cache_len, fused=5, kv_bits=kb)
+        models[kb].capture(warmup=2)
+        print(json.dumps({"kv_bits": kb, "kv_cache_bytes": models[kb].kv_cache_bytes(), **info}), flush=True)
+    model = models[min(models)]
     lib, code = load(), DTYPE_CODE[model.dtype]
     hd, hq, hkv, nl = shape.head_dim, shape.n_heads, shape.n_kv_heads, len(model.blocks)
     g = torch.Generator(device=dev).manual_seed(1)
     sampler = ClockSampler(0)
     sampler.start()
-    model.reset_state()
-    model.prefill(torch.randint(0, shape.vocab, (1, 512), generator=g, device=dev), chunk=args.chunk)  # warm-up: modules, routes
+    for m in models.values():
+        m.reset_state()
+        m.prefill(torch.randint(0, shape.vocab, (1, 512), generator=g, device=dev), chunk=args.chunk)  # warm-up: modules, routes
     for T in [int(x) for x in args.lengths.split(",")]:
         prompt = torch.randint(0, shape.vocab, (1, T), generator=g, device=dev)
-        model.reset_state()
-        total_ms = timed(dev, lambda: model.prefill(prompt, chunk=args.chunk))
-        # the same attention launches over the caches the prefill filled
-        qr = torch.randn(min(T, args.chunk), hq * hd, generator=g, device=dev).half()
-        out = torch.empty_like(qr)
-        chunks = [(c0, min(args.chunk, T - c0)) for c0 in range(0, T, args.chunk)]
+        for kb, m in models.items():
+            m.reset_state()
+            total_ms = timed(dev, lambda: m.prefill(prompt, chunk=args.chunk))
+            # the same attention launches over the caches the prefill filled (kv8: the staging pair)
+            qr = torch.randn(min(T, args.chunk), hq * hd, generator=g, device=dev).half()
+            out = torch.empty_like(qr)
+            chunks = [(c0, min(args.chunk, T - c0)) for c0 in range(0, T, args.chunk)]
+            kc, vc = m._kv8_stage if kb == 8 else (None, None)
 
-        def attention():
-            for c0, n in chunks:
-                for blk in model.blocks:
-                    check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(blk["k_cache"]), ptr(blk["v_cache"]), ptr(out), c0, n, hq, hkv, args.cache_len, hd,
-                                                         1, code, stream_ptr(dev)))
-        attention()
-        attn_ms = timed(dev, attention)
-        flops = 4.0 * hd * hq * (T * (T + 1) // 2) * nl
-        line = {"prompt_len": T, "chunk": args.chunk, "cache_len": args.cache_len, "prefill_ms": round(total_ms, 2),
-                "prompt_tok_s": round(T / total_ms * 1e3, 1), "attn_ms": round(attn_ms, 2), "rest_ms": round(total_ms - attn_ms, 2),
-                "attn_share": round(attn_ms / total_ms, 3), "attn_tflops": round(flops / attn_ms / 1e9, 1),
-                "attn_frac_of_989": round(flops / attn_ms / 1e9 / PEAK_TFLOPS, 3)}
-        if T <= args.sdpa_max:
-            q = torch.randn(1, hq, T, hd, generator=g, device=dev).half()
-            k = torch.randn(1, hkv, T, hd, generator=g, device=dev).half().repeat_interleave(hq // hkv, dim=1)
-            v = torch.randn(1, hkv, T, hd, generator=g, device=dev).half().repeat_interleave(hq // hkv, dim=1)
-            F.scaled_dot_product_attention(q, k, v, is_causal=True)
-            sd_ms = timed(dev, lambda: F.scaled_dot_product_attention(q, k, v, is_causal=True)) * nl
-            line.update({"sdpa_ms": round(sd_ms, 2), "sdpa_tflops": round(flops / sd_ms / 1e9, 1), "attn_vs_sdpa": round(sd_ms / attn_ms, 3)})
-            del q, k, v
-        line.update(info)
-        print(json.dumps(line), flush=True)
-        del qr, out
+            def attention():
+                for c0, n in chunks:
+                    for blk in m.blocks:
+                        check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(blk["k_cache"] if kc is None else kc), ptr(blk["v_cache"] if vc is None else vc),
+                                                             ptr(out), c0, n, hq, hkv, args.cache_len, hd, 1, code, stream_ptr(dev)))
+            attention()
+            attn_ms = timed(dev, attention)
+            flops = 4.0 * hd * hq * (T * (T + 1) // 2) * nl
+            line = {"prompt_len": T, "kv_bits": kb, "chunk": args.chunk, "cache_len": args.cache_len, "prefill_ms": round(total_ms, 2),
+                    "prompt_tok_s": round(T / total_ms * 1e3, 1), "attn_ms": round(attn_ms, 2), "rest_ms": round(total_ms - attn_ms, 2),
+                    "attn_share": round(attn_ms / total_ms, 3), "attn_tflops": round(flops / attn_ms / 1e9, 1),
+                    "attn_frac_of_989": round(flops / attn_ms / 1e9 / PEAK_TFLOPS, 3)}
+            if kb == 8:  # the staging dequantisation of rows [0, c0) the prefill ran before each chunk's attention
+                def staging():
+                    for c0, n in chunks:
+                        if c0 == 0:
+                            continue
+                        for blk in m.blocks:
+                            for h in range(hkv):
+                                for c, dst in (("k", kc), ("v", vc)):
+                                    check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][0, h]), ptr(blk[c + "_scale"][0, h]), ptr(blk[c + "_zero"][0, h]),
+                                                                  ptr(dst[0, h]), c0, hd, m.kv_group_size, 8, 1, code, stream_ptr(dev)))
+                st_ms = timed(dev, staging)
+                line.update({"staging_ms": round(st_ms, 2), "staging_share": round(st_ms / total_ms, 4)})
+            if kb == 16 and T <= args.sdpa_max:
+                q = torch.randn(1, hq, T, hd, generator=g, device=dev).half()
+                k = torch.randn(1, hkv, T, hd, generator=g, device=dev).half().repeat_interleave(hq // hkv, dim=1)
+                v = torch.randn(1, hkv, T, hd, generator=g, device=dev).half().repeat_interleave(hq // hkv, dim=1)
+                F.scaled_dot_product_attention(q, k, v, is_causal=True)
+                sd_ms = timed(dev, lambda: F.scaled_dot_product_attention(q, k, v, is_causal=True)) * nl
+                line.update({"sdpa_ms": round(sd_ms, 2), "sdpa_tflops": round(flops / sd_ms / 1e9, 1), "attn_vs_sdpa": round(sd_ms / attn_ms, 3)})
+                del q, k, v
+            line.update(info)
+            print(json.dumps(line), flush=True)
+            del qr, out
     # the captured one-token step, fed from position 0
     model.reset_state()
     model.decode()
@@ -104,6 +129,22 @@ def main():
     print(json.dumps({"decode_steps": steps, "decode_total_ms": round(dec_ms, 1), "decode_tok_s": round(steps / dec_ms * 1e3, 1), **info}), flush=True)
     clocks = sampler.stop()
     print(json.dumps({"clocks": clocks, **info}), flush=True)
+    if args.logits_prompt and len(models) > 1:
+        # last-position logits of the 8-bit cache against the fp16 / bf16 cache after the same prompt, same weights (seed)
+        del models, model
+        torch.cuda.empty_cache()
+        prompt = torch.randint(0, shape.vocab, (1, args.logits_prompt), generator=g, device=dev)
+        for dt in (torch.float16, torch.bfloat16):
+            logits = {}
+            for kb in (16, 8):
+                m = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=dt, device=dev, cache_len=args.logits_prompt, fused=5, kv_bits=kb)
+                m.prefill(prompt, chunk=args.chunk)
+                logits[kb] = m.last_logits.float().clone()
+                del m
+                torch.cuda.empty_cache()
+            rel = float((logits[8] - logits[16]).norm() / logits[16].norm())
+            print(json.dumps({"logits_prompt": args.logits_prompt, "dtype": str(dt).split(".")[-1], "kv8_vs_kv16_logits_rel_l2": rel,
+                              "same_argmax": bool(torch.equal(logits[8].argmax(-1), logits[16].argmax(-1))), **info}), flush=True)
 
 
 if __name__ == "__main__":
