@@ -16,6 +16,14 @@ namespace hqq {
 // plain code; the cluster argmax (DSMEM) is not emulated
 __device__ __forceinline__ uint32_t ld_sys_u32(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
 __device__ __forceinline__ void prefetch_l2(const void*) {}
+// shared-memory integer atomics of the sampling kernel: the emulator resumes a block's threads one at a time and switches only
+// at collectives, so a plain read-modify-write is atomic there
+__device__ __forceinline__ void smem_add(unsigned* p, unsigned v) { *p += v; }
+__device__ __forceinline__ void smem_add(unsigned long long* p, unsigned long long v) { *p += v; }
+__device__ __forceinline__ void smem_max(unsigned* p, unsigned v) { if (v > *p) *p = v; }
+__device__ __forceinline__ void smem_max(unsigned long long* p, unsigned long long v) { if (v > *p) *p = v; }
+__device__ __forceinline__ uint32_t umulhi32(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) >> 32); }
+__device__ __forceinline__ unsigned long long f32_to_u64_rn(float a) { return (unsigned long long)llrintf(a); }  // 0 <= a < 2^63
 #else
 __device__ __forceinline__ uint32_t ld_sys_u32(const uint32_t* p) {
   uint32_t v;
@@ -23,6 +31,12 @@ __device__ __forceinline__ uint32_t ld_sys_u32(const uint32_t* p) {
   return v;
 }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
+__device__ __forceinline__ void smem_add(unsigned* p, unsigned v) { atomicAdd(p, v); }
+__device__ __forceinline__ void smem_add(unsigned long long* p, unsigned long long v) { atomicAdd(p, v); }
+__device__ __forceinline__ void smem_max(unsigned* p, unsigned v) { atomicMax(p, v); }
+__device__ __forceinline__ void smem_max(unsigned long long* p, unsigned long long v) { atomicMax(p, v); }
+__device__ __forceinline__ uint32_t umulhi32(uint32_t a, uint32_t b) { return __umulhi(a, b); }
+__device__ __forceinline__ unsigned long long f32_to_u64_rn(float a) { return __float2ull_rn(a); }
 #endif
 
 template <typename T> __device__ __forceinline__ T from_f32(float v);
@@ -1184,6 +1198,240 @@ int prefill_args(const char* name, int pos0, int n_tok, int n_q, int n_kv, int L
   return HQQ_OK;
 }
 
+// ---- sampling: temperature, top-k, top-p and a Gumbel race (hqq_b200_glue_sample; the definition is in include/hqq_b200.h) --------
+// One CTA of 1024 threads per row.  Each 16-bit value maps to a monotone ordered key (-0 with +0), so the top-k pivot and the top-p
+// threshold are keys, found by a radix select: a 256-bin histogram of the high byte, then one of the low byte inside the bin that
+// holds the answer.  Counts and fixed-point masses round(w * 2^32), w = exp((l - max) / T) <= 1, are integers summed with shared
+// atomics: any order gives the same bits.  Passes over the row: without a filter one (the race); with a filter three --
+//   1. high-byte counts and the maximum;
+//   2. low-byte counts and masses inside the top-k pivot bin, high-byte masses above it;
+//   3. the race over the kept elements.  When the top-p threshold lies in a higher bin than the top-k pivot, this pass also sums
+//      the low-byte masses of that bin and keeps one race winner per low byte there; the threshold then picks among those.
+// The race skips the Philox draw and the logarithms of an element that cannot win: g <= 16.64, so l / T + 17 below the key of an
+// element this thread has already kept is a loss.
+constexpr int kSampleThreads = 1024;
+constexpr float kGumbelMax = 17.0f;  // above the largest g, -log(-log(1 - 2^-24)) = 16.64
+
+__device__ __forceinline__ uint32_t sample_key(uint32_t bits) {
+  if (bits == 0x8000u) bits = 0;  // -0 orders with +0
+  return (bits & 0x8000u) ? (~bits & 0xFFFFu) : (bits | 0x8000u);
+}
+
+template <typename T> __device__ __forceinline__ float sample_key_value(uint32_t k) {
+  const unsigned short bits = (unsigned short)((k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu));
+  return to_f32<T>(*reinterpret_cast<const T*>(&bits));
+}
+
+// Philox4x32-10 (Salmon et al., SC'11): counter c, key (k0, k1)
+__device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r > 0) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint32_t hi0 = umulhi32(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
+    const uint32_t hi1 = umulhi32(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
+    const uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
+    c[0] = n0; c[1] = lo1; c[2] = n2; c[3] = lo0;
+  }
+}
+
+__device__ __forceinline__ unsigned long long sample_mass(float l, float m, float temperature) {
+  return f32_to_u64_rn(expf(__fdiv_rn(__fsub_rn(l, m), temperature)) * 4294967296.0f);
+}
+
+// Warp 0: the bin b of bins[0..256) where the sum from bin 255 down first reaches target, and the sum of the bins above b.
+// Needs 1 <= target <= the sum of all bins.
+template <typename C>
+__device__ __forceinline__ void find_from_top(const C* bins, unsigned long long target, int* bin_out, unsigned long long* above_out) {
+  const int lane = threadIdx.x & 31;
+  unsigned long long s = 0;
+  for (int j = 0; j < 8; ++j) s += bins[lane * 8 + j];
+  unsigned long long suf = s;  // sum of lanes lane..31
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long t = __shfl_sync(0xffffffffu, suf, lane + o < 32 ? lane + o : 31);
+    if (lane + o < 32) suf += t;
+  }
+  unsigned long long above = suf - s;
+  if (above < target && target <= suf) {
+    for (int j = 7; j >= 0; --j) {
+      const unsigned long long c = bins[lane * 8 + j];
+      if (above + c >= target) { *bin_out = lane * 8 + j; *above_out = above; break; }
+      above += c;
+    }
+  }
+}
+
+// warp sum of bins[0..256)
+__device__ __forceinline__ unsigned long long warp_bin_sum(const unsigned long long* bins) {
+  unsigned long long s = 0;
+  for (int j = 0; j < 8; ++j) s += bins[(threadIdx.x & 31) * 8 + j];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __restrict__ logits, int n, long long ld, float temperature, int top_k,
+                                                                float top_p, uint32_t seed_lo, uint32_t seed_hi,
+                                                                const unsigned long long* __restrict__ counter, long long* __restrict__ out) {
+  __shared__ unsigned cnt_hi[256], cnt_lo[256];
+  __shared__ unsigned long long mass_hi[256], mass_lo[256], best_lo[256], red[32];
+  __shared__ unsigned max_key;
+  __shared__ int sel_bin;
+  __shared__ unsigned long long sel_above, sel_target;
+  const int tid = threadIdx.x;
+  const uint32_t row = blockIdx.x;
+  const T* x = logits + (long long)row * ld;
+  const bool use_k = top_k > 0 && top_k < n, use_p = top_p < 1.0f;
+  for (int i = tid; i < 256; i += kSampleThreads) { cnt_hi[i] = 0; cnt_lo[i] = 0; mass_hi[i] = 0; mass_lo[i] = 0; best_lo[i] = 0; }
+  if (tid == 0) { max_key = 0; sel_bin = 0; sel_above = 0; }
+  pdl_launch_dependents();
+  pdl_wait();
+  const unsigned long long ctr = *counter;
+  __syncthreads();
+  auto each = [&](auto&& f) {
+    for (int i = tid * 8; i < n; i += kSampleThreads * 8) {
+      if (i + 8 <= n) {
+        const Vec<T, 8> v = *reinterpret_cast<const Vec<T, 8>*>(x + i);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f(i + j, v.v[j]);
+      } else {
+        for (int j = i; j < n; ++j) f(j, x[j]);
+      }
+    }
+  };
+
+  int hb_k = -1, lb_k = 0;   // top-k pivot key hb_k << 8 | lb_k; hb_k -1: no top-k
+  uint32_t thr = 0;          // kept: key >= thr ...
+  int split = -1;            // ... or, when split >= 0: high byte > split, or high byte == split and low byte >= the top-p low byte
+  unsigned long long p_left = 0;  // split >= 0: the mass the low bytes of bin `split` must still supply
+  if (use_k || use_p) {
+    unsigned mk = 0;
+    each([&](int, T v) {
+      const uint32_t k = sample_key(bits16(v));
+      smem_add(&cnt_hi[k >> 8], 1u);
+      mk = k > mk ? k : mk;
+    });
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const unsigned t = __shfl_xor_sync(0xffffffffu, mk, o); mk = t > mk ? t : mk; }
+    if ((tid & 31) == 0) smem_max(&max_key, mk);
+    __syncthreads();
+    if (use_k && tid < 32) find_from_top(cnt_hi, (unsigned long long)top_k, &sel_bin, &sel_above);
+    __syncthreads();
+    const unsigned long long k_left = (unsigned long long)top_k - sel_above;
+    if (use_k) hb_k = sel_bin;
+    const float m = sample_key_value<T>(max_key);
+    each([&](int, T v) {
+      const uint32_t k = sample_key(bits16(v));
+      const int hi = (int)(k >> 8);
+      if (hi < hb_k || (hi > hb_k && !use_p)) return;
+      const unsigned long long w = use_p ? sample_mass(to_f32<T>(v), m, temperature) : 0ull;
+      if (hi == hb_k) {
+        smem_add(&cnt_lo[k & 255u], 1u);
+        if (w) smem_add(&mass_lo[k & 255u], w);
+      } else if (w) {
+        smem_add(&mass_hi[hi], w);
+      }
+    });
+    __syncthreads();
+    if (use_k) {
+      if (tid < 32) find_from_top(cnt_lo, k_left, &sel_bin, &sel_above);
+      __syncthreads();
+      lb_k = sel_bin;
+      thr = ((uint32_t)hb_k << 8) | (uint32_t)lb_k;
+      if (tid < 256 && tid < lb_k) mass_lo[tid] = 0;  // the pivot bin keeps its low bytes >= lb_k
+      __syncthreads();
+    }
+    if (use_p) {
+      if (tid < 32) {
+        if (hb_k >= 0) {
+          const unsigned long long s = warp_bin_sum(mass_lo);
+          if (tid == 0) mass_hi[hb_k] = s;
+        }
+        __syncwarp();
+        const unsigned long long total = warp_bin_sum(mass_hi);
+        const unsigned long long target = (unsigned long long)ceil((double)top_p * (double)total);
+        if (tid == 0) sel_target = target;
+        find_from_top(mass_hi, target, &sel_bin, &sel_above);
+      }
+      __syncthreads();
+      const int hb_p = sel_bin;
+      p_left = sel_target - sel_above;
+      __syncthreads();
+      if (hb_p == hb_k) {  // the threshold lies in the pivot bin, whose low-byte masses are at hand
+        if (tid < 32) find_from_top(mass_lo, p_left, &sel_bin, &sel_above);
+        __syncthreads();
+        thr = ((uint32_t)hb_p << 8) | (uint32_t)sel_bin;
+      } else {
+        split = hb_p;
+        for (int i = tid; i < 256; i += kSampleThreads) mass_lo[i] = 0;
+        __syncthreads();
+      }
+    }
+  }
+
+  // the race: the kept element with the largest l / T + g (lowest index on equal keys), g = -log(-log u) from Philox
+  unsigned long long best = 0;
+  float best_r = -INFINITY;
+  long long pq = -1;
+  uint32_t ph[4] = {0, 0, 0, 0};
+  const float m_p = split >= 0 ? sample_key_value<T>(max_key) : 0.0f;
+  each([&](int i, T v) {
+    const uint32_t k = sample_key(bits16(v));
+    bool edge = false;
+    if (split >= 0) {
+      const int hi = (int)(k >> 8);
+      if (hi < split) return;
+      edge = hi == split;
+    } else if (k < thr) {
+      return;
+    }
+    const float l = to_f32<T>(v);
+    if (edge) {
+      const unsigned long long w = sample_mass(l, m_p, temperature);
+      if (w) smem_add(&mass_lo[k & 255u], w);
+    }
+    const float lt = __fdiv_rn(l, temperature);
+    if (__fadd_rn(lt, kGumbelMax) < best_r) return;
+    if ((long long)(i >> 2) != pq) {
+      pq = i >> 2;
+      ph[0] = (uint32_t)pq; ph[1] = row; ph[2] = (uint32_t)ctr; ph[3] = (uint32_t)(ctr >> 32);
+      philox4x32_10(ph, seed_lo, seed_hi);
+    }
+    const int wi = i & 3;
+    const uint32_t word = wi == 0 ? ph[0] : wi == 1 ? ph[1] : wi == 2 ? ph[2] : ph[3];
+    const float u = ((float)(word >> 9) + 0.5f) * 0x1p-23f;  // exact: 24 significant bits at most
+    const float r = __fadd_rn(lt, -logf(-logf(u)));
+    const uint32_t ur = __float_as_uint(r);
+    const unsigned long long key = ((unsigned long long)((ur & 0x80000000u) ? ~ur : (ur | 0x80000000u)) << 32) | (0xFFFFFFFFu - (uint32_t)i);
+    if (edge) {
+      smem_max(&best_lo[k & 255u], key);
+    } else if (key > best) {
+      best = key;
+      best_r = r;
+    }
+  });
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, best, o); best = t > best ? t : best; }
+  if ((tid & 31) == 0) red[tid >> 5] = best;
+  __syncthreads();
+  if (tid < 32) {
+    best = red[tid];
+    if (split >= 0) {  // the top-p low byte of bin `split`, then the winners of the low bytes at or above it
+      find_from_top(mass_lo, p_left, &sel_bin, &sel_above);
+      __syncwarp();
+      const int lb = *reinterpret_cast<volatile int*>(&sel_bin);
+      for (int j = 0; j < 8; ++j) {
+        const int bin = tid * 8 + j;
+        if (bin >= lb && best_lo[bin] > best) best = best_lo[bin];
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, best, o); best = t > best ? t : best; }
+    if (tid == 0) out[row] = (long long)(0xFFFFFFFFu - (uint32_t)(best & 0xFFFFFFFFull));
+  }
+}
+
 }  // namespace
 
 #ifndef HQQ_EMU
@@ -1482,6 +1730,27 @@ extern "C" int hqq_b200_glue_attn_prefill(const void* q_rot, const void* k_cache
     if (int rc = reserve_smem<attn_prefill_kernel<E>>(kPreSmemBytes)) return rc;
     return launch_pdl("attn_prefill", attn_prefill_kernel<E>, grid, dim3(kPreThreads), kPreSmemBytes, st, (const E*)q_rot, (const E*)k_cache,
                       (const E*)v_cache, (E*)out, pos0, T, n_q_heads, n_kv_heads, cache_len, scale_log2);
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
+                                    const uint64_t* counter, int64_t* out, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_sample";
+  HQQ_REQUIRE(logits && counter && out, HQQ_E_INVALID, "%s: null pointer", name);
+  HQQ_REQUIRE(dtype == HQQ_F16 || dtype == HQQ_BF16, HQQ_E_INVALID, "%s: dtype must be f16/bf16", name);
+  HQQ_REQUIRE(temperature > 0.0f && temperature <= 3.40282347e38f, HQQ_E_INVALID, "%s: temperature must be finite and > 0 (got %g)", name, (double)temperature);
+  HQQ_REQUIRE(top_k >= 0, HQQ_E_INVALID, "%s: top_k must be >= 0 (got %d)", name, top_k);
+  HQQ_REQUIRE(top_p > 0.0f && top_p <= 1.0f, HQQ_E_INVALID, "%s: top_p must lie in (0, 1] (got %g)", name, (double)top_p);
+  HQQ_REQUIRE(n > 0 && ld >= n && rows > 0 && rows <= 65535, HQQ_E_INVALID, "%s: needs n > 0, ld >= n and 1 <= rows <= 65535 (n=%d ld=%d rows=%d)", name,
+              n, ld, rows);
+  HQQ_REQUIRE(aligned(logits, 16) && ld % 8 == 0, HQQ_E_INVALID, "%s: rows must start on 16-byte boundaries (logits 16-byte aligned, ld %% 8 == 0; ld=%d)",
+              name, ld);
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto t) {
+    using E = decltype(t);
+    return launch_pdl("sample", sample_kernel<E>, dim3((unsigned)rows), dim3(kSampleThreads), 0, st, (const E*)logits, n, (long long)ld, temperature, top_k,
+                      top_p, (uint32_t)seed, (uint32_t)(seed >> 32), (const unsigned long long*)counter, (long long*)out);
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }

@@ -112,6 +112,66 @@ def kv8_dequantize(q: torch.Tensor, scale: torch.Tensor, zero: torch.Tensor) -> 
     return ((qs - zero.unsqueeze(-1)) * scale.unsqueeze(-1)).reshape(q.shape)
 
 
+_PHILOX_M = (0xD2511F53, 0xCD9E8D57)
+_PHILOX_W = (0x9E3779B9, 0xBB67AE85)
+_U32 = 0xFFFFFFFF
+
+
+def _mulhilo32(a: torch.Tensor, m: int):
+    """High and low 32-bit words of a * m, a int64 in [0, 2^32), m a 32-bit constant; exact in int64 through 16-bit limbs."""
+    p0 = a * (m & 0xFFFF)                # < 2^48
+    p1 = a * (m >> 16)                   # < 2^48
+    s = ((p1 & 0xFFFF) << 16) + p0       # < 2^49
+    return (p1 >> 16) + (s >> 32), s & _U32
+
+
+def philox_uniforms(n: int, rows: int, seed: int, counter, device=None) -> torch.Tensor:
+    """The race's uniforms of hqq_b200_glue_sample on framework ops: u [rows, n] in float64, u[b, i] = ((x >> 9) + 0.5) * 2^-23 with x
+    word i % 4 of Philox4x32-10 under key (seed & 0xFFFFFFFF, seed >> 32) and counter (i / 4, b, ctr & 0xFFFFFFFF, ctr >> 32).
+    counter: a python int or an int64 tensor of one element (read on the device, so a captured graph sees it advance)."""
+    if not torch.is_tensor(counter):
+        counter = torch.tensor([int(counter)], dtype=torch.int64, device=device)
+    device = counter.device
+    ctr = counter.reshape(1, 1).to(torch.int64)
+    nq = -(-n // 4)
+    c0 = torch.arange(nq, dtype=torch.int64, device=device).view(1, nq).expand(rows, nq)
+    c1 = torch.arange(rows, dtype=torch.int64, device=device).view(rows, 1).expand(rows, nq)
+    c2, c3 = (ctr & _U32).expand(rows, nq), ((ctr >> 32) & _U32).expand(rows, nq)
+    k0, k1 = int(seed) & _U32, (int(seed) >> 32) & _U32
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + _PHILOX_W[0]) & _U32, (k1 + _PHILOX_W[1]) & _U32
+        hi0, lo0 = _mulhilo32(c0, _PHILOX_M[0])
+        hi1, lo1 = _mulhilo32(c2, _PHILOX_M[1])
+        c0, c1, c2, c3 = hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0
+    x = torch.stack((c0, c1, c2, c3), dim=-1).reshape(rows, 4 * nq)[:, :n]
+    return ((x >> 9).double() + 0.5) * 2.0 ** -23
+
+
+def sample_tokens(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, seed: int, counter) -> torch.Tensor:
+    """hqq_b200_glue_sample restated on framework ops in float64 (the definition is in include/hqq_b200.h): logits [rows, n] in
+    fp16 / bf16, row b sampled with Philox counter (., b, counter); returns int64 [rows].  temperature and top_p are taken at fp32
+    precision, as the kernel receives them.  Top-k compares the 16-bit values as stored.  The reference generator's
+    torch.where(logits < pivot, -inf, logits) on fp16(logits / T) can merge neighbouring values by that rounding; here they stay
+    apart, so its keep set can be larger than ours at the pivot."""
+    T = float(torch.tensor(temperature, dtype=torch.float32))
+    P = float(torch.tensor(top_p, dtype=torch.float32))
+    rows, n = logits.shape
+    lv = logits.double()
+    keep = torch.ones_like(lv, dtype=torch.bool)
+    if 0 < top_k < n:
+        keep = lv >= torch.topk(lv, top_k, dim=-1).values[:, -1:]
+    if P < 1.0:
+        w = torch.where(keep, torch.exp((lv - lv.amax(dim=-1, keepdim=True)) / T), torch.zeros_like(lv))
+        vs, order = torch.sort(torch.where(keep, lv, torch.full_like(lv, -math.inf)), dim=-1, descending=True)
+        cum = w.gather(1, order).cumsum(dim=-1)
+        j = (cum < P * cum[:, -1:]).sum(dim=-1, keepdim=True).clamp(max=n - 1)
+        keep = keep & (lv >= vs.gather(1, j))
+    u = philox_uniforms(n, rows, seed, counter, logits.device)
+    key = torch.where(keep, lv / T - torch.log(-torch.log(u)), torch.full_like(lv, -math.inf))
+    return torch.argmax(key, dim=-1)
+
+
 def shard_dims(shape: LlamaShape, tp: int):
     """Per-rank sizes of the sharded projections (pure host logic, unit-tested on CPU)."""
     if shape.n_heads % tp or shape.n_kv_heads % tp or shape.inter % tp:
@@ -127,8 +187,22 @@ class DecodeModel:
     def __init__(self, shape: LlamaShape = LLAMA3_8B, nbits: int = 4, group_size: int = 64, dtype=torch.float16,
                  device="cuda", cache_len: int = 256, tp: int = 1, rank: int = 0, seed: int = 0, process_group=None,
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
-                 kv_bits: int = 16, kv_group_size: int = 64):
+                 kv_bits: int = 16, kv_group_size: int = 64, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
+                 top_p: float = 1.0, sample_seed: int = 0):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
+        # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
+        # top-k, top-p, then a Gumbel race on Philox numbers keyed by sample_seed and countered by _sample_ctr -- instead of the argmax.
+        # The defaults are those of the reference's HFGenerator; like there, the parameters are fixed for the model's life.
+        t32 = float(torch.tensor(float(temperature), dtype=torch.float32)) if isinstance(temperature, (int, float)) else math.nan
+        if not (math.isfinite(t32) and t32 > 0):  # the kernel takes it as fp32
+            raise ValueError(f"temperature must be finite and > 0 in fp32 (got {temperature!r})")
+        if not (isinstance(top_k, int) and top_k >= 0):
+            raise ValueError(f"top_k must be an int >= 0, 0 for off (got {top_k!r})")
+        if not (isinstance(top_p, (int, float)) and 0 < float(torch.tensor(float(top_p), dtype=torch.float32)) <= 1 and top_p <= 1):
+            raise ValueError(f"top_p must lie in (0, 1], 1 for off (got {top_p!r})")
+        if not (isinstance(sample_seed, int) and 0 <= sample_seed < 2 ** 64):
+            raise ValueError(f"sample_seed must be an int in [0, 2^64) (got {sample_seed!r})")
+        self.do_sample, self.temperature, self.top_k, self.top_p, self.sample_seed = bool(do_sample), float(temperature), int(top_k), float(top_p), int(sample_seed)
         # kv_bits 8: every layer's K and V cache in HQQ's 8-bit format (kv8_quantize_rows), groups of kv_group_size along the head dim
         if kv_bits not in (16, 8):
             raise ValueError(f"kv_bits must be 16 or 8 (got {kv_bits!r})")
@@ -214,6 +288,7 @@ class DecodeModel:
         self.tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
         self.pos = torch.zeros(1, dtype=torch.long, device=self.device)
         self.next_tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
+        self._sample_ctr = torch.zeros(1, dtype=torch.long, device=self.device)  # Philox counter: + 1 per sampled token
         self.graph = None
         self.last_logits = None  # set by prefill(): logits of the last prompt position of each sequence
 
@@ -299,7 +374,10 @@ class DecodeModel:
             h = h + y
         h = F.rms_norm(h, (s.hidden,), self.final_norm, s.rms_eps)
         logits = torch.matmul(h, self.lm_head.t())
-        if self.tp > 1:  # vocabulary shards: the global maximum, then the lowest global index that attains it (two small all-reduces)
+        if self.do_sample:
+            self.next_tok.copy_(self._sample_ref(logits))
+            self._sample_ctr.add_(1)
+        elif self.tp > 1:  # vocabulary shards: the global maximum, then the lowest global index that attains it (two small all-reduces)
             val, idx = torch.max(logits.float(), dim=-1)
             gmax = val.clone()
             torch.distributed.all_reduce(gmax, op=torch.distributed.ReduceOp.MAX, group=self.pg)
@@ -322,14 +400,62 @@ class DecodeModel:
         """kv_bits 8 on framework ops: the dequantised K and V cache rows [0, end)."""
         return tuple(kv8_dequantize(blk[n + "_cache"][:, :, :end], blk[n + "_scale"][:, :, :end], blk[n + "_zero"][:, :, :end]) for n in ("k", "v"))
 
+    def _sample_ref(self, logits):
+        """do_sample on framework ops (fused=False): sample_tokens on the full-vocabulary rows (under tensor parallelism every rank
+        gathers the shards and draws the same tokens)."""
+        if self.tp > 1:
+            g = torch.empty(self.tp * logits.shape[0], logits.shape[1], dtype=logits.dtype, device=logits.device)
+            torch.distributed.all_gather_into_tensor(g, logits.contiguous(), group=self.pg)
+            logits = g.view(self.tp, -1, self.vocab_shard).transpose(0, 1).reshape(-1, self.shape.vocab)
+        return sample_tokens(logits, self.temperature, self.top_k, self.top_p, self.sample_seed, self._sample_ctr)
+
+    def _sample_buffers(self, rows):
+        """What _sample_rows needs for `rows` sequences: the all-gather target under tensor parallelism, and padded rows where the
+        gathered layout or the vocabulary length does not give 16-byte aligned rows."""
+        n, d = self.shape.vocab, {}
+        if self.tp > 1:
+            d["sample_gather"] = torch.zeros(self.tp * rows, self.vocab_shard, dtype=self.dtype, device=self.device)
+        if n % 8 or (self.tp > 1 and rows > 1):
+            d["sample_rows"] = torch.zeros(rows, -(-n // 8) * 8, dtype=self.dtype, device=self.device)
+        return d
+
+    def _sample_rows(self, logits, bufs):
+        """Full-vocabulary rows for hqq_b200_glue_sample from this rank's logits [rows, vocab / tp]: with tp > 1 one NCCL all-gather
+        of the shards (capturable), rearranged to [rows, vocab] when rows > 1; rows padded to a multiple of 8 elements when the
+        vocabulary is not one (the kernel reads 16-byte vectors)."""
+        B, n = logits.shape[0], self.shape.vocab
+        if self.tp > 1:
+            g = bufs["sample_gather"]
+            torch.distributed.all_gather_into_tensor(g, logits, group=self.pg)
+            if "sample_rows" not in bufs:
+                return g.view(B, n)  # one row: the shards follow each other
+            src = g.view(self.tp, B, self.vocab_shard).transpose(0, 1)  # [B, tp, vocab / tp]
+        else:
+            if "sample_rows" not in bufs:
+                return logits
+            src = logits.view(B, 1, n)
+        rows = bufs["sample_rows"]
+        rows[:, :n].view(B, self.tp, self.vocab_shard).copy_(src)
+        return rows
+
+    def _sample(self, lib, rows, out, code, st):
+        """One launch of hqq_b200_glue_sample over rows [B, >= vocab]: out[b] = the token of row b at the current _sample_ctr."""
+        from ._lib import check, ptr
+        check(lib.hqq_b200_glue_sample(ptr(rows), self.shape.vocab, rows.stride(0), rows.shape[0], self.temperature, self.top_k, self.top_p,
+                                       self.sample_seed, ptr(self._sample_ctr), ptr(out), code, st))
+
     def _head(self, lib, x, code, st):
         """Final projection + greedy pick inside the captured step: fp16 lm_head through the library GEMV (it is not an HQQ
         layer), then our argmax kernel; with tp > 1 each rank covers its vocabulary shard and the MAX of the ranks' 8-byte
         {value : index} keys picks the winner -- exchanged inside the argmax launch over peer-mapped memory ("p2p"), or by one
-        NCCL all-reduce ("nccl")."""
+        NCCL all-reduce ("nccl").  do_sample: the sampling kernel on the full rows instead (with tp > 1 after one all-gather of the
+        shards, so every rank draws the same token)."""
         from ._lib import check, ptr
         b = self._bufs
         torch.matmul(x, self.lm_head.t(), out=b["logits"])
+        if self.do_sample:
+            self._sample(lib, self._sample_rows(b["logits"], b), self.next_tok, code, st)
+            return
         if self.batch > 1:  # a row per sequence: framework ops (with tp > 1: the global maximum, then the lowest index that attains it)
             if self.tp == 1:
                 self.next_tok.copy_(torch.argmax(b["logits"], dim=-1))
@@ -403,6 +529,8 @@ class DecodeModel:
         norm(delta, self.final_norm)
         self._head(lib, b["x"], code, st)
         self.pos.add_(1).remainder_(self.cache_len)
+        if self.do_sample:
+            self._sample_ctr.add_(1)
 
     def _setup_exchange(self):
         """Buffers of tagged 32-bit words {tag16 : value16} through which the one-token kernels hand activations to each other
@@ -495,15 +623,17 @@ class DecodeModel:
             check(lib.hqq_b200_glue_add_rmsnorm(ptr(h_cur), ptr(delta), ptr(self.final_norm), ptr(b["x"]), s.hidden, s.rms_eps, code, st))
         self._head(lib, b["x"], code, st)
         self.pos.add_(1).remainder_(self.cache_len)
+        if self.do_sample:
+            self._sample_ctr.add_(1)
 
     def prefill(self, tokens: torch.Tensor, start: int = 0, chunk: int = 2048) -> torch.Tensor:
         """Take in a prompt: `tokens` [batch, T] (or [T] when batch is 1) at positions start .. start + T - 1 of every sequence.
         The prompt runs in chunks of at most `chunk` tokens (batch * chunk <= 65535, the row limit of the rows kernels); each
         chunk goes through every block, writing its rotated k and v into the caches.  Only the last position of each sequence
-        goes through the final norm, the lm_head and the argmax; self.last_logits [batch, vocab / tp] keeps those logits (this
-        rank's vocabulary shard).  Afterwards self.pos = (start + T) mod cache_len -- the steps' own wrap, so a prompt that fills
+        goes through the final norm, the lm_head and the argmax (with do_sample: the sampling kernel at the current sample counter,
+        which then advances by one); self.last_logits [batch, vocab / tp] keeps those logits (this rank's vocabulary shard).  Afterwards self.pos = (start + T) mod cache_len -- the steps' own wrap, so a prompt that fills
         the cache leaves the next step at position 0 as a step at the last position does -- and self.tok [batch] holds the greedy
-        next token, which is returned: a captured decode step continues from there.
+        (do_sample: the sampled) next token, which is returned: a captured decode step continues from there.
 
         fused (any value but False): the package's kernels -- add+RMSNorm rows, the routed q/k/v linears at M = batch * chunk,
         RoPE + cache append, causal GQA attention over the cache (csrc/decode_glue.cu), o, add+RMSNorm rows, gate/up, SiLU*mul,
@@ -638,6 +768,10 @@ class DecodeModel:
             x = F.rms_norm(h + delta, (s.hidden,), self.final_norm, s.rms_eps)
             logits = torch.matmul(x, self.lm_head.t())
             self.last_logits = logits
+            if self.do_sample:
+                tok = self._sample_ref(logits)
+                self._sample_ctr.add_(1)
+                return tok
             if self.tp == 1:
                 return torch.argmax(logits, dim=-1)
             val, idx = torch.max(logits.float(), dim=-1)
@@ -653,6 +787,11 @@ class DecodeModel:
         x = torch.empty_like(h)
         check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(delta), ptr(self.final_norm), ptr(x), B, s.hidden, s.rms_eps, code, st))
         self.last_logits = torch.matmul(x, self.lm_head.t())
+        if self.do_sample:
+            tok = torch.empty(B, dtype=torch.long, device=self.device)
+            self._sample(lib, self._sample_rows(self.last_logits, self._sample_buffers(B)), tok, code, st)
+            self._sample_ctr.add_(1)
+            return tok
         # the argmax kernel reads 16-byte vectors: every row starts on a 16-byte boundary whatever the vocabulary shard's length
         n = self.vocab_shard
         rows = torch.empty(B, -(-n // 8) * 8, dtype=self.dtype, device=self.device)
@@ -672,6 +811,8 @@ class DecodeModel:
                       "v": z(s.n_kv_heads // tp * s.head_dim), "a": z(s.n_heads // tp * s.head_dim), "o": z(s.hidden),
                       "gate": z(s.inter // tp), "up": z(s.inter // tp), "act": z(s.inter // tp), "down": z(s.hidden), "logits": z(self.vocab_shard),
                       "key": torch.zeros(1, dtype=torch.long, device=dev)}
+        if self.do_sample:
+            self._bufs.update(self._sample_buffers(self.batch))
         if self.attn_kernel != "single":  # partials + tickets, zeroed once: every launch leaves the tickets at zero
             from ._lib import load
             with torch.cuda.device(dev):
@@ -703,6 +844,7 @@ class DecodeModel:
         """Position 0, empty KV caches, `token` as the first input: the state every token-stream comparison starts from."""
         self.tok.fill_(token)
         self.pos.zero_()
+        self._sample_ctr.zero_()
         for blk in self.blocks:
             for name in ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero"):
                 if name in blk:

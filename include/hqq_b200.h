@@ -314,6 +314,22 @@ int hqq_b200_glue_argmax_key(const void* logits, int n, int64_t index_offset, in
  * the tp keys of this step in its own area and writes the global argmax (first index on ties) to out[0]. */
 int hqq_b200_glue_argmax_tp(const void* logits, int n, int64_t index_offset, void* const* peer_keys, int tp, int rank,
                             const int* step_ctr, int64_t* out, int dtype, void* stream);
+/* Sampling in place of the argmax: row b of `rows` starts at logits + b * ld (elements; 16-byte aligned rows: logits 16-byte
+ * aligned, ld % 8 == 0) and out[b] receives its token.  For a row l[0..n) and temperature > 0, top_k >= 0 (0: off), top_p in
+ * (0, 1] (1: off), in the order of transformers' warpers:
+ *   1. top-k: v_k = the top_k-th largest value of l, repeats counted; keep every i with l[i] >= v_k (ties at the pivot are all
+ *      kept).  Off when top_k == 0 or top_k >= n.  The selection compares the 16-bit values as stored (-0 == +0), not l / T.
+ *   2. top-p: p_i ~ exp((l[i] - max l) / T) over the kept set; v_p = the largest value such that the kept elements with l >= v_p
+ *      carry at least top_p of the mass; keep those (ties again all kept; the maximum always survives).  The masses are fixed
+ *      point, round(exp((l[i] - max) / T) * 2^32) of the fp32 exponential, summed in 64-bit integers.
+ *   3. race: the token is the kept i with the largest l[i] / T + g_i (fp32), lowest index on equal keys; g_i = -log(-log u_i) with
+ *      u_i = ((x >> 9) + 0.5) * 2^-23 (exact in fp32, in (0, 1)), x = word i % 4 of Philox4x32-10 with key (seed & 0xFFFFFFFF,
+ *      seed >> 32) and counter (i / 4, b, *counter & 0xFFFFFFFF, *counter >> 32).
+ * The token is a function of (row bits, n, temperature, top_k, top_p, seed, *counter, b) alone: not of the grid, rows, ld or the
+ * GPU.  top_k = 1 gives the argmax when the maximum is unique.  *counter is read, never written (the decode harness advances it
+ * by one per sampled token).  No workspace, no atomics outside shared memory.  Needs rows <= 65535. */
+int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
+                         const uint64_t* counter, int64_t* out, int dtype, void* stream);
 
 /* Number of kernels launched by this library on the calling thread since the last reset
  * (used by bench.py for its gpu_launches claim).                                        */
