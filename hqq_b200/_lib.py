@@ -65,6 +65,12 @@ SIGNATURES = {
     "hqq_b200_glue_rope_attn_decode_split_kv8": (c_int, [c_void_p] * 14 + [c_int] * 7 + [c_void_p]),
     "hqq_b200_glue_rope_append_rows_kv8": (c_int, [c_void_p] * 14 + [c_int] * 9 + [c_void_p]),
     "hqq_b200_glue_attn_prefill": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_batch_seqpos": (c_int, [c_void_p] * 9 + [c_int] * 6 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_seqpos": (c_int, [c_void_p] * 10 + [c_int] * 6 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_kv8_seqpos": (c_int, [c_void_p] * 14 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_varlen": (c_int, [c_void_p] * 10 + [c_int] * 6 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv8_varlen": (c_int, [c_void_p] * 16 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_attn_prefill_varlen": (c_int, [c_void_p] * 6 + [c_int] * 6 + [c_void_p]),
     "hqq_b200_glue_argmax": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_key": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_tp": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),

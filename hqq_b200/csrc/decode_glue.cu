@@ -141,8 +141,10 @@ __global__ void __launch_bounds__(256) silu_mul_kernel(const T* __restrict__ g, 
 // bound by load latency, not bandwidth: (1) rows 0..pos-1 were written by earlier steps, so they are prefetched into L2
 // BEFORE griddepcontrol.wait, under the tail of the q/k/v kernel (pos itself is only written by the non-PDL kernel that ends
 // a step, a full barrier); (2) both position loops keep 8-16 independent loads in flight per thread.
+// SEQPOS (ragged batches, BATCH only): sequence b sits at its own position pos_p[b], and everything derived from the position --
+// the prefetched rows, the RoPE row, the written row, the loop bounds -- follows it.
 constexpr int kAttnThreads = 256;
-template <typename T, bool BATCH>
+template <typename T, bool BATCH, bool SEQPOS = false>
 __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in,
                                                                         const T* __restrict__ cos_t, const T* __restrict__ sin_t,
                                                                         T* __restrict__ k_cache, T* __restrict__ v_cache, const long long* __restrict__ pos_p,
@@ -160,7 +162,8 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
     k_in += b * n_kv * hd; v_in += b * n_kv * hd;
     k_cache += b * n_kv * L * hd; v_cache += b * n_kv * L * hd;
   }
-  const int pos = (int)pos_p[0];
+  static_assert(BATCH || !SEQPOS, "per-sequence positions need the batch layout");
+  const int pos = (int)pos_p[SEQPOS ? blockIdx.y : 0];
   pdl_launch_dependents();
   {
     // one 128-byte line per prefetch; pos rows of hd * sizeof(T) bytes each in both caches
@@ -365,7 +368,8 @@ __device__ __forceinline__ void split_merge(const float* wp, float* __restrict__
 
 // grid = (S, n_kv, batch), block = 256.  q / out [batch, n_q * 128], k / v [batch, n_kv * 128], caches [batch, n_kv, L, 128].
 // part: [batch, n_kv, S, G, 2 + 128] floats (m, l, o per head), tickets: [batch, n_kv] uint32, zero between launches.
-template <typename T>
+// SEQPOS: sequence b at its own position pos_p[b]; its chunk, staged rows, RoPE row and written row follow it (S stays fixed).
+template <typename T, bool SEQPOS = false>
 __global__ void __launch_bounds__(kSplitThreads, 1)
     rope_attn_decode_split_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
                                   const T* __restrict__ sin_t, T* __restrict__ k_cache, T* __restrict__ v_cache, const long long* __restrict__ pos_p,
@@ -391,7 +395,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
   int* last = reinterpret_cast<int*>(vf + kHd);
 
   // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
-  const int pos = (int)pos_p[0], n_pos = pos + 1;
+  const int pos = (int)pos_p[SEQPOS ? b : 0], n_pos = pos + 1;
   const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
   const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
   const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
@@ -654,8 +658,8 @@ static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kKv8RingBytes, "
 __device__ __forceinline__ int swz8(int r, int c) { return r * kHd + ((c ^ (r & 7)) << 4); }  // 16-byte chunk c of level row r
 
 // grid = (S, n_kv, batch), block = 256.  q / out, k / v as rope_attn_decode_split_kernel; levels [batch, n_kv, L, 128] uint8, meta
-// [batch, n_kv, L, 128 / gs] T; part / tickets as there.
-template <typename T>
+// [batch, n_kv, L, 128 / gs] T; part / tickets as there.  SEQPOS as there.
+template <typename T, bool SEQPOS = false>
 __global__ void __launch_bounds__(kSplitThreads, 1)
     rope_attn_decode_split_kv8_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
                                       const T* __restrict__ sin_t, uint8_t* __restrict__ k_q, T* __restrict__ k_s, T* __restrict__ k_z,
@@ -685,7 +689,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
   int* last = reinterpret_cast<int*>(fm + 8);
 
   // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
-  const int pos = (int)pos_p[0], n_pos = pos + 1;
+  const int pos = (int)pos_p[SEQPOS ? b : 0], n_pos = pos + 1;
   const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
   const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
   const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
@@ -933,15 +937,35 @@ constexpr int kPreTileBytes = kPreTile * kHd * 2;         // one K or V tile, 16
 constexpr int kPreStageBytes = 2 * kPreTileBytes;
 constexpr int kPreSmemBytes = kPreStages * kPreStageBytes;  // 96 KB
 
+// Variable-length prefill (VARLEN instantiations of the three prefill kernels): slot b contributes n_tok[b] >= 0 rows at positions
+// pos0[b] .. pos0[b] + n_tok[b] - 1, packed in slot order from token row row0[b] = sum of n_tok[b'] for b' < b (equal lengths give
+// the b T + t layout).  The grids are sized by the longest slot; CTAs past their slot's rows exit, so a slot with no rows is neither
+// read nor written.  The arrays travel by value in the parameter block (3 KB), so a launch needs no upload and no workspace.
+constexpr int kVarlenMaxBatch = 256;
+struct VarlenRows {
+  int pos0[kVarlenMaxBatch];
+  int n_tok[kVarlenMaxBatch];
+  int row0[kVarlenMaxBatch];
+};
+struct NoVarlen {};  // the fixed-length instantiations: their uniform pos0 / T are the scalar arguments
+template <bool VARLEN> using VarlenArg = typename std::conditional<VARLEN, VarlenRows, NoVarlen>::type;
+
 // grid = (T, batch), block = 256.  q / q_out [batch T, n_q 128], k / v [batch T, n_kv 128] (row b T + t), caches [batch, n_kv, L, 128].
-template <typename T>
+// VARLEN: grid = (max T, batch), rows as VarlenRows lays them out.
+template <typename T, bool VARLEN = false>
 __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                                const T* __restrict__ cos_t, const T* __restrict__ sin_t, T* __restrict__ k_cache,
                                                                T* __restrict__ v_cache, T* __restrict__ q_out, int pos0, int n_tok, int n_q,
-                                                               int n_kv, int L) {
-  const int t = (int)blockIdx.x, b = (int)blockIdx.y, p = pos0 + t;
+                                                               int n_kv, int L, const VarlenArg<VARLEN> vl) {
+  const int t = (int)blockIdx.x, b = (int)blockIdx.y;
+  long long row = (long long)b * n_tok + t;
+  if constexpr (VARLEN) {
+    if (t >= vl.n_tok[b]) return;  // past this slot's rows
+    pos0 = vl.pos0[b];
+    row = (long long)vl.row0[b] + t;
+  }
+  const int p = pos0 + t;
   {
-    const long long row = (long long)b * n_tok + t;
     q += row * n_q * kHd; q_out += row * n_q * kHd;
     k += row * n_kv * kHd; v += row * n_kv * kHd;
     k_cache += (long long)b * n_kv * L * kHd; v_cache += (long long)b * n_kv * L * kHd;
@@ -969,16 +993,25 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
 // Prefill into an 8-bit cache: rope_append_rows_kernel's RoPE, then every k and v row quantised as the kv8 decode kernel quantises
 // row pos (the same levels and meta bit for bit), and its dequantisation written to the staging caches at the same row.
 // grid = (T, batch), block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position (k and v of each kv head).
-// Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.
-template <typename T>
+// Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.  VARLEN as
+// rope_append_rows_kernel.
+template <typename T, bool VARLEN = false>
 __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                                    const T* __restrict__ cos_t, const T* __restrict__ sin_t, uint8_t* __restrict__ k_q,
                                                                    T* __restrict__ k_s, T* __restrict__ k_z, uint8_t* __restrict__ v_q,
                                                                    T* __restrict__ v_s, T* __restrict__ v_z, T* __restrict__ k_st, T* __restrict__ v_st,
-                                                                   T* __restrict__ q_out, int pos0, int n_tok, int n_q, int n_kv, int L, int gs) {
-  const int t = (int)blockIdx.x, b = (int)blockIdx.y, p = pos0 + t, ng = kHd / gs;
+                                                                   T* __restrict__ q_out, int pos0, int n_tok, int n_q, int n_kv, int L, int gs,
+                                                                   const VarlenArg<VARLEN> vl) {
+  const int t = (int)blockIdx.x, b = (int)blockIdx.y, ng = kHd / gs;
+  long long row = (long long)b * n_tok + t;
+  if constexpr (VARLEN) {
+    if (t >= vl.n_tok[b]) return;  // past this slot's rows
+    pos0 = vl.pos0[b];
+    row = (long long)vl.row0[b] + t;
+  }
+  const int p = pos0 + t;
   {
-    const long long row = (long long)b * n_tok + t, kv = (long long)b * n_kv;
+    const long long kv = (long long)b * n_kv;
     q += row * n_q * kHd; q_out += row * n_q * kHd;
     k += row * n_kv * kHd; v += row * n_kv * kHd;
     k_q += kv * L * kHd; v_q += kv * L * kHd; k_st += kv * L * kHd; v_st += kv * L * kHd;
@@ -1032,15 +1065,23 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
 
 // grid = (n_kv, batch, ceil(T G / 128)), block = 256: the query block is the slowest grid index, so the blocks with the longest key
 // range are dispatched first across all kv heads and sequences.  q (rotated) / out [batch T, n_q 128] (row b T + t), caches
-// [batch, n_kv, L, 128].
-template <typename T>
+// [batch, n_kv, L, 128].  VARLEN: grid = (n_kv, batch, ceil(max T G / 128)), rows as VarlenRows lays them out; the query blocks
+// past a slot's rows exit.
+template <typename T, bool VARLEN = false>
 __global__ void __launch_bounds__(kPreThreads, 1)
     attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k_cache, const T* __restrict__ v_cache, T* __restrict__ out, int pos0,
-                        int n_tok, int n_q, int n_kv, int L, float scale_log2) {
+                        int n_tok, int n_q, int n_kv, int L, float scale_log2, const VarlenArg<VARLEN> vl) {
   extern __shared__ __align__(16) char smem[];
   constexpr int ST = kPreStages;
   const int G = n_q / n_kv;
   const int rb = (int)(gridDim.z - 1 - blockIdx.z), kvh = (int)blockIdx.x, b = (int)blockIdx.y;  // longest query blocks first
+  long long qrow0 = (long long)b * n_tok;  // token row of the slot's first position
+  if constexpr (VARLEN) {
+    pos0 = vl.pos0[b];
+    n_tok = vl.n_tok[b];
+    qrow0 = vl.row0[b];
+    if (rb * kPreRows >= n_tok * G) return;  // past this slot's query rows
+  }
   const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
   {
     const long long kv = (long long)b * n_kv + kvh;
@@ -1055,8 +1096,8 @@ __global__ void __launch_bounds__(kPreThreads, 1)
   const int ra = wr0 + g, rb8 = wr0 + g + 8;
   const bool va = ra < n_rows, vb = rb8 < n_rows;
   const int pa = pos0 + (va ? ra / G : n_tok - 1), pb = pos0 + (vb ? rb8 / G : n_tok - 1);
-  const long long oa = ((long long)b * n_tok + (pa - pos0)) * n_q * kHd + (long long)(kvh * G + ra % G) * kHd;
-  const long long ob = ((long long)b * n_tok + (pb - pos0)) * n_q * kHd + (long long)(kvh * G + rb8 % G) * kHd;
+  const long long oa = (qrow0 + (pa - pos0)) * n_q * kHd + (long long)(kvh * G + ra % G) * kHd;
+  const long long ob = (qrow0 + (pb - pos0)) * n_q * kHd + (long long)(kvh * G + rb8 % G) * kHd;
   pdl_launch_dependents();
   pdl_wait();
 
@@ -1195,6 +1236,29 @@ int prefill_args(const char* name, int pos0, int n_tok, int n_q, int n_kv, int L
               name, hd, n_q, n_kv, L);
   HQQ_REQUIRE(n_tok >= 1 && pos0 >= 0 && n_tok <= L && pos0 <= L - n_tok, HQQ_E_INVALID, "%s: needs 1 <= T and pos0 + T <= cache_len (pos0=%d T=%d cache_len=%d)",
               name, pos0, n_tok, L);
+  return HQQ_OK;
+}
+
+// The checks of the three variable-length prefill entry points: the shape checks of prefill_args, then the host arrays pos0 / n_tok
+// of `batch` slots into vl (with the packed row offsets) and the longest slot's row count into max_t.
+int varlen_args(const char* name, const int* pos0, const int* n_tok, int n_q, int n_kv, int L, int hd, int batch, int dtype, VarlenRows& vl,
+                int& max_t) {
+  HQQ_REQUIRE(pos0 && n_tok, HQQ_E_INVALID, "%s: null pos0 / n_tok", name);
+  HQQ_REQUIRE(batch > 0 && batch <= kVarlenMaxBatch, HQQ_E_INVALID, "%s: batch %d (1 .. %d)", name, batch, kVarlenMaxBatch);
+  if (int rc = prefill_args(name, 0, 1, n_q, n_kv, L, hd, batch, dtype)) return rc;
+  long long rows = 0;
+  max_t = 0;
+  for (int b = 0; b < batch; ++b) {
+    HQQ_REQUIRE(n_tok[b] >= 0 && pos0[b] >= 0 && n_tok[b] <= L && pos0[b] <= L - n_tok[b], HQQ_E_INVALID,
+                "%s: slot %d needs 0 <= T, 0 <= pos0 and pos0 + T <= cache_len (pos0=%d T=%d cache_len=%d)", name, b, pos0[b], n_tok[b], L);
+    vl.pos0[b] = pos0[b];
+    vl.n_tok[b] = n_tok[b];
+    vl.row0[b] = (int)rows;
+    rows += n_tok[b];
+    max_t = max(max_t, n_tok[b]);
+    HQQ_REQUIRE(rows <= 65535, HQQ_E_INVALID, "%s: at most 65535 rows in all slots", name);
+  }
+  HQQ_REQUIRE(rows >= 1, HQQ_E_INVALID, "%s: needs at least one row", name);
   return HQQ_OK;
 }
 
@@ -1574,13 +1638,13 @@ extern "C" int hqq_b200_glue_silu_mul(const void* gate, const void* up, void* y,
   return HQQ_E_INVALID;
 }
 
-extern "C" int hqq_b200_glue_rope_attn_decode_batch(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                              void* k_cache, void* v_cache, const int64_t* pos, void* out, int n_q_heads, int n_kv_heads,
-                                              int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out, HQQ_E_INVALID, "hqq_b200_glue_rope_attn_decode: null pointer");
-  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "hqq_b200_glue_rope_attn_decode: batch %d", batch);
+static int rope_attn_decode_batch(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
+                                  const void* sin_table, void* k_cache, void* v_cache, const int64_t* pos, void* out, int n_q_heads, int n_kv_heads,
+                                  int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out, HQQ_E_INVALID, "%s: null pointer", name);
+  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
   HQQ_REQUIRE(head_dim == 128 && n_kv_heads > 0 && n_q_heads % n_kv_heads == 0 && cache_len > 0 && cache_len <= 8192, HQQ_E_UNSUPPORTED,
-              "hqq_b200_glue_rope_attn_decode: needs head_dim 128, cache_len <= 8192");
+              "%s: needs head_dim 128, cache_len <= 8192", name);
   cudaStream_t st = (cudaStream_t)stream;
   const int body = 2 * head_dim + cache_len > 8 * head_dim ? 2 * head_dim + cache_len : 8 * head_dim;
   const size_t smem = (size_t)(body + 32) * sizeof(float);
@@ -1591,12 +1655,31 @@ extern "C" int hqq_b200_glue_rope_attn_decode_batch(const void* q, const void* k
                       (const T*)cos_table, (const T*)sin_table, (T*)k_cache, (T*)v_cache, (const long long*)pos, (T*)out, n_q_heads, n_kv_heads,
                       cache_len, head_dim, scale);
   };
-  if (dtype == HQQ_F16) return batch > 1 ? go(rope_attn_decode_kernel<__half, true>, __half()) : go(rope_attn_decode_kernel<__half, false>, __half());
-  if (dtype == HQQ_BF16)
+  if (dtype == HQQ_F16) {
+    if (seqpos) return go(rope_attn_decode_kernel<__half, true, true>, __half());
+    return batch > 1 ? go(rope_attn_decode_kernel<__half, true>, __half()) : go(rope_attn_decode_kernel<__half, false>, __half());
+  }
+  if (dtype == HQQ_BF16) {
+    if (seqpos) return go(rope_attn_decode_kernel<__nv_bfloat16, true, true>, __nv_bfloat16());
     return batch > 1 ? go(rope_attn_decode_kernel<__nv_bfloat16, true>, __nv_bfloat16())
                      : go(rope_attn_decode_kernel<__nv_bfloat16, false>, __nv_bfloat16());
-  set_error("hqq_b200_glue_rope_attn_decode: dtype must be f16/bf16");
+  }
+  set_error("%s: dtype must be f16/bf16", name);
   return HQQ_E_INVALID;
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_batch(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                              void* k_cache, void* v_cache, const int64_t* pos, void* out, int n_q_heads, int n_kv_heads,
+                                              int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_attn_decode_batch("hqq_b200_glue_rope_attn_decode", false, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, n_q_heads,
+                                n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_batch_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                     void* k_cache, void* v_cache, const int64_t* pos, void* out, int n_q_heads, int n_kv_heads,
+                                                     int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_attn_decode_batch("hqq_b200_glue_rope_attn_decode_batch_seqpos", true, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out,
+                                n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
@@ -1613,16 +1696,25 @@ extern "C" size_t hqq_b200_glue_rope_attn_decode_split_workspace_bytes(int n_q_h
   return groups * s_max * (size_t)(n_q_heads / n_kv_heads) * (size_t)(head_dim + 2) * sizeof(float) + groups * sizeof(unsigned);
 }
 
-extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                    void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
-                                                    int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out && workspace, HQQ_E_INVALID,
-              "hqq_b200_glue_rope_attn_decode_split: null pointer");
-  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "hqq_b200_glue_rope_attn_decode_split: batch %d", batch);
-  HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0, HQQ_E_INVALID, "hqq_b200_glue_rope_attn_decode_split: workspace must be 4-byte aligned");
+template <typename T, bool SEQPOS>
+static int launch_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache, void* v_cache,
+                               const int64_t* pos, void* out, float* part, unsigned* tickets, int n_q_heads, int n_kv_heads, int cache_len,
+                               float scale_log2, dim3 grid, cudaStream_t st) {
+  if (int rc = reserve_smem<rope_attn_decode_split_kernel<T, SEQPOS>>(kSmemBytes)) return rc;
+  return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<T, SEQPOS>, grid, dim3(kSplitThreads), kSmemBytes, st, (const T*)q,
+                    (const T*)k, (const T*)v, (const T*)cos_table, (const T*)sin_table, (T*)k_cache, (T*)v_cache, (const long long*)pos, (T*)out,
+                    part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2);
+}
+
+static int rope_attn_decode_split(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
+                                  const void* sin_table, void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                  int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out && workspace, HQQ_E_INVALID, "%s: null pointer", name);
+  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
+  HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0, HQQ_E_INVALID, "%s: workspace must be 4-byte aligned", name);
   HQQ_REQUIRE(head_dim == kHd && n_kv_heads > 0 && n_kv_heads <= 65535 && n_q_heads % n_kv_heads == 0 && n_q_heads / n_kv_heads >= 1 &&
                   n_q_heads / n_kv_heads <= kSplitMaxGroup && cache_len > 0 && cache_len <= kSplitMaxLen,
-              HQQ_E_UNSUPPORTED, "hqq_b200_glue_rope_attn_decode_split: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072");
+              HQQ_E_UNSUPPORTED, "%s: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072", name);
   cudaStream_t st = (cudaStream_t)stream;
   const int S = split_count(n_kv_heads, cache_len);
   const int G = n_q_heads / n_kv_heads;
@@ -1631,28 +1723,33 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k
   unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
   const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
-  if (dtype == HQQ_F16) {
-    if (int rc = reserve_smem<rope_attn_decode_split_kernel<__half>>(kSmemBytes)) return rc;
-    return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<__half>, grid, dim3(kSplitThreads), kSmemBytes, st, (const __half*)q,
-                      (const __half*)k, (const __half*)v, (const __half*)cos_table, (const __half*)sin_table, (__half*)k_cache, (__half*)v_cache,
-                      (const long long*)pos, (__half*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2);
-  }
-  if (dtype == HQQ_BF16) {
-    if (int rc = reserve_smem<rope_attn_decode_split_kernel<__nv_bfloat16>>(kSmemBytes)) return rc;
-    return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<__nv_bfloat16>, grid, dim3(kSplitThreads), kSmemBytes, st,
-                      (const __nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (const __nv_bfloat16*)cos_table,
-                      (const __nv_bfloat16*)sin_table, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, (const long long*)pos, (__nv_bfloat16*)out,
-                      part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2);
-  }
-  set_error("hqq_b200_glue_rope_attn_decode_split: dtype must be f16/bf16");
+  auto go = [&](auto f) {
+    return f(q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2, grid, st);
+  };
+  if (dtype == HQQ_F16) return seqpos ? go(launch_decode_split<__half, true>) : go(launch_decode_split<__half, false>);
+  if (dtype == HQQ_BF16) return seqpos ? go(launch_decode_split<__nv_bfloat16, true>) : go(launch_decode_split<__nv_bfloat16, false>);
+  set_error("%s: dtype must be f16/bf16", name);
   return HQQ_E_INVALID;
 }
 
-extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
-                                                        const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
-                                                        int head_dim, int group_size, int batch, int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_rope_attn_decode_split_kv8";
+extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                    void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                    int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split", false, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, workspace,
+                                n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                           void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                           int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_seqpos", true, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out,
+                                workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
+static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
+                                      const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                      const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                      int group_size, int batch, int dtype, void* stream) {
   HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && pos && out && workspace, HQQ_E_INVALID,
               "%s: null pointer", name);
   HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
@@ -1669,17 +1766,35 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8(const void* q, const voi
   unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
   const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
-  auto go = [&](auto tag) {
+  auto go = [&](auto tag, auto sp) {
     using E = decltype(tag);
-    if (int rc = reserve_smem<rope_attn_decode_split_kv8_kernel<E>>(kKv8SmemBytes)) return rc;
-    return launch_pdl("rope_attn_decode_split_kv8", rope_attn_decode_split_kv8_kernel<E>, grid, dim3(kSplitThreads), kKv8SmemBytes, st, (const E*)q,
-                      (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q,
-                      (E*)v_scale, (E*)v_zero, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, group_size, scale_log2);
+    constexpr bool SP = decltype(sp)::value;
+    if (int rc = reserve_smem<rope_attn_decode_split_kv8_kernel<E, SP>>(kKv8SmemBytes)) return rc;
+    return launch_pdl("rope_attn_decode_split_kv8", rope_attn_decode_split_kv8_kernel<E, SP>, grid, dim3(kSplitThreads), kKv8SmemBytes, st,
+                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
+                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, group_size,
+                      scale_log2);
   };
-  if (dtype == HQQ_F16) return go(__half());
-  if (dtype == HQQ_BF16) return go(__nv_bfloat16());
+  if (dtype == HQQ_F16) return seqpos ? go(__half(), std::true_type()) : go(__half(), std::false_type());
+  if (dtype == HQQ_BF16) return seqpos ? go(__nv_bfloat16(), std::true_type()) : go(__nv_bfloat16(), std::false_type());
   set_error("%s: dtype must be f16/bf16", name);
   return HQQ_E_INVALID;
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                        const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
+                                                        int head_dim, int group_size, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv8", false, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
+                                    v_zero, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                               void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                               const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
+                                                               int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv8_seqpos", true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q,
+                                    v_scale, v_zero, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_q,
@@ -1696,7 +1811,28 @@ extern "C" int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, 
     using E = decltype(tag);
     return launch_pdl("rope_append_rows_kv8", rope_append_rows_kv8_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q,
                       (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q,
-                      (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0, T, n_q_heads, n_kv_heads, cache_len, group_size);
+                      (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0, T, n_q_heads, n_kv_heads, cache_len, group_size, NoVarlen());
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage,
+                                                         void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads,
+                                                         int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_kv8_varlen";
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
+              HQQ_E_INVALID, "%s: null pointer", name);
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows_kv8_varlen", rope_append_rows_kv8_kernel<E, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
+                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
+                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl);
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
@@ -1712,7 +1848,25 @@ extern "C" int hqq_b200_glue_rope_append_rows(const void* q, const void* k, cons
     using E = decltype(tag);
     return launch_pdl("rope_append_rows", rope_append_rows_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k,
                       (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, pos0, T, n_q_heads, n_kv_heads,
-                      cache_len);
+                      cache_len, NoVarlen());
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                     void* k_cache, void* v_cache, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                                     int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_varlen";
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && q_out, HQQ_E_INVALID, "%s: null pointer", name);
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows_varlen", rope_append_rows_kernel<E, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
+                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, 0, 0,
+                      n_q_heads, n_kv_heads, cache_len, vl);
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
@@ -1729,7 +1883,27 @@ extern "C" int hqq_b200_glue_attn_prefill(const void* q_rot, const void* k_cache
     using E = decltype(tag);
     if (int rc = reserve_smem<attn_prefill_kernel<E>>(kPreSmemBytes)) return rc;
     return launch_pdl("attn_prefill", attn_prefill_kernel<E>, grid, dim3(kPreThreads), kPreSmemBytes, st, (const E*)q_rot, (const E*)k_cache,
-                      (const E*)v_cache, (E*)out, pos0, T, n_q_heads, n_kv_heads, cache_len, scale_log2);
+                      (const E*)v_cache, (E*)out, pos0, T, n_q_heads, n_kv_heads, cache_len, scale_log2, NoVarlen());
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_attn_prefill_varlen(const void* q_rot, const void* k_cache, const void* v_cache, void* out, const int* pos0,
+                                                 const int* n_tok, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int dtype,
+                                                 void* stream) {
+  const char* name = "hqq_b200_glue_attn_prefill_varlen";
+  HQQ_REQUIRE(q_rot && k_cache && v_cache && out, HQQ_E_INVALID, "%s: null pointer", name);
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
+  const dim3 grid((unsigned)n_kv_heads, (unsigned)batch, (unsigned)cdiv((int64_t)max_t * (n_q_heads / n_kv_heads), kPreRows));  // z <= 8192
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    if (int rc = reserve_smem<attn_prefill_kernel<E, true>>(kPreSmemBytes)) return rc;
+    return launch_pdl("attn_prefill_varlen", attn_prefill_kernel<E, true>, grid, dim3(kPreThreads), kPreSmemBytes, st, (const E*)q_rot,
+                      (const E*)k_cache, (const E*)v_cache, (E*)out, 0, 0, n_q_heads, n_kv_heads, cache_len, scale_log2, vl);
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }

@@ -188,7 +188,7 @@ class DecodeModel:
                  device="cuda", cache_len: int = 256, tp: int = 1, rank: int = 0, seed: int = 0, process_group=None,
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
                  kv_bits: int = 16, kv_group_size: int = 64, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
-                 top_p: float = 1.0, sample_seed: int = 0):
+                 top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
         # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
         # top-k, top-p, then a Gumbel race on Philox numbers keyed by sample_seed and countered by _sample_ctr -- instead of the argmax.
@@ -217,7 +217,13 @@ class DecodeModel:
         self.batch = int(batch)
         if self.batch < 1:
             raise ValueError("batch must be >= 1")
-        if self.batch > 1 and fused:
+        # ragged: every sequence sits at its own position (self.pos is int64 [batch]); prefill takes prompts of different lengths in
+        # one packed pass and can refill one slot while the others keep their caches.  The decode steps run the _seqpos attention
+        # kernels, prefill the _varlen ones; everything else is row-independent at M = batch already.
+        self.ragged = bool(ragged)
+        if self.ragged and self.batch > 256:
+            raise ValueError("ragged batches hold at most 256 sequences")
+        if (self.batch > 1 or self.ragged) and fused:
             fused = True  # the 8-launch path with the batched glue kernels; the one-token kernels (fused=5) and their exchange are M = 1 only
         self.fused = fused
         import os
@@ -286,7 +292,8 @@ class DecodeModel:
         self.arange = torch.arange(cache_len, device=self.device)
         # static I/O for graph capture
         self.tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
-        self.pos = torch.zeros(1, dtype=torch.long, device=self.device)
+        self.pos = torch.zeros(self.batch if self.ragged else 1, dtype=torch.long, device=self.device)
+        self._slot_idx = torch.arange(self.batch, device=self.device)
         self.next_tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
         self._sample_ctr = torch.zeros(1, dtype=torch.long, device=self.device)  # Philox counter: + 1 per sampled token
         self.graph = None
@@ -309,14 +316,16 @@ class DecodeModel:
         from ._lib import check, ptr
         b = self._bufs
         if self.kv_bits == 8:
-            check(lib.hqq_b200_glue_rope_attn_decode_split_kv8(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                               ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
-                                                               ptr(blk["v_zero"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
-                                                               self.shape.head_dim, self.kv_group_size, self.batch, code, st))
+            fn = lib.hqq_b200_glue_rope_attn_decode_split_kv8_seqpos if self.ragged else lib.hqq_b200_glue_rope_attn_decode_split_kv8
+            check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                     ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
+                     ptr(blk["v_zero"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
+                     self.shape.head_dim, self.kv_group_size, self.batch, code, st))
             return
-        check(lib.hqq_b200_glue_rope_attn_decode_split(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                       ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
-                                                       self.shape.head_dim, self.batch, code, st))
+        fn = lib.hqq_b200_glue_rope_attn_decode_split_seqpos if self.ragged else lib.hqq_b200_glue_rope_attn_decode_split
+        check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                 ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
+                 self.shape.head_dim, self.batch, code, st))
 
     # bytes one decode step must read from HBM (SURVEY.md 8d): packed weights + meta + fp16 lm_head row-major
     def bytes_per_token(self, nbits=None, group_size=None) -> float:
@@ -345,16 +354,30 @@ class DecodeModel:
         B = self.batch
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         h = self.embed.index_select(0, self.tok)  # [B, hidden]
-        cos = self.cos.index_select(0, self.pos).view(1, 1, hd)
-        sin = self.sin.index_select(0, self.pos).view(1, 1, hd)
-        mask = (self.arange <= self.pos).view(1, 1, 1, self.cache_len)
+        if self.ragged:  # sequence b at position pos[b]: its own RoPE row and causal mask
+            cos = self.cos.index_select(0, self.pos).view(B, 1, hd)
+            sin = self.sin.index_select(0, self.pos).view(B, 1, hd)
+            mask = (self.arange.view(1, -1) <= self.pos.view(B, 1)).view(B, 1, 1, self.cache_len)
+        else:
+            cos = self.cos.index_select(0, self.pos).view(1, 1, hd)
+            sin = self.sin.index_select(0, self.pos).view(1, 1, hd)
+            mask = (self.arange <= self.pos).view(1, 1, 1, self.cache_len)
         for blk in self.blocks:
             x = F.rms_norm(h, (s.hidden,), blk["norm1"], s.rms_eps)
             q, k, v = self._multi(x, (blk["q"], blk["k"], blk["v"]))  # one launch: the three matrices share x
             q, k, v = q.view(B, hq, hd), k.view(B, hkv, hd), v.view(B, hkv, hd)
             q = self._rope(q, cos, sin)
             k = self._rope(k, cos, sin)
-            if self.kv_bits == 8:  # the rotated rows quantised into the cache; attention over the dequantised cache
+            if self.ragged:  # row pos[b] of sequence b
+                for name, x in (("k", k), ("v", v.view(B, hkv, hd))):
+                    if self.kv_bits == 8:
+                        lv, sc, ze = kv8_quantize_rows(x, self.kv_group_size)
+                        for suffix, val in (("_cache", lv), ("_scale", sc), ("_zero", ze)):
+                            blk[name + suffix][self._slot_idx, :, self.pos] = val
+                    else:
+                        blk[name + "_cache"][self._slot_idx, :, self.pos] = x
+                kc, vc = self._kv8_read(blk, self.cache_len) if self.kv_bits == 8 else (blk["k_cache"], blk["v_cache"])
+            elif self.kv_bits == 8:  # the rotated rows quantised into the cache; attention over the dequantised cache
                 self._kv8_write(blk, k.view(B, hkv, 1, hd), v.view(B, hkv, 1, hd), self.pos)
                 kc, vc = self._kv8_read(blk, self.cache_len)
             else:
@@ -513,9 +536,10 @@ class DecodeModel:
             if self.attn_kernel != "single":
                 self._attn_split(lib, blk, hq, hkv, code, st)
             else:
-                check(lib.hqq_b200_glue_rope_attn_decode_batch(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                               ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), hq, hkv, self.cache_len, hd, B, code,
-                                                               st))
+                fn = lib.hqq_b200_glue_rope_attn_decode_batch_seqpos if self.ragged else lib.hqq_b200_glue_rope_attn_decode_batch
+                check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                         ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), hq, hkv, self.cache_len, hd, B, code,
+                         st))
             self._lin(b["a"], (blk["o"],), [b["o"]])
             if self.tp > 1:
                 torch.distributed.all_reduce(b["o"], group=self.pg)
@@ -645,7 +669,11 @@ class DecodeModel:
         kv_bits 8: the rows kernel quantises k and v into the 8-bit cache as the decode kernel does and writes their dequantisation
         into a staging pair [batch, n_kv, cache_len, 128] in T (allocated once, shared by all layers); staging rows [0, start of the
         chunk) are dequantised from the cache per layer and chunk (hqq_b200_dequantize), and the attention kernel reads the staging
-        pair.  fused=False quantises into the cache and attends over its dequantisation."""
+        pair.  fused=False quantises into the cache and attends over its dequantisation.
+
+        ragged: see _prefill_ragged (`tokens` is a list of per-slot prompts or None)."""
+        if self.ragged:
+            return self._prefill_ragged(tokens, start, chunk)
         s, B = self.shape, self.batch
         tokens = torch.as_tensor(tokens, device=self.device)
         if tokens.dim() == 1 and B == 1:
@@ -672,15 +700,92 @@ class DecodeModel:
         self.pos.fill_((start + T) % self.cache_len)
         return self.tok.clone()
 
-    def _prefill_chunk_fused(self, ids, p0, hd, hq, hkv):
+    def _prefill_ragged(self, prompts, start=0, chunk=2048) -> torch.Tensor:
+        """Prefill of a ragged batch: `prompts` holds `batch` entries, each a 1-D token tensor or None (that slot's pos, tok and
+        caches stay as they are); a [batch, T] tensor stands for the equal-length list.  `start` is an int or one per slot.  Slot b
+        takes in its prompt at positions start_b .. start_b + T_b - 1.  Each chunk takes up to `chunk` tokens from every slot that
+        has tokens left (at most 65535 rows in all) and runs them packed in slot order through every block: the linears at
+        M = sum of the slots' rows, the _varlen RoPE / append and attention kernels.  With kv_bits 8 the staging rows [0, pos0) are
+        dequantised for the slots in the chunk only.  Each slot's last position goes through the final norm, the lm_head and the
+        pick (with do_sample: Philox row index = the slot, the counter advancing by one per call).  Afterwards pos[b] =
+        (start_b + T_b) mod cache_len and tok[b] holds the next token for every prefilled slot; tok is returned and last_logits holds
+        the prefilled slots' rows in slot order.  Refilling one slot -- continuous batching -- is a prefill with None for every other
+        slot: rows past the slot's new position are never read, so its old cache needs no clearing.
+        fused=False: each slot runs the lock-step reference walk (_prefill_chunk_ref) on its own cache."""
+        s, B, L = self.shape, self.batch, self.cache_len
+        if torch.is_tensor(prompts) and prompts.dim() == 2 and prompts.shape[0] == B:
+            prompts = list(prompts.unbind(0))
+        if not isinstance(prompts, (list, tuple)) or len(prompts) != B:
+            raise ValueError(f"prompts must be a list of batch={B} entries (1-D token tensors or None) or a [batch, T] tensor")
+        toks = []
+        for b, p in enumerate(prompts):
+            if p is None:
+                toks.append(None)
+                continue
+            t = torch.as_tensor(p, device=self.device)
+            if t.dim() != 1 or t.numel() < 1:
+                raise ValueError(f"prompt {b} must be a non-empty 1-D token tensor, got shape {tuple(t.shape)}")
+            toks.append(t.to(torch.long))
+        slots = [b for b in range(B) if toks[b] is not None]
+        if not slots:
+            raise ValueError("prefill needs at least one prompt")
+        starts = [start] * B if isinstance(start, int) else list(start)
+        if len(starts) != B:
+            raise ValueError(f"start must be an int or a list of batch={B} ints")
+        for b in slots:
+            T = int(toks[b].numel())
+            if not (isinstance(starts[b], int) and starts[b] >= 0 and starts[b] + T <= L):
+                raise ValueError(f"prompt {b}: positions [{starts[b]}, {starts[b] + T}) must lie in the cache [0, {L})")
+        chunk = min(int(chunk), 65535)
+        if chunk < 1:
+            raise ValueError("chunk must be >= 1")
+        hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
+        last = {}
+        with torch.no_grad():
+            if not self.fused:
+                for b in slots:
+                    T = int(toks[b].numel())
+                    for c0 in range(0, T, chunk):
+                        n = min(chunk, T - c0)
+                        h, delta = self._prefill_chunk_ref(toks[b][c0:c0 + n].view(1, n), starts[b] + c0, hd, hq, hkv, slot=b)
+                    last[b] = (h[-1], delta[-1])
+            else:
+                done = [0] * B
+                while any(toks[b] is not None and done[b] < toks[b].numel() for b in range(B)):
+                    budget, n_tok, pos0 = 65535, [0] * B, [0] * B
+                    for b in slots:
+                        n_tok[b] = min(chunk, int(toks[b].numel()) - done[b], budget)
+                        pos0[b] = starts[b] + done[b] if n_tok[b] else 0
+                        budget -= n_tok[b]
+                    ids = torch.cat([toks[b][done[b]:done[b] + n_tok[b]] for b in slots if n_tok[b]])
+                    h, delta = self._prefill_chunk_fused(ids.view(1, -1), 0, hd, hq, hkv, varlen=(pos0, n_tok))
+                    r = 0
+                    for b in range(B):
+                        r += n_tok[b]
+                        if n_tok[b]:
+                            done[b] += n_tok[b]
+                            if done[b] == toks[b].numel():
+                                last[b] = (h[r - 1], delta[r - 1])
+            tok = self._prefill_head(torch.stack([last[b][0] for b in slots]), torch.stack([last[b][1] for b in slots]), slots=slots)
+        idx = torch.tensor(slots, device=self.device)
+        self.tok.index_copy_(0, idx, tok)
+        self.pos.index_copy_(0, idx, torch.tensor([(starts[b] + int(toks[b].numel())) % L for b in slots], device=self.device))
+        return self.tok.clone()
+
+    def _prefill_chunk_fused(self, ids, p0, hd, hq, hkv, varlen=None):
         """One chunk on the package's kernels; returns the residual stream h [M, hidden] before the last block's MLP delta, and
-        that delta (the final norm adds them for the rows it needs)."""
+        that delta (the final norm adds them for the rows it needs).  varlen = (pos0, n_tok) host lists of the ragged batch's slots:
+        ids [1, M] packed in slot order and the _varlen kernels (p0 unused)."""
         from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
         lib, s = load(), self.shape
         st = stream_ptr(self.device)
         code = DTYPE_CODE[self.dtype]
         B, n = ids.shape
         M = B * n
+        if varlen is not None:
+            import ctypes
+            B = self.batch
+            vp0, vnt = (ctypes.c_int * B)(*varlen[0]), (ctypes.c_int * B)(*varlen[1])
         e = lambda w: torch.empty(M, w, device=self.device, dtype=self.dtype)
         h = self.embed.index_select(0, ids.reshape(-1))  # [M, hidden], row b * n + t
         x, q, k, v, qr, a, o = e(s.hidden), e(hq * hd), e(hkv * hd), e(hkv * hd), e(hq * hd), e(hq * hd), e(s.hidden)
@@ -699,20 +804,34 @@ class DecodeModel:
                 # kernel is the one of the fp16 cache, reading the staging pair
                 kst, vst = self._kv8_stage
                 for bi in range(B):
+                    sp0 = p0 if varlen is None else (varlen[0][bi] if varlen[1][bi] else 0)  # slots outside the chunk: nothing
                     for hh in range(hkv):
                         for c, dst in (("k", kst), ("v", vst)):
-                            if p0 > 0:
+                            if sp0 > 0:
                                 check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][bi, hh]), ptr(blk[c + "_scale"][bi, hh]), ptr(blk[c + "_zero"][bi, hh]),
-                                                              ptr(dst[bi, hh]), p0, hd, self.kv_group_size, 8, 1, code, st))
-                check(lib.hqq_b200_glue_rope_append_rows_kv8(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]),
-                                                             ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(kst),
-                                                             ptr(vst), ptr(qr), p0, n, hq, hkv, self.cache_len, hd, self.kv_group_size, B, code, st))
+                                                              ptr(dst[bi, hh]), sp0, hd, self.kv_group_size, 8, 1, code, st))
+                if varlen is not None:
+                    check(lib.hqq_b200_glue_rope_append_rows_kv8_varlen(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                                        ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
+                                                                        ptr(blk["v_zero"]), ptr(kst), ptr(vst), ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd,
+                                                                        self.kv_group_size, B, code, st))
+                else:
+                    check(lib.hqq_b200_glue_rope_append_rows_kv8(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]),
+                                                                 ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(kst),
+                                                                 ptr(vst), ptr(qr), p0, n, hq, hkv, self.cache_len, hd, self.kv_group_size, B, code, st))
                 kc, vc = kst, vst
+            elif varlen is not None:
+                check(lib.hqq_b200_glue_rope_append_rows_varlen(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                                ptr(blk["v_cache"]), ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd, B, code, st))
+                kc, vc = blk["k_cache"], blk["v_cache"]
             else:
                 check(lib.hqq_b200_glue_rope_append_rows(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
                                                          ptr(qr), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
                 kc, vc = blk["k_cache"], blk["v_cache"]
-            check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(kc), ptr(vc), ptr(a), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
+            if varlen is not None:
+                check(lib.hqq_b200_glue_attn_prefill_varlen(ptr(qr), ptr(kc), ptr(vc), ptr(a), vp0, vnt, hq, hkv, self.cache_len, hd, B, code, st))
+            else:
+                check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(kc), ptr(vc), ptr(a), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
             self._lin(a, (blk["o"],), [o])
             if self.tp > 1:
                 torch.distributed.all_reduce(o, group=self.pg)
@@ -725,8 +844,8 @@ class DecodeModel:
             delta = down
         return h, delta
 
-    def _prefill_chunk_ref(self, ids, p0, hd, hq, hkv):
-        """The same chunk on framework ops (fused=False)."""
+    def _prefill_chunk_ref(self, ids, p0, hd, hq, hkv, slot=None):
+        """The same chunk on framework ops (fused=False); slot: ids [1, n] of that slot only, on that slot's caches."""
         s = self.shape
         B, n = ids.shape
         M = B * n
@@ -736,6 +855,7 @@ class DecodeModel:
         mask = torch.arange(end, device=self.device).view(1, end) <= torch.arange(p0, end, device=self.device).view(n, 1)  # [n, end]
         delta = None
         for blk in self.blocks:
+            cb = blk if slot is None else {n: t[slot:slot + 1] for n, t in blk.items() if n.startswith(("k_", "v_"))}
             if delta is not None:
                 h = h + delta
             x = F.rms_norm(h, (s.hidden,), blk["norm1"], s.rms_eps)
@@ -743,12 +863,12 @@ class DecodeModel:
             q = self._rope(q.view(B, n, hq, hd), cos, sin)
             k = self._rope(k.view(B, n, hkv, hd), cos, sin)
             if self.kv_bits == 8:
-                self._kv8_write(blk, k.transpose(1, 2), v.view(B, n, hkv, hd).transpose(1, 2), torch.arange(p0, end, device=self.device))
-                kc, vc = self._kv8_read(blk, end)
+                self._kv8_write(cb, k.transpose(1, 2), v.view(B, n, hkv, hd).transpose(1, 2), torch.arange(p0, end, device=self.device))
+                kc, vc = self._kv8_read(cb, end)
             else:
-                blk["k_cache"][:, :, p0:end] = k.transpose(1, 2)
-                blk["v_cache"][:, :, p0:end] = v.view(B, n, hkv, hd).transpose(1, 2)
-                kc, vc = blk["k_cache"][:, :, :end], blk["v_cache"][:, :, :end]
+                cb["k_cache"][:, :, p0:end] = k.transpose(1, 2)
+                cb["v_cache"][:, :, p0:end] = v.view(B, n, hkv, hd).transpose(1, 2)
+                kc, vc = cb["k_cache"][:, :, :end], cb["v_cache"][:, :, :end]
             a = F.scaled_dot_product_attention(q.transpose(1, 2), kc, vc, attn_mask=mask, enable_gqa=True)
             o = blk["o"](a.transpose(1, 2).reshape(M, hq * hd))
             if self.tp > 1:
@@ -761,15 +881,25 @@ class DecodeModel:
                 torch.distributed.all_reduce(delta, group=self.pg)
         return h, delta
 
-    def _prefill_head(self, h, delta):
-        """Final norm, lm_head and greedy pick for the last position of each sequence: h, delta [batch, hidden]."""
-        s, B = self.shape, self.batch
+    def _prefill_head(self, h, delta, slots=None):
+        """Final norm, lm_head and greedy pick for the last position of each sequence: h, delta [batch, hidden].  slots (ragged): h,
+        delta hold the rows of those slots; with do_sample row b is drawn with Philox row index b, its slot."""
+        s, B = self.shape, h.shape[0]
+
+        def full(lg):  # do_sample on a ragged subset: the rows at their slots in a [batch, vocab / tp] block (the others discarded)
+            if slots is None:
+                return lg
+            f = torch.zeros(self.batch, lg.shape[1], dtype=lg.dtype, device=lg.device)
+            f[torch.tensor(slots, device=lg.device)] = lg
+            return f
+
+        pick = (lambda t: t) if slots is None else (lambda t: t[torch.tensor(slots, device=t.device)])
         if not self.fused:
             x = F.rms_norm(h + delta, (s.hidden,), self.final_norm, s.rms_eps)
             logits = torch.matmul(x, self.lm_head.t())
             self.last_logits = logits
             if self.do_sample:
-                tok = self._sample_ref(logits)
+                tok = pick(self._sample_ref(full(logits)))
                 self._sample_ctr.add_(1)
                 return tok
             if self.tp == 1:
@@ -788,10 +918,11 @@ class DecodeModel:
         check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(delta), ptr(self.final_norm), ptr(x), B, s.hidden, s.rms_eps, code, st))
         self.last_logits = torch.matmul(x, self.lm_head.t())
         if self.do_sample:
-            tok = torch.empty(B, dtype=torch.long, device=self.device)
-            self._sample(lib, self._sample_rows(self.last_logits, self._sample_buffers(B)), tok, code, st)
+            rows = full(self.last_logits)
+            tok = torch.empty(rows.shape[0], dtype=torch.long, device=self.device)
+            self._sample(lib, self._sample_rows(rows, self._sample_buffers(rows.shape[0])), tok, code, st)
             self._sample_ctr.add_(1)
-            return tok
+            return pick(tok)
         # the argmax kernel reads 16-byte vectors: every row starts on a 16-byte boundary whatever the vocabulary shard's length
         n = self.vocab_shard
         rows = torch.empty(B, -(-n // 8) * 8, dtype=self.dtype, device=self.device)

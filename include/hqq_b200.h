@@ -301,6 +301,50 @@ int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, const void*
 int hqq_b200_glue_attn_prefill(const void* q_rot, const void* k_cache, const void* v_cache, void* out,
                                int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                int batch, int dtype, void* stream);
+/* Ragged batches: the three decode attention entry points with one position per sequence.  Same arguments, layouts, split count,
+ * workspace (hqq_b200_glue_rope_attn_decode_split_workspace_bytes) and limits as hqq_b200_glue_rope_attn_decode_batch /
+ * _split / _split_kv8, except that pos is a device int64 [batch] and sequence b decodes at position pos[b]: its RoPE row, its
+ * cache row written, its attended rows 0 .. pos[b] and, for the split forms, its chunking all follow pos[b].  Sequence b's output
+ * and cache rows are bit for bit those of the lock-step entry point called with batch 1 on sequence b's slices at position pos[b].
+ * Every pos[b] and cache rows [0, pos[b]) of every sequence are read BEFORE the programmatic-dependency wait: they must have been
+ * written by an earlier, completed launch, not by the kernel directly in front of this one. */
+int hqq_b200_glue_rope_attn_decode_batch_seqpos(const void* q, const void* k, const void* v,
+                                                const void* cos_table, const void* sin_table,
+                                                void* k_cache, void* v_cache, const int64_t* pos, void* out,
+                                                int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_attn_decode_split_seqpos(const void* q, const void* k, const void* v,
+                                                const void* cos_table, const void* sin_table,
+                                                void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace,
+                                                int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_attn_decode_split_kv8_seqpos(const void* q, const void* k, const void* v,
+                                                    const void* cos_table, const void* sin_table,
+                                                    void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                    const int64_t* pos, void* out, void* workspace,
+                                                    int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                                    int batch, int dtype, void* stream);
+/* Variable-length prefill: the three prefill entry points with prompts of different lengths in one launch.  pos0 and n_tok are
+ * HOST arrays of `batch` entries: slot b contributes n_tok[b] >= 0 rows at positions pos0[b] .. pos0[b] + n_tok[b] - 1.  Token rows
+ * of q, k, v, q_out and out are packed in slot order: slot b's rows start at row n_tok[0] + ... + n_tok[b - 1] (with equal lengths
+ * T this is the b*T + t layout of the fixed-length calls).  A slot with n_tok[b] == 0 is neither read nor written.  Every row, cache
+ * row and attention row is bit for bit what the fixed-length entry point gives when called with batch 1 on that slot alone.
+ * Needs 1 <= batch <= 256, 0 <= pos0[b], pos0[b] + n_tok[b] <= cache_len, 1 <= n_tok[0] + ... + n_tok[batch - 1] <= 65535;
+ * the other limits are those of the fixed-length calls. */
+int hqq_b200_glue_rope_append_rows_varlen(const void* q, const void* k, const void* v,
+                                          const void* cos_table, const void* sin_table,
+                                          void* k_cache, void* v_cache, void* q_out, const int* pos0, const int* n_tok,
+                                          int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                          int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_kv8_varlen(const void* q, const void* k, const void* v,
+                                              const void* cos_table, const void* sin_table,
+                                              void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                              void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok,
+                                              int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                              int batch, int dtype, void* stream);
+int hqq_b200_glue_attn_prefill_varlen(const void* q_rot, const void* k_cache, const void* v_cache, void* out,
+                                      const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads, int cache_len,
+                                      int head_dim, int batch, int dtype, void* stream);
 /* out[0] = argmax(logits[0..n)) (first index on ties) */
 int hqq_b200_glue_argmax(const void* logits, int n, int64_t* out, int dtype, void* stream);
 /* Vocabulary-sharded lm_head (tensor parallel decode): out_key[0] = a signed 64-bit key {ordered(max) : 0xFFFFFFFF - (index_offset +
