@@ -71,6 +71,13 @@ SIGNATURES = {
     "hqq_b200_glue_rope_append_rows_varlen": (c_int, [c_void_p] * 10 + [c_int] * 6 + [c_void_p]),
     "hqq_b200_glue_rope_append_rows_kv8_varlen": (c_int, [c_void_p] * 16 + [c_int] * 7 + [c_void_p]),
     "hqq_b200_glue_attn_prefill_varlen": (c_int, [c_void_p] * 6 + [c_int] * 6 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_batch_paged": (c_int, [c_void_p] * 10 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_paged": (c_int, [c_void_p] * 11 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_kv8_paged": (c_int, [c_void_p] * 15 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_paged": (c_int, [c_void_p] * 11 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv8_paged": (c_int, [c_void_p] * 17 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_kv8_stage_paged": (c_int, [c_void_p] * 11 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_attn_prefill_paged": (c_int, [c_void_p] * 7 + [c_int] * 7 + [c_void_p]),
     "hqq_b200_glue_argmax": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_key": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_tp": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),

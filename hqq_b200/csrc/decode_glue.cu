@@ -135,6 +135,21 @@ __global__ void __launch_bounds__(256) silu_mul_kernel(const T* __restrict__ g, 
   }
 }
 
+// Paged KV cache (PAGED instantiations of the ragged kernels): a cache is a pool of pages [pages, n_kv, 64, 128], a page holding 64
+// positions of one sequence for every kv head, and row p of slot b, kv head h lives at row (table[b][p / 64] n_kv + h) 64 + p % 64 of
+// the pool; table is int32 [batch, L / 64].  Decode tiles (16 positions) and prefill tiles (64), aligned to absolute positions, never
+// straddle a page: one table read per tile.  Nothing else changes -- arithmetic, tiling, chunks, tickets, merge order.  Like pos, the
+// table entries are read before griddepcontrol.wait, so they must have been written by an earlier, completed launch.
+constexpr int kPage = 64;
+struct PageTable { const int* table; };
+struct NoPages {};  // the contiguous-cache instantiations
+template <bool PAGED> using PageArg = typename std::conditional<PAGED, PageTable, NoPages>::type;
+
+// pool row of position p of kv head kvh through the slot's table row tab
+__device__ __forceinline__ long long page_row(const int* tab, int n_kv, int kvh, int p) {
+  return ((long long)tab[p >> 6] * n_kv + kvh) * kPage + (p & (kPage - 1));
+}
+
 // RoPE (rotate-half, cos/sin tables [L, hd]) + KV-cache append + single-token GQA attention over cache[0..pos].
 // grid = n_q_heads, block = 256 threads (8 warps).  caches are [n_kv_heads, L, hd], hd = 128.
 // The step streams ~5 GB of weights between two visits of a layer's cache, so the rows are cold in DRAM and the kernel is
@@ -143,12 +158,14 @@ __global__ void __launch_bounds__(256) silu_mul_kernel(const T* __restrict__ g, 
 // a step, a full barrier); (2) both position loops keep 8-16 independent loads in flight per thread.
 // SEQPOS (ragged batches, BATCH only): sequence b sits at its own position pos_p[b], and everything derived from the position --
 // the prefetched rows, the RoPE row, the written row, the loop bounds -- follows it.
+// PAGED (SEQPOS only): the caches are page pools and every row, the prefetched ones included, is found through the slot's table row.
 constexpr int kAttnThreads = 256;
-template <typename T, bool BATCH, bool SEQPOS = false>
+template <typename T, bool BATCH, bool SEQPOS = false, bool PAGED = false>
 __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in,
                                                                         const T* __restrict__ cos_t, const T* __restrict__ sin_t,
                                                                         T* __restrict__ k_cache, T* __restrict__ v_cache, const long long* __restrict__ pos_p,
-                                                                        T* __restrict__ out, int n_q, int n_kv, int L, int hd, float scale) {
+                                                                        T* __restrict__ out, int n_q, int n_kv, int L, int hd, float scale,
+                                                                        const PageArg<PAGED> pg) {
   extern __shared__ float sm[];  // q[hd] | knew[hd] | p[L]  (later reused as [8][hd] partial outputs) | red[32]
   constexpr int NW = kAttnThreads / 32;
   float* qs = sm;
@@ -160,12 +177,29 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
     const long long b = blockIdx.y;  // instantiation is the kernel as it was (its position loops lost 1 us per layer at 200
     q_in += b * n_q * hd; out += b * n_q * hd;  // cached positions when the offsets were applied unconditionally)
     k_in += b * n_kv * hd; v_in += b * n_kv * hd;
-    k_cache += b * n_kv * L * hd; v_cache += b * n_kv * L * hd;
+    if constexpr (!PAGED) { k_cache += b * n_kv * L * hd; v_cache += b * n_kv * L * hd; }
   }
   static_assert(BATCH || !SEQPOS, "per-sequence positions need the batch layout");
+  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
+  const int* tab = nullptr;
+  if constexpr (PAGED) tab = pg.table + (long long)blockIdx.y * (L / kPage);
+  // cache row (in units of hd elements) of position t of this head
+  auto row = [&](int t) -> long long {
+    if constexpr (PAGED) return page_row(tab, n_kv, kvh, t);
+    else return (long long)kvh * L + t;
+  };
   const int pos = (int)pos_p[SEQPOS ? blockIdx.y : 0];
   pdl_launch_dependents();
-  {
+  if constexpr (PAGED) {
+    // the same lines page by page: a row is two 128-byte lines (hd 128, 16-bit T)
+    const char* kb = reinterpret_cast<const char*>(k_cache);
+    const char* vb = reinterpret_cast<const char*>(v_cache);
+    for (int i = d; i < 2 * pos; i += kAttnThreads) {
+      const long long off = row(i >> 1) * (hd * (int)sizeof(T)) + ((i & 1) << 7);
+      prefetch_l2(kb + off);
+      prefetch_l2(vb + off);
+    }
+  } else {
     // one 128-byte line per prefetch; pos rows of hd * sizeof(T) bytes each in both caches
     const char* kb = reinterpret_cast<const char*>(k_cache + (long long)kvh * L * hd);
     const char* vb = reinterpret_cast<const char*>(v_cache + (long long)kvh * L * hd);
@@ -188,8 +222,8 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
     const T kn = from_f32<T>(to_f32<T>(from_f32<T>(kx * c)) + to_f32<T>(from_f32<T>(kr * s)));
     ks[d] = to_f32<T>(kn);
     if (h % (n_q / n_kv) == 0) {  // one head of the group owns the cache write
-      k_cache[((long long)kvh * L + pos) * hd + d] = kn;
-      v_cache[((long long)kvh * L + pos) * hd + d] = v_in[kvh * hd + d];
+      k_cache[row(pos) * hd + d] = kn;
+      v_cache[row(pos) * hd + d] = v_in[kvh * hd + d];
     }
   }
   __syncthreads();
@@ -201,7 +235,7 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
     if (t == pos) {
       for (int i = 0; i < hd; ++i) acc += qs[i] * ks[i];
     } else {
-      const T* kr = k_cache + ((long long)kvh * L + t) * hd;
+      const T* kr = k_cache + row(t) * hd;
       Vec<T, 8> kv[16];
 #pragma unroll
       for (int i = 0; i < 16; ++i) kv[i] = *reinterpret_cast<const Vec<T, 8>*>(kr + i * 8);
@@ -237,11 +271,15 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
     const int w = d >> 5, l = d & 31;
     float o4[4] = {0.f, 0.f, 0.f, 0.f};
     const T* vbase = v_cache + (long long)kvh * L * hd + 4 * l;
+    auto vrow = [&](int t) -> const T* {  // lane's four dims of position t
+      if constexpr (PAGED) return v_cache + row(t) * hd + 4 * l;
+      else return vbase + (long long)t * hd;
+    };
     int t = w;
     for (; t + 7 * NW < pos; t += 8 * NW) {
       Vec<T, 4> vv[8];
 #pragma unroll
-      for (int u = 0; u < 8; ++u) vv[u] = *reinterpret_cast<const Vec<T, 4>*>(vbase + (long long)(t + u * NW) * hd);
+      for (int u = 0; u < 8; ++u) vv[u] = *reinterpret_cast<const Vec<T, 4>*>(vrow(t + u * NW));
 #pragma unroll
       for (int u = 0; u < 8; ++u) {
         const float pt = ps[t + u * NW];
@@ -250,7 +288,7 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
       }
     }
     for (; t < pos; t += NW) {
-      const Vec<T, 4> vv = *reinterpret_cast<const Vec<T, 4>*>(vbase + (long long)t * hd);
+      const Vec<T, 4> vv = *reinterpret_cast<const Vec<T, 4>*>(vrow(t));
       const float pt = ps[t];
 #pragma unroll
       for (int j = 0; j < 4; ++j) o4[j] += pt * to_f32<T>(vv.v[j]);
@@ -369,20 +407,24 @@ __device__ __forceinline__ void split_merge(const float* wp, float* __restrict__
 // grid = (S, n_kv, batch), block = 256.  q / out [batch, n_q * 128], k / v [batch, n_kv * 128], caches [batch, n_kv, L, 128].
 // part: [batch, n_kv, S, G, 2 + 128] floats (m, l, o per head), tickets: [batch, n_kv] uint32, zero between launches.
 // SEQPOS: sequence b at its own position pos_p[b]; its chunk, staged rows, RoPE row and written row follow it (S stays fixed).
-template <typename T, bool SEQPOS = false>
+// PAGED (SEQPOS only): caches are page pools [pages, n_kv, 64, 128]; a tile's rows are found with one read of the table row.
+template <typename T, bool SEQPOS = false, bool PAGED = false>
 __global__ void __launch_bounds__(kSplitThreads, 1)
     rope_attn_decode_split_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
                                   const T* __restrict__ sin_t, T* __restrict__ k_cache, T* __restrict__ v_cache, const long long* __restrict__ pos_p,
                                   T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
-                                  float scale_log2) {
+                                  float scale_log2, const PageArg<PAGED> pg) {
   extern __shared__ __align__(16) char smem[];
   constexpr int NW = kSplitWarps, ST = kSplitStages;
   const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
   const int G = n_q / n_kv;
   const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
+  const int* tab = nullptr;
+  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
   {
     const long long kv = (long long)b * n_kv + kvh;
-    k_cache += kv * L * kHd; v_cache += kv * L * kHd;
+    if constexpr (!PAGED) { k_cache += kv * L * kHd; v_cache += kv * L * kHd; }
     k_in += kv * kHd; v_in += kv * kHd;
     q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
     part += kv * S * G * kPartFloats;
@@ -408,12 +450,14 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
     if (i < my_tiles) {
       const int t0 = c0 + (warp + i * NW) * kSplitTile;
       char* st = ring + (i % ST) * kStageBytes;
+      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
+      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
 #pragma unroll 4
       for (int j = lane; j < 2 * kSplitTile * 16; j += 32) {
         const int isv = j >> 8, r = (j >> 4) & 15, c = j & 15, p = t0 + r;
         char* dst = st + isv * kTileBytes + swz(r, c);
         if (p < pos) {
-          split_cp16(dst, (isv ? v_cache : k_cache) + (long long)p * kHd + c * 8);
+          split_cp16(dst, (isv ? v_cache : k_cache) + (rt + p) * kHd + c * 8);
         } else if (p > pos || fresh) {
           uint4 val;
           val.x = val.y = val.z = val.w = 0u;
@@ -443,8 +487,10 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
       kf[d] = r;
       vf[d] = v_in[d];
       if (split == 0) {  // one writer per (sequence, kv head); no CTA of this launch reads cache row pos
-        k_cache[(long long)pos * kHd + d] = r;
-        v_cache[(long long)pos * kHd + d] = v_in[d];
+        long long pr = pos;
+        if constexpr (PAGED) pr = page_row(tab, n_kv, kvh, pos);
+        k_cache[pr * kHd + d] = r;
+        v_cache[pr * kHd + d] = v_in[d];
       }
     }
   }
@@ -658,23 +704,29 @@ static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kKv8RingBytes, "
 __device__ __forceinline__ int swz8(int r, int c) { return r * kHd + ((c ^ (r & 7)) << 4); }  // 16-byte chunk c of level row r
 
 // grid = (S, n_kv, batch), block = 256.  q / out, k / v as rope_attn_decode_split_kernel; levels [batch, n_kv, L, 128] uint8, meta
-// [batch, n_kv, L, 128 / gs] T; part / tickets as there.  SEQPOS as there.
-template <typename T, bool SEQPOS = false>
+// [batch, n_kv, L, 128 / gs] T; part / tickets as there.  SEQPOS and PAGED as there (paged levels [pages, n_kv, 64, 128], meta
+// [pages, n_kv, 64, 128 / gs]).
+template <typename T, bool SEQPOS = false, bool PAGED = false>
 __global__ void __launch_bounds__(kSplitThreads, 1)
     rope_attn_decode_split_kv8_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
                                       const T* __restrict__ sin_t, uint8_t* __restrict__ k_q, T* __restrict__ k_s, T* __restrict__ k_z,
                                       uint8_t* __restrict__ v_q, T* __restrict__ v_s, T* __restrict__ v_z, const long long* __restrict__ pos_p,
                                       T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
-                                      int gs, float scale_log2) {
+                                      int gs, float scale_log2, const PageArg<PAGED> pg) {
   extern __shared__ __align__(16) char smem[];
   constexpr int NW = kSplitWarps, ST = kKv8Stages;
   const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
   const int G = n_q / n_kv, ng = kHd / gs;
   const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
+  const int* tab = nullptr;
+  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
   {
     const long long kv = (long long)b * n_kv + kvh;
-    k_q += kv * L * kHd; v_q += kv * L * kHd;
-    k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+    if constexpr (!PAGED) {
+      k_q += kv * L * kHd; v_q += kv * L * kHd;
+      k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+    }
     k_in += kv * kHd; v_in += kv * kHd;
     q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
     part += kv * S * G * kPartFloats;
@@ -703,12 +755,14 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
     if (i < my_tiles) {
       const int t0 = c0 + (warp + i * NW) * kSplitTile;
       char* st = ring + (i % ST) * kKv8StageBytes;
+      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
+      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
 #pragma unroll 4
       for (int j = lane; j < 2 * kSplitTile * 8; j += 32) {
         const int isv = j >> 7, r = (j >> 3) & 15, c = j & 7, p = t0 + r;
         char* dst = st + isv * kKv8LvlBytes + swz8(r, c);
         if (p < pos) {
-          split_cp16(dst, (isv ? v_q : k_q) + (long long)p * kHd + c * 16);
+          split_cp16(dst, (isv ? v_q : k_q) + (rt + p) * kHd + c * 16);
         } else if (p > pos || fresh) {
           uint4 val;
           val.x = val.y = val.z = val.w = 0u;
@@ -718,7 +772,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
       }
       if (lane < 8 * ng) {  // 4 arrays x 2 ng chunks
         const int a = lane / (2 * ng), j = lane % (2 * ng), rows = 8 / ng, r0 = j * rows;
-        const T* src = (a == 0 ? k_s : a == 1 ? k_z : a == 2 ? v_s : v_z) + (long long)(t0 + r0) * ng;
+        const T* src = (a == 0 ? k_s : a == 1 ? k_z : a == 2 ? v_s : v_z) + (rt + (t0 + r0)) * ng;
         char* dst = st + 2 * kKv8LvlBytes + a * kKv8MetaBytes + j * 16;
         if (t0 + r0 + rows <= pos && ((uintptr_t)src & 15) == 0) {
           split_cp16(dst, src);
@@ -765,10 +819,12 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
     const int grp = 4 * lane / gs;
     if ((4 * lane) % gs == 0) { fm[4 * warp + grp] = sc; fm[4 * warp + 2 + grp] = ze; }
     if (split == 0) {
-      *reinterpret_cast<uint32_t*>((warp ? v_q : k_q) + (long long)pos * kHd + 4 * lane) = q;
+      long long pr = pos;
+      if constexpr (PAGED) pr = page_row(tab, n_kv, kvh, pos);
+      *reinterpret_cast<uint32_t*>((warp ? v_q : k_q) + pr * kHd + 4 * lane) = q;
       if ((4 * lane) % gs == 0) {
-        (warp ? v_s : k_s)[(long long)pos * ng + grp] = sc;
-        (warp ? v_z : k_z)[(long long)pos * ng + grp] = ze;
+        (warp ? v_s : k_s)[pr * ng + grp] = sc;
+        (warp ? v_z : k_z)[pr * ng + grp] = ze;
       }
     }
   }
@@ -951,12 +1007,14 @@ struct NoVarlen {};  // the fixed-length instantiations: their uniform pos0 / T 
 template <bool VARLEN> using VarlenArg = typename std::conditional<VARLEN, VarlenRows, NoVarlen>::type;
 
 // grid = (T, batch), block = 256.  q / q_out [batch T, n_q 128], k / v [batch T, n_kv 128] (row b T + t), caches [batch, n_kv, L, 128].
-// VARLEN: grid = (max T, batch), rows as VarlenRows lays them out.
-template <typename T, bool VARLEN = false>
+// VARLEN: grid = (max T, batch), rows as VarlenRows lays them out.  PAGED (VARLEN only): page pools, the CTA's position found with one
+// table read.
+template <typename T, bool VARLEN = false, bool PAGED = false>
 __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                                const T* __restrict__ cos_t, const T* __restrict__ sin_t, T* __restrict__ k_cache,
                                                                T* __restrict__ v_cache, T* __restrict__ q_out, int pos0, int n_tok, int n_q,
-                                                               int n_kv, int L, const VarlenArg<VARLEN> vl) {
+                                                               int n_kv, int L, const VarlenArg<VARLEN> vl, const PageArg<PAGED> pg) {
+  static_assert(VARLEN || !PAGED, "a paged cache needs the variable-length layout");
   const int t = (int)blockIdx.x, b = (int)blockIdx.y;
   long long row = (long long)b * n_tok + t;
   if constexpr (VARLEN) {
@@ -968,8 +1026,10 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
   {
     q += row * n_q * kHd; q_out += row * n_q * kHd;
     k += row * n_kv * kHd; v += row * n_kv * kHd;
-    k_cache += (long long)b * n_kv * L * kHd; v_cache += (long long)b * n_kv * L * kHd;
+    if constexpr (!PAGED) { k_cache += (long long)b * n_kv * L * kHd; v_cache += (long long)b * n_kv * L * kHd; }
   }
+  long long c0 = 0;  // PAGED: pool row of position p of kv head 0
+  if constexpr (PAGED) c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
   pdl_launch_dependents();
   pdl_wait();
   constexpr int half = kHd / 2;
@@ -982,10 +1042,12 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
       const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
       const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
       if (h < n_q) q_out[h * kHd + d] = r;
+      else if constexpr (PAGED) k_cache[(c0 + (long long)(h - n_q) * kPage) * kHd + d] = r;
       else k_cache[((long long)(h - n_q) * L + p) * kHd + d] = r;
     } else {
       const int kvh = h - n_q - n_kv;
-      v_cache[((long long)kvh * L + p) * kHd + d] = v[kvh * kHd + d];
+      if constexpr (PAGED) v_cache[(c0 + (long long)kvh * kPage) * kHd + d] = v[kvh * kHd + d];
+      else v_cache[((long long)kvh * L + p) * kHd + d] = v[kvh * kHd + d];
     }
   }
 }
@@ -994,14 +1056,15 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
 // row pos (the same levels and meta bit for bit), and its dequantisation written to the staging caches at the same row.
 // grid = (T, batch), block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position (k and v of each kv head).
 // Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.  VARLEN as
-// rope_append_rows_kernel.
-template <typename T, bool VARLEN = false>
+// rope_append_rows_kernel.  PAGED as there: levels and meta in the page pools, the staging pair stays [batch, n_kv, L, 128].
+template <typename T, bool VARLEN = false, bool PAGED = false>
 __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                                    const T* __restrict__ cos_t, const T* __restrict__ sin_t, uint8_t* __restrict__ k_q,
                                                                    T* __restrict__ k_s, T* __restrict__ k_z, uint8_t* __restrict__ v_q,
                                                                    T* __restrict__ v_s, T* __restrict__ v_z, T* __restrict__ k_st, T* __restrict__ v_st,
                                                                    T* __restrict__ q_out, int pos0, int n_tok, int n_q, int n_kv, int L, int gs,
-                                                                   const VarlenArg<VARLEN> vl) {
+                                                                   const VarlenArg<VARLEN> vl, const PageArg<PAGED> pg) {
+  static_assert(VARLEN || !PAGED, "a paged cache needs the variable-length layout");
   const int t = (int)blockIdx.x, b = (int)blockIdx.y, ng = kHd / gs;
   long long row = (long long)b * n_tok + t;
   if constexpr (VARLEN) {
@@ -1014,9 +1077,15 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
     const long long kv = (long long)b * n_kv;
     q += row * n_q * kHd; q_out += row * n_q * kHd;
     k += row * n_kv * kHd; v += row * n_kv * kHd;
-    k_q += kv * L * kHd; v_q += kv * L * kHd; k_st += kv * L * kHd; v_st += kv * L * kHd;
-    k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+    if constexpr (!PAGED) {
+      k_q += kv * L * kHd; v_q += kv * L * kHd; k_st += kv * L * kHd; v_st += kv * L * kHd;
+      k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+    } else {
+      k_st += kv * L * kHd; v_st += kv * L * kHd;
+    }
   }
+  long long c0 = 0;  // PAGED: pool row of position p of kv head 0
+  if constexpr (PAGED) c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
   pdl_launch_dependents();
   pdl_wait();
   constexpr int half = kHd / 2;
@@ -1048,10 +1117,12 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
     T sc, ze;
     const uint32_t lv = kv8_quant4<T>(x, gs, sc, ze);
     const long long row = (long long)kvh * L + p;
-    *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + row * kHd + 4 * lane) = lv;
+    long long crow = row;
+    if constexpr (PAGED) crow = c0 + (long long)kvh * kPage;
+    *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + crow * kHd + 4 * lane) = lv;
     if ((4 * lane) % gs == 0) {
-      (isv ? v_s : k_s)[row * ng + 4 * lane / gs] = sc;
-      (isv ? v_z : k_z)[row * ng + 4 * lane / gs] = ze;
+      (isv ? v_s : k_s)[crow * ng + 4 * lane / gs] = sc;
+      (isv ? v_z : k_z)[crow * ng + 4 * lane / gs] = ze;
     }
     typename Pair<T>::type s2, z2;
     s2.x = s2.y = sc;
@@ -1063,14 +1134,45 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
   }
 }
 
+// Prefill into a paged 8-bit cache: staging rows [0, pos0[b]) of every slot with n_tok[b] > 0, dequantised from the page pools through
+// the table with the rows kernel's arithmetic (kv8_deq2: T(T(q - z) * s), what hqq_b200_dequantize gives).  grid = (max pos0, batch),
+// block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position, four elements per lane.  The table is read before the
+// wait, the pools after it.
+template <typename T>
+__global__ void __launch_bounds__(256) kv8_stage_paged_kernel(const uint8_t* __restrict__ k_q, const T* __restrict__ k_s, const T* __restrict__ k_z,
+                                                              const uint8_t* __restrict__ v_q, const T* __restrict__ v_s, const T* __restrict__ v_z,
+                                                              T* __restrict__ k_st, T* __restrict__ v_st, int n_kv, int L, int gs, const VarlenRows vl,
+                                                              const PageTable pg) {
+  const int p = (int)blockIdx.x, b = (int)blockIdx.y, ng = kHd / gs;
+  if (vl.n_tok[b] == 0 || p >= vl.pos0[b]) return;  // slot outside the chunk, or a row the rows kernel writes
+  const long long c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
+  pdl_launch_dependents();
+  pdl_wait();
+  const int warp = (int)threadIdx.x >> 5, lane = (int)threadIdx.x & 31;
+  for (int r = warp; r < 2 * n_kv; r += (int)blockDim.x >> 5) {
+    const int kvh = r >> 1, isv = r & 1, grp = 4 * lane / gs;
+    const long long crow = c0 + (long long)kvh * kPage;
+    const uint32_t lv = *reinterpret_cast<const uint32_t*>((isv ? v_q : k_q) + crow * kHd + 4 * lane);
+    typename Pair<T>::type s2, z2;
+    s2.x = s2.y = (isv ? v_s : k_s)[crow * ng + grp];
+    z2.x = z2.y = (isv ? v_z : k_z)[crow * ng + grp];
+    uint2 y;
+    y.x = kv8_deq2<T, 0>(lv, z2, s2);
+    y.y = kv8_deq2<T, 1>(lv, z2, s2);
+    *reinterpret_cast<uint2*>((isv ? v_st : k_st) + (((long long)b * n_kv + kvh) * L + p) * kHd + 4 * lane) = y;
+  }
+}
+
 // grid = (n_kv, batch, ceil(T G / 128)), block = 256: the query block is the slowest grid index, so the blocks with the longest key
 // range are dispatched first across all kv heads and sequences.  q (rotated) / out [batch T, n_q 128] (row b T + t), caches
 // [batch, n_kv, L, 128].  VARLEN: grid = (n_kv, batch, ceil(max T G / 128)), rows as VarlenRows lays them out; the query blocks
-// past a slot's rows exit.
-template <typename T, bool VARLEN = false>
+// past a slot's rows exit.  PAGED (VARLEN only): page pools, one table read per 64-position tile (a tile is one page).
+template <typename T, bool VARLEN = false, bool PAGED = false>
 __global__ void __launch_bounds__(kPreThreads, 1)
     attn_prefill_kernel(const T* __restrict__ q, const T* __restrict__ k_cache, const T* __restrict__ v_cache, T* __restrict__ out, int pos0,
-                        int n_tok, int n_q, int n_kv, int L, float scale_log2, const VarlenArg<VARLEN> vl) {
+                        int n_tok, int n_q, int n_kv, int L, float scale_log2, const VarlenArg<VARLEN> vl, const PageArg<PAGED> pg) {
+  static_assert(VARLEN || !PAGED, "a paged cache needs the variable-length layout");
+  static_assert(kPreTile == kPage, "a prefill tile is one page");
   extern __shared__ __align__(16) char smem[];
   constexpr int ST = kPreStages;
   const int G = n_q / n_kv;
@@ -1083,10 +1185,12 @@ __global__ void __launch_bounds__(kPreThreads, 1)
     if (rb * kPreRows >= n_tok * G) return;  // past this slot's query rows
   }
   const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
-  {
+  if constexpr (!PAGED) {
     const long long kv = (long long)b * n_kv + kvh;
     k_cache += kv * L * kHd; v_cache += kv * L * kHd;
   }
+  const int* tab = nullptr;
+  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
   const int n_rows = n_tok * G, row0 = rb * kPreRows;
   const int n_tiles = (pos0 + (min(row0 + kPreRows, n_rows) - 1) / G) / kPreTile + 1;  // through the CTA's last position
   const int lim = pos0 + n_tok;                                                          // rows >= lim are never loaded
@@ -1105,12 +1209,14 @@ __global__ void __launch_bounds__(kPreThreads, 1)
     if (j < n_tiles) {
       const int t0 = j * kPreTile;
       char* st = smem + (j % ST) * kPreStageBytes;
+      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
+      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
 #pragma unroll 4
       for (int c = tid; c < 2 * kPreTile * 16; c += kPreThreads) {
         const int isv = c >> 10, r = (c >> 4) & (kPreTile - 1), ch = c & 15, p = t0 + r;
         char* dst = st + isv * kPreTileBytes + swz(r, ch);
         if (p < lim) {
-          split_cp16(dst, (isv ? v_cache : k_cache) + (long long)p * kHd + ch * 8);
+          split_cp16(dst, (isv ? v_cache : k_cache) + (rt + p) * kHd + ch * 8);
         } else {
           uint4 z;
           z.x = z.y = z.z = z.w = 0u;
@@ -1638,9 +1744,18 @@ extern "C" int hqq_b200_glue_silu_mul(const void* gate, const void* up, void* y,
   return HQQ_E_INVALID;
 }
 
+// The checks every paged entry point adds: a table, whole pages, at least one page besides the sink.
+static int paged_args(const char* name, const int* table, int cache_len, int n_pages) {
+  HQQ_REQUIRE(table, HQQ_E_INVALID, "%s: null page table", name);
+  HQQ_REQUIRE(cache_len > 0 && cache_len % kPage == 0, HQQ_E_INVALID, "%s: cache_len must be a multiple of %d (got %d)", name, kPage, cache_len);
+  HQQ_REQUIRE(n_pages >= 1, HQQ_E_INVALID, "%s: n_pages must be >= 1 (got %d)", name, n_pages);
+  return HQQ_OK;
+}
+
+// table == nullptr: contiguous caches; else page pools (seqpos only)
 static int rope_attn_decode_batch(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
-                                  const void* sin_table, void* k_cache, void* v_cache, const int64_t* pos, void* out, int n_q_heads, int n_kv_heads,
-                                  int cache_len, int head_dim, int batch, int dtype, void* stream) {
+                                  const void* sin_table, void* k_cache, void* v_cache, const int* table, const int64_t* pos, void* out, int n_q_heads,
+                                  int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
   HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out, HQQ_E_INVALID, "%s: null pointer", name);
   HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
   HQQ_REQUIRE(head_dim == 128 && n_kv_heads > 0 && n_q_heads % n_kv_heads == 0 && cache_len > 0 && cache_len <= 8192, HQQ_E_UNSUPPORTED,
@@ -1649,20 +1764,23 @@ static int rope_attn_decode_batch(const char* name, bool seqpos, const void* q, 
   const int body = 2 * head_dim + cache_len > 8 * head_dim ? 2 * head_dim + cache_len : 8 * head_dim;
   const size_t smem = (size_t)(body + 32) * sizeof(float);
   const float scale = 1.0f / sqrtf((float)head_dim);
-  auto go = [&](auto kernel, auto tag) {
+  auto go = [&](auto kernel, auto tag, auto pg) {
     using T = decltype(tag);
     return launch_pdl("rope_attn_decode", kernel, dim3(n_q_heads, batch), dim3(kAttnThreads), smem, st, (const T*)q, (const T*)k, (const T*)v,
                       (const T*)cos_table, (const T*)sin_table, (T*)k_cache, (T*)v_cache, (const long long*)pos, (T*)out, n_q_heads, n_kv_heads,
-                      cache_len, head_dim, scale);
+                      cache_len, head_dim, scale, pg);
   };
+  const PageTable pt{table};
   if (dtype == HQQ_F16) {
-    if (seqpos) return go(rope_attn_decode_kernel<__half, true, true>, __half());
-    return batch > 1 ? go(rope_attn_decode_kernel<__half, true>, __half()) : go(rope_attn_decode_kernel<__half, false>, __half());
+    if (table) return go(rope_attn_decode_kernel<__half, true, true, true>, __half(), pt);
+    if (seqpos) return go(rope_attn_decode_kernel<__half, true, true>, __half(), NoPages());
+    return batch > 1 ? go(rope_attn_decode_kernel<__half, true>, __half(), NoPages()) : go(rope_attn_decode_kernel<__half, false>, __half(), NoPages());
   }
   if (dtype == HQQ_BF16) {
-    if (seqpos) return go(rope_attn_decode_kernel<__nv_bfloat16, true, true>, __nv_bfloat16());
-    return batch > 1 ? go(rope_attn_decode_kernel<__nv_bfloat16, true>, __nv_bfloat16())
-                     : go(rope_attn_decode_kernel<__nv_bfloat16, false>, __nv_bfloat16());
+    if (table) return go(rope_attn_decode_kernel<__nv_bfloat16, true, true, true>, __nv_bfloat16(), pt);
+    if (seqpos) return go(rope_attn_decode_kernel<__nv_bfloat16, true, true>, __nv_bfloat16(), NoPages());
+    return batch > 1 ? go(rope_attn_decode_kernel<__nv_bfloat16, true>, __nv_bfloat16(), NoPages())
+                     : go(rope_attn_decode_kernel<__nv_bfloat16, false>, __nv_bfloat16(), NoPages());
   }
   set_error("%s: dtype must be f16/bf16", name);
   return HQQ_E_INVALID;
@@ -1671,15 +1789,24 @@ static int rope_attn_decode_batch(const char* name, bool seqpos, const void* q, 
 extern "C" int hqq_b200_glue_rope_attn_decode_batch(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                               void* k_cache, void* v_cache, const int64_t* pos, void* out, int n_q_heads, int n_kv_heads,
                                               int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  return rope_attn_decode_batch("hqq_b200_glue_rope_attn_decode", false, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, n_q_heads,
+  return rope_attn_decode_batch("hqq_b200_glue_rope_attn_decode", false, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, pos, out, n_q_heads,
                                 n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_batch_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                      void* k_cache, void* v_cache, const int64_t* pos, void* out, int n_q_heads, int n_kv_heads,
                                                      int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  return rope_attn_decode_batch("hqq_b200_glue_rope_attn_decode_batch_seqpos", true, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out,
+  return rope_attn_decode_batch("hqq_b200_glue_rope_attn_decode_batch_seqpos", true, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, pos, out,
                                 n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_batch_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                          void* k_pool, void* v_pool, const int* table, const int64_t* pos, void* out, int n_q_heads,
+                                                          int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_attn_decode_batch_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_attn_decode_batch(name, true, q, k, v, cos_table, sin_table, k_pool, v_pool, table, pos, out, n_q_heads, n_kv_heads, cache_len, head_dim,
+                                batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
@@ -1696,19 +1823,20 @@ extern "C" size_t hqq_b200_glue_rope_attn_decode_split_workspace_bytes(int n_q_h
   return groups * s_max * (size_t)(n_q_heads / n_kv_heads) * (size_t)(head_dim + 2) * sizeof(float) + groups * sizeof(unsigned);
 }
 
-template <typename T, bool SEQPOS>
+template <typename T, bool SEQPOS, bool PAGED>
 static int launch_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache, void* v_cache,
                                const int64_t* pos, void* out, float* part, unsigned* tickets, int n_q_heads, int n_kv_heads, int cache_len,
-                               float scale_log2, dim3 grid, cudaStream_t st) {
-  if (int rc = reserve_smem<rope_attn_decode_split_kernel<T, SEQPOS>>(kSmemBytes)) return rc;
-  return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<T, SEQPOS>, grid, dim3(kSplitThreads), kSmemBytes, st, (const T*)q,
+                               float scale_log2, dim3 grid, cudaStream_t st, PageArg<PAGED> pg) {
+  if (int rc = reserve_smem<rope_attn_decode_split_kernel<T, SEQPOS, PAGED>>(kSmemBytes)) return rc;
+  return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<T, SEQPOS, PAGED>, grid, dim3(kSplitThreads), kSmemBytes, st, (const T*)q,
                     (const T*)k, (const T*)v, (const T*)cos_table, (const T*)sin_table, (T*)k_cache, (T*)v_cache, (const long long*)pos, (T*)out,
-                    part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2);
+                    part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2, pg);
 }
 
+// table == nullptr: contiguous caches; else page pools (seqpos only)
 static int rope_attn_decode_split(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
-                                  const void* sin_table, void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
-                                  int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+                                  const void* sin_table, void* k_cache, void* v_cache, const int* table, const int64_t* pos, void* out, void* workspace,
+                                  int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
   HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out && workspace, HQQ_E_INVALID, "%s: null pointer", name);
   HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
   HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0, HQQ_E_INVALID, "%s: workspace must be 4-byte aligned", name);
@@ -1723,11 +1851,18 @@ static int rope_attn_decode_split(const char* name, bool seqpos, const void* q, 
   unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
   const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
-  auto go = [&](auto f) {
-    return f(q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2, grid, st);
+  auto go = [&](auto f, auto pg) {
+    return f(q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2, grid, st, pg);
   };
-  if (dtype == HQQ_F16) return seqpos ? go(launch_decode_split<__half, true>) : go(launch_decode_split<__half, false>);
-  if (dtype == HQQ_BF16) return seqpos ? go(launch_decode_split<__nv_bfloat16, true>) : go(launch_decode_split<__nv_bfloat16, false>);
+  const PageTable pt{table};
+  if (dtype == HQQ_F16) {
+    if (table) return go(launch_decode_split<__half, true, true>, pt);
+    return seqpos ? go(launch_decode_split<__half, true, false>, NoPages()) : go(launch_decode_split<__half, false, false>, NoPages());
+  }
+  if (dtype == HQQ_BF16) {
+    if (table) return go(launch_decode_split<__nv_bfloat16, true, true>, pt);
+    return seqpos ? go(launch_decode_split<__nv_bfloat16, true, false>, NoPages()) : go(launch_decode_split<__nv_bfloat16, false, false>, NoPages());
+  }
   set_error("%s: dtype must be f16/bf16", name);
   return HQQ_E_INVALID;
 }
@@ -1735,20 +1870,31 @@ static int rope_attn_decode_split(const char* name, bool seqpos, const void* q, 
 extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                     void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
                                                     int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split", false, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, workspace,
-                                n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split", false, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, pos, out,
+                                workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_split_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                            void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
                                                            int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_seqpos", true, q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out,
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_seqpos", true, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, pos, out,
                                 workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
+extern "C" int hqq_b200_glue_rope_attn_decode_split_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                          void* k_pool, void* v_pool, const int* table, const int64_t* pos, void* out, void* workspace,
+                                                          int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
+                                                          void* stream) {
+  const char* name = "hqq_b200_glue_rope_attn_decode_split_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_attn_decode_split(name, true, q, k, v, cos_table, sin_table, k_pool, v_pool, table, pos, out, workspace, n_q_heads, n_kv_heads, cache_len,
+                                head_dim, batch, dtype, stream);
+}
+
+// table == nullptr: contiguous caches; else page pools (seqpos only)
 static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
                                       const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
-                                      const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                      const int* table, const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                       int group_size, int batch, int dtype, void* stream) {
   HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && pos && out && workspace, HQQ_E_INVALID,
               "%s: null pointer", name);
@@ -1766,17 +1912,25 @@ static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void*
   unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
   const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
-  auto go = [&](auto tag, auto sp) {
+  auto go = [&](auto tag, auto sp, auto pg) {
     using E = decltype(tag);
     constexpr bool SP = decltype(sp)::value;
-    if (int rc = reserve_smem<rope_attn_decode_split_kv8_kernel<E, SP>>(kKv8SmemBytes)) return rc;
-    return launch_pdl("rope_attn_decode_split_kv8", rope_attn_decode_split_kv8_kernel<E, SP>, grid, dim3(kSplitThreads), kKv8SmemBytes, st,
+    constexpr bool PG = std::is_same<decltype(pg), PageTable>::value;
+    if (int rc = reserve_smem<rope_attn_decode_split_kv8_kernel<E, SP, PG>>(kKv8SmemBytes)) return rc;
+    return launch_pdl("rope_attn_decode_split_kv8", rope_attn_decode_split_kv8_kernel<E, SP, PG>, grid, dim3(kSplitThreads), kKv8SmemBytes, st,
                       (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
                       (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, group_size,
-                      scale_log2);
+                      scale_log2, pg);
   };
-  if (dtype == HQQ_F16) return seqpos ? go(__half(), std::true_type()) : go(__half(), std::false_type());
-  if (dtype == HQQ_BF16) return seqpos ? go(__nv_bfloat16(), std::true_type()) : go(__nv_bfloat16(), std::false_type());
+  const PageTable pt{table};
+  if (dtype == HQQ_F16) {
+    if (table) return go(__half(), std::true_type(), pt);
+    return seqpos ? go(__half(), std::true_type(), NoPages()) : go(__half(), std::false_type(), NoPages());
+  }
+  if (dtype == HQQ_BF16) {
+    if (table) return go(__nv_bfloat16(), std::true_type(), pt);
+    return seqpos ? go(__nv_bfloat16(), std::true_type(), NoPages()) : go(__nv_bfloat16(), std::false_type(), NoPages());
+  }
   set_error("%s: dtype must be f16/bf16", name);
   return HQQ_E_INVALID;
 }
@@ -1786,7 +1940,7 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8(const void* q, const voi
                                                         const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
                                                         int head_dim, int group_size, int batch, int dtype, void* stream) {
   return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv8", false, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
-                                    v_zero, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+                                    v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
@@ -1794,7 +1948,17 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_seqpos(const void* q, co
                                                                const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
                                                                int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
   return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv8_seqpos", true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q,
-                                    v_scale, v_zero, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+                                    v_scale, v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                              void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                              const int* table, const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
+                                                              int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_attn_decode_split_kv8_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_attn_decode_split_kv8(name, true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, pos, out, workspace,
+                                    n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_q,
@@ -1811,7 +1975,8 @@ extern "C" int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, 
     using E = decltype(tag);
     return launch_pdl("rope_append_rows_kv8", rope_append_rows_kv8_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q,
                       (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q,
-                      (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0, T, n_q_heads, n_kv_heads, cache_len, group_size, NoVarlen());
+                      (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0, T, n_q_heads, n_kv_heads, cache_len, group_size, NoVarlen(),
+                      NoPages());
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
@@ -1832,7 +1997,8 @@ extern "C" int hqq_b200_glue_rope_append_rows_kv8_varlen(const void* q, const vo
     using E = decltype(tag);
     return launch_pdl("rope_append_rows_kv8_varlen", rope_append_rows_kv8_kernel<E, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
                       (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
-                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl);
+                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl,
+                      NoPages());
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
@@ -1848,7 +2014,7 @@ extern "C" int hqq_b200_glue_rope_append_rows(const void* q, const void* k, cons
     using E = decltype(tag);
     return launch_pdl("rope_append_rows", rope_append_rows_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k,
                       (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, pos0, T, n_q_heads, n_kv_heads,
-                      cache_len, NoVarlen());
+                      cache_len, NoVarlen(), NoPages());
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
@@ -1866,7 +2032,7 @@ extern "C" int hqq_b200_glue_rope_append_rows_varlen(const void* q, const void* 
     using E = decltype(tag);
     return launch_pdl("rope_append_rows_varlen", rope_append_rows_kernel<E, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
                       (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, 0, 0,
-                      n_q_heads, n_kv_heads, cache_len, vl);
+                      n_q_heads, n_kv_heads, cache_len, vl, NoPages());
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
@@ -1883,7 +2049,7 @@ extern "C" int hqq_b200_glue_attn_prefill(const void* q_rot, const void* k_cache
     using E = decltype(tag);
     if (int rc = reserve_smem<attn_prefill_kernel<E>>(kPreSmemBytes)) return rc;
     return launch_pdl("attn_prefill", attn_prefill_kernel<E>, grid, dim3(kPreThreads), kPreSmemBytes, st, (const E*)q_rot, (const E*)k_cache,
-                      (const E*)v_cache, (E*)out, pos0, T, n_q_heads, n_kv_heads, cache_len, scale_log2, NoVarlen());
+                      (const E*)v_cache, (E*)out, pos0, T, n_q_heads, n_kv_heads, cache_len, scale_log2, NoVarlen(), NoPages());
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
@@ -1903,7 +2069,96 @@ extern "C" int hqq_b200_glue_attn_prefill_varlen(const void* q_rot, const void* 
     using E = decltype(tag);
     if (int rc = reserve_smem<attn_prefill_kernel<E, true>>(kPreSmemBytes)) return rc;
     return launch_pdl("attn_prefill_varlen", attn_prefill_kernel<E, true>, grid, dim3(kPreThreads), kPreSmemBytes, st, (const E*)q_rot,
-                      (const E*)k_cache, (const E*)v_cache, (E*)out, 0, 0, n_q_heads, n_kv_heads, cache_len, scale_log2, vl);
+                      (const E*)k_cache, (const E*)v_cache, (E*)out, 0, 0, n_q_heads, n_kv_heads, cache_len, scale_log2, vl, NoPages());
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                    void* k_pool, void* v_pool, const int* table, void* q_out, const int* pos0, const int* n_tok,
+                                                    int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
+                                                    void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_paged";
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_pool && v_pool && q_out, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows_paged", rope_append_rows_kernel<E, true, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
+                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_pool, (E*)v_pool, (E*)q_out, 0, 0,
+                      n_q_heads, n_kv_heads, cache_len, vl, PageTable{table});
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
+                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
+                                                        void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_kv8_paged";
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
+              HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows_kv8_paged", rope_append_rows_kv8_kernel<E, true, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
+                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
+                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl,
+                      PageTable{table});
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_kv8_stage_paged(const void* k_q, const void* k_scale, const void* k_zero, const void* v_q, const void* v_scale,
+                                             const void* v_zero, const int* table, void* k_stage, void* v_stage, const int* pos0, const int* n_tok,
+                                             int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_kv8_stage_paged";
+  HQQ_REQUIRE(k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_kv_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  int max_p = 0;  // rows to refill: [0, pos0[b]) of the slots in the chunk
+  for (int b = 0; b < batch; ++b)
+    if (vl.n_tok[b] > 0) max_p = max(max_p, vl.pos0[b]);
+  if (max_p == 0) return HQQ_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    return launch_pdl("kv8_stage_paged", kv8_stage_paged_kernel<E>, dim3((unsigned)max_p, (unsigned)batch), dim3(256), 0, st, (const uint8_t*)k_q,
+                      (const E*)k_scale, (const E*)k_zero, (const uint8_t*)v_q, (const E*)v_scale, (const E*)v_zero, (E*)k_stage, (E*)v_stage, n_kv_heads,
+                      cache_len, group_size, vl, PageTable{table});
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_attn_prefill_paged(const void* q_rot, const void* k_pool, const void* v_pool, const int* table, void* out, const int* pos0,
+                                                const int* n_tok, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages,
+                                                int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_attn_prefill_paged";
+  HQQ_REQUIRE(q_rot && k_pool && v_pool && out, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
+  const dim3 grid((unsigned)n_kv_heads, (unsigned)batch, (unsigned)cdiv((int64_t)max_t * (n_q_heads / n_kv_heads), kPreRows));  // z <= 8192
+  auto go = [&](auto tag) {
+    using E = decltype(tag);
+    if (int rc = reserve_smem<attn_prefill_kernel<E, true, true>>(kPreSmemBytes)) return rc;
+    return launch_pdl("attn_prefill_paged", attn_prefill_kernel<E, true, true>, grid, dim3(kPreThreads), kPreSmemBytes, st, (const E*)q_rot,
+                      (const E*)k_pool, (const E*)v_pool, (E*)out, 0, 0, n_q_heads, n_kv_heads, cache_len, scale_log2, vl, PageTable{table});
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }

@@ -172,6 +172,163 @@ def sample_tokens(logits: torch.Tensor, temperature: float, top_k: int, top_p: f
     return torch.argmax(key, dim=-1)
 
 
+KV_PAGE = 64  # positions per page of a paged KV cache (csrc/decode_glue.cu kPage)
+
+
+class PageAllocator:
+    """Host bookkeeping of a paged KV cache (DecodeModel(kv_pages=N)), pure Python: no device access, so it is testable without a
+    GPU.  Pages 0 .. N-1 are real, page N is the sink.  table[b][j] names the page that holds positions 64 j .. 64 j + 63 of slot b;
+    every entry not backed by a real page points at the sink, so an entry is always a valid index.  A real page carries one reference
+    per table entry that names it, and returns to the free list when the last one goes.  pos mirrors the device positions (every
+    slot steps, a released one into the sink); active marks the slots whose steps get pages.
+
+    Invariant: the entries past a slot's current page are the sink.  So a slot only writes into pages it entered fresh or copied,
+    and a shared page is never written.  Each operation returns (writes, copies): table entries (b, j, page) to store on the device
+    and pages (src, dst) to copy in every layer, copies first.  An operation that runs out of pages raises RuntimeError and leaves
+    the state as it was."""
+
+    def __init__(self, n_pages: int, batch: int, cache_len: int):
+        if not (isinstance(n_pages, int) and n_pages >= 1):
+            raise ValueError(f"kv_pages must be an int >= 1 (got {n_pages!r})")
+        if cache_len % KV_PAGE:
+            raise ValueError(f"a paged cache needs cache_len % {KV_PAGE} == 0 (got {cache_len})")
+        self.n_pages, self.batch, self.cache_len = n_pages, batch, cache_len
+        self.sink = n_pages
+        self.entries = cache_len // KV_PAGE
+        self.reset()
+
+    def reset(self):
+        """Every page free, every entry the sink, every slot active at position 0."""
+        self.table = [[self.sink] * self.entries for _ in range(self.batch)]
+        self.ref = [0] * self.n_pages
+        self.free = list(range(self.n_pages - 1, -1, -1))  # pop() hands out the lowest free page
+        self.pos = [0] * self.batch
+        self.active = [True] * self.batch
+
+    @property
+    def free_pages(self) -> int:
+        return len(self.free)
+
+    def pages_of(self, b: int) -> int:
+        return sum(p != self.sink for p in self.table[b])
+
+    # ---- primitives: they record the device writes in w
+    def _take(self):
+        if not self.free:
+            raise RuntimeError(f"paged KV cache: out of pages (all {self.n_pages} in use)")
+        p = self.free.pop()
+        self.ref[p] = 1
+        return p
+
+    def _drop(self, p):
+        if p != self.sink:
+            self.ref[p] -= 1
+            if self.ref[p] == 0:
+                self.free.append(p)
+
+    def _set(self, w, b, j, p):
+        self.table[b][j] = p
+        w.append((b, j, p))
+
+    def _clear(self, w, b, first=0):
+        """Entries first.. of slot b back to the sink."""
+        for j in range(first, self.entries):
+            if self.table[b][j] != self.sink:
+                self._drop(self.table[b][j])
+                self._set(w, b, j, self.sink)
+
+    def _atomic(self, fn):
+        snap = ([r[:] for r in self.table], self.ref[:], self.free[:], self.pos[:], self.active[:])
+        try:
+            return fn()
+        except (RuntimeError, ValueError):
+            self.table, self.ref, self.free, self.pos, self.active = snap
+            raise
+
+    # ---- operations
+    def step(self):
+        """Pages for one decode step, then every position advances by one (mod cache_len).  An active slot about to write row p with
+        p % 64 == 0 gets a fresh page for entry p / 64; at p == 0 (the wrap) its previous lap's pages are returned first."""
+        edge = [b for b in range(self.batch) if self.active[b] and self.pos[b] % KV_PAGE == 0]
+
+        def run():
+            w = []
+            for b in edge:  # every reference is given up before any page is taken
+                if self.pos[b] == 0:
+                    self._clear(w, b)
+                else:
+                    j = self.pos[b] // KV_PAGE
+                    self._drop(self.table[b][j])
+            for b in edge:
+                self._set(w, b, self.pos[b] // KV_PAGE, self._take())
+            return w, []
+        ops = self._atomic(run) if edge else ([], [])
+        self.pos = [(p + 1) % self.cache_len for p in self.pos]
+        return ops
+
+    def prefill(self, spans):
+        """Back the rows a prefill writes.  spans: {slot: (start, T)}, rows start .. start + T - 1.  A page the prompt enters at its
+        first row gets a fresh page; the page it enters mid-page must be backed already and is copied first if shared.  Entries past
+        the prompt's last page go back to the sink.  ValueError if positions [0, start) hold no pages."""
+        for b, (start, _) in spans.items():
+            if any(self.table[b][j] == self.sink for j in range(-(-start // KV_PAGE))):
+                raise ValueError(f"slot {b}: positions [0, {start}) are not all backed by pages (released, or never written)")
+
+        def run():
+            w, copies, fresh = [], [], []
+            for b, (start, T) in spans.items():
+                first, last = start // KV_PAGE, (start + T - 1) // KV_PAGE
+                self._clear(w, b, last + 1)
+                for j in range(first, last + 1):
+                    p = self.table[b][j]
+                    if j * KV_PAGE >= start:
+                        self._drop(p)
+                        fresh.append((b, j))
+                    elif self.ref[p] > 1:  # copy-on-write of the shared page the prompt continues
+                        q = self._take()
+                        copies.append((p, q))
+                        self._drop(p)
+                        self._set(w, b, j, q)
+            for b, j in fresh:
+                self._set(w, b, j, self._take())
+            for b, (start, T) in spans.items():
+                self.pos[b] = (start + T) % self.cache_len
+                self.active[b] = True
+            return w, copies
+        return self._atomic(run)
+
+    def release(self, b: int):
+        """Slot b's pages back to the free list, its entries to the sink; it keeps stepping, into the sink, until a prefill or a
+        fork targets it again."""
+        w = []
+        self._clear(w, b)
+        self.active[b] = False
+        return w, []
+
+    def fork(self, src: int, dst: int):
+        """dst continues src: dst is released, then shares src's full pages below pos[src] and gets a copy of the partial one."""
+        if src == dst:
+            raise ValueError("fork needs two different slots")
+        if not self.active[src]:
+            raise ValueError(f"slot {src} is released: nothing to fork")
+
+        def run():
+            w, copies = self.release(dst)
+            p = self.pos[src]
+            for j in range(p // KV_PAGE):
+                pg = self.table[src][j]
+                self.ref[pg] += 1
+                self._set(w, dst, j, pg)
+            if p % KV_PAGE:
+                q = self._take()
+                copies.append((self.table[src][p // KV_PAGE], q))
+                self._set(w, dst, p // KV_PAGE, q)
+            self.pos[dst] = p
+            self.active[dst] = True
+            return w, copies
+        return self._atomic(run)
+
+
 def shard_dims(shape: LlamaShape, tp: int):
     """Per-rank sizes of the sharded projections (pure host logic, unit-tested on CPU)."""
     if shape.n_heads % tp or shape.n_kv_heads % tp or shape.inter % tp:
@@ -188,7 +345,7 @@ class DecodeModel:
                  device="cuda", cache_len: int = 256, tp: int = 1, rank: int = 0, seed: int = 0, process_group=None,
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
                  kv_bits: int = 16, kv_group_size: int = 64, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
-                 top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False):
+                 top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
         # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
         # top-k, top-p, then a Gumbel race on Philox numbers keyed by sample_seed and countered by _sample_ctr -- instead of the argmax.
@@ -223,6 +380,14 @@ class DecodeModel:
         self.ragged = bool(ragged)
         if self.ragged and self.batch > 256:
             raise ValueError("ragged batches hold at most 256 sequences")
+        # kv_pages N (ragged only): every layer's cache is a pool of N + 1 pages [N + 1, n_kv, 64, 128] (page N the sink) and the
+        # slots reach their rows through one shared device page_table [batch, cache_len / 64]; PageAllocator hands out the pages.
+        # The kernels are the ragged ones' PAGED twins: a paged model computes the unpaged ragged model's bits.
+        self.kv_pages = kv_pages
+        if kv_pages is not None:
+            if not self.ragged:
+                raise ValueError("kv_pages needs ragged=True")
+            self.pages = PageAllocator(kv_pages, self.batch, cache_len)
         if (self.batch > 1 or self.ragged) and fused:
             fused = True  # the 8-launch path with the batched glue kernels; the one-token kernels (fused=5) and their exchange are M = 1 only
         self.fused = fused
@@ -281,11 +446,12 @@ class DecodeModel:
             blk["norm2"] = torch.ones(shape.hidden, device=self.device, dtype=dtype)
             hkv = shape.n_kv_heads // tp
             cdt = torch.uint8 if self.kv_bits == 8 else dtype
-            blk["k_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=cdt)
-            blk["v_cache"] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim, device=self.device, dtype=cdt)
+            rows = (self.batch, hkv, cache_len) if kv_pages is None else (kv_pages + 1, hkv, KV_PAGE)
+            blk["k_cache"] = torch.zeros(*rows, shape.head_dim, device=self.device, dtype=cdt)
+            blk["v_cache"] = torch.zeros(*rows, shape.head_dim, device=self.device, dtype=cdt)
             if self.kv_bits == 8:
                 for name in ("k_scale", "k_zero", "v_scale", "v_zero"):
-                    blk[name] = torch.zeros(self.batch, hkv, cache_len, shape.head_dim // kv_group_size, device=self.device, dtype=dtype)
+                    blk[name] = torch.zeros(*rows, shape.head_dim // kv_group_size, device=self.device, dtype=dtype)
             self.blocks.append(blk)
         self._kv8_stage = None  # kv_bits 8: dequantised fp16 / bf16 K and V for the prefill attention, allocated by the first fused prefill
         self.cos, self.sin = rope_tables(shape, cache_len, dtype, self.device)  # [cache_len, hd]
@@ -296,6 +462,8 @@ class DecodeModel:
         self._slot_idx = torch.arange(self.batch, device=self.device)
         self.next_tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
         self._sample_ctr = torch.zeros(1, dtype=torch.long, device=self.device)  # Philox counter: + 1 per sampled token
+        if kv_pages is not None:
+            self.page_table = torch.full((self.batch, cache_len // KV_PAGE), kv_pages, dtype=torch.int32, device=self.device)
         self.graph = None
         self.last_logits = None  # set by prefill(): logits of the last prompt position of each sequence
 
@@ -307,14 +475,77 @@ class DecodeModel:
             return "split_kv8"
         return "split" if self.cache_len > SINGLE_ATTN_MAX_LEN else "single"
 
+    _CACHE_NAMES = ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero")
+
+    @property
+    def free_pages(self) -> int:
+        """kv_pages: the pages no slot holds."""
+        return self.pages.free_pages
+
+    def cache_view(self, blk) -> dict:
+        """A layer's caches in the contiguous layout [batch, n_kv, cache_len, ...]: the tensors themselves, or with kv_pages a copy
+        gathered through the page table (rows no page backs read the sink)."""
+        names = [n for n in self._CACHE_NAMES if n in blk]
+        if self.kv_pages is None:
+            return {n: blk[n] for n in names}
+        idx = self.page_table.long()
+        B, E = idx.shape
+        return {n: blk[n][idx].permute(0, 2, 1, 3, 4).reshape(B, blk[n].shape[1], E * KV_PAGE, blk[n].shape[3]) for n in names}
+
+    def _apply_pages(self, ops):
+        """A PageAllocator operation's result on the device, in stream order and without a sync: page copies in every layer, then
+        the table entries (scalar fills)."""
+        writes, copies = ops
+        for src, dst in copies:
+            for blk in self.blocks:
+                for n in self._CACHE_NAMES:
+                    if n in blk:
+                        blk[n][dst].copy_(blk[n][src])
+        for b, j, p in writes:
+            self.page_table[b, j] = p
+
+    def release(self, b: int):
+        """kv_pages: slot b's pages go back to the pool and its table row to the sink.  The slot keeps stepping (all slots do), into
+        the sink; its tokens mean nothing until a prefill or a fork targets it again.  The other slots are unaffected."""
+        self._paged_only("release")
+        self._apply_pages(self.pages.release(int(b)))
+
+    def fork(self, src: int, dst: int):
+        """kv_pages: slot dst continues slot src -- dst is released, then shares src's full pages below pos[src] (stored once) and
+        gets a copy of the partial page in every layer; pos and tok are copied.  Neither slot ever writes a shared page."""
+        self._paged_only("fork")
+        src, dst = int(src), int(dst)
+        if not (0 <= src < self.batch and 0 <= dst < self.batch):
+            raise ValueError(f"fork: slots must lie in [0, {self.batch})")
+        self._apply_pages(self.pages.fork(src, dst))
+        self.pos[dst].copy_(self.pos[src])
+        self.tok[dst].copy_(self.tok[src])
+
+    def _paged_only(self, what):
+        if self.kv_pages is None:
+            raise ValueError(f"{what} needs a paged KV cache (kv_pages)")
+
     def kv_cache_bytes(self) -> int:
-        """Bytes of every layer's KV cache on this rank: fp16 / bf16 rows, or levels plus scale and zero with kv_bits 8."""
+        """Bytes of every layer's KV cache on this rank: fp16 / bf16 rows, or levels plus scale and zero with kv_bits 8 (with
+        kv_pages: the page pools, sink included)."""
         names = ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero")
         return sum(blk[n].numel() * blk[n].element_size() for blk in self.blocks for n in names if n in blk)
 
     def _attn_split(self, lib, blk, hq, hkv, code, st):
         from ._lib import check, ptr
         b = self._bufs
+        paged = self.kv_pages is not None
+        if paged and self.kv_bits == 8:
+            check(lib.hqq_b200_glue_rope_attn_decode_split_kv8_paged(
+                ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]),
+                ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(self.page_table), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq,
+                hkv, self.cache_len, self.shape.head_dim, self.kv_group_size, self.batch, self.kv_pages, code, st))
+            return
+        if paged:
+            check(lib.hqq_b200_glue_rope_attn_decode_split_paged(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                                 ptr(blk["v_cache"]), ptr(self.page_table), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq,
+                                                                 hkv, self.cache_len, self.shape.head_dim, self.batch, self.kv_pages, code, st))
+            return
         if self.kv_bits == 8:
             fn = lib.hqq_b200_glue_rope_attn_decode_split_kv8_seqpos if self.ragged else lib.hqq_b200_glue_rope_attn_decode_split_kv8
             check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
@@ -368,15 +599,20 @@ class DecodeModel:
             q, k, v = q.view(B, hq, hd), k.view(B, hkv, hd), v.view(B, hkv, hd)
             q = self._rope(q, cos, sin)
             k = self._rope(k, cos, sin)
-            if self.ragged:  # row pos[b] of sequence b
+            if self.ragged:  # row pos[b] of sequence b (kv_pages: through the page table)
+                if self.kv_pages is None:
+                    at = (self._slot_idx, slice(None), self.pos)
+                else:
+                    at = (self.page_table[self._slot_idx, self.pos // KV_PAGE].long(), slice(None), self.pos % KV_PAGE)
                 for name, x in (("k", k), ("v", v.view(B, hkv, hd))):
                     if self.kv_bits == 8:
                         lv, sc, ze = kv8_quantize_rows(x, self.kv_group_size)
                         for suffix, val in (("_cache", lv), ("_scale", sc), ("_zero", ze)):
-                            blk[name + suffix][self._slot_idx, :, self.pos] = val
+                            blk[name + suffix][at] = val
                     else:
-                        blk[name + "_cache"][self._slot_idx, :, self.pos] = x
-                kc, vc = self._kv8_read(blk, self.cache_len) if self.kv_bits == 8 else (blk["k_cache"], blk["v_cache"])
+                        blk[name + "_cache"][at] = x
+                cv = self.cache_view(blk)
+                kc, vc = self._kv8_read(cv, self.cache_len) if self.kv_bits == 8 else (cv["k_cache"], cv["v_cache"])
             elif self.kv_bits == 8:  # the rotated rows quantised into the cache; attention over the dequantised cache
                 self._kv8_write(blk, k.view(B, hkv, 1, hd), v.view(B, hkv, 1, hd), self.pos)
                 kc, vc = self._kv8_read(blk, self.cache_len)
@@ -535,6 +771,10 @@ class DecodeModel:
             self._lin(b["x"], (blk["q"], blk["k"], blk["v"]), [b["q"], b["k"], b["v"]])
             if self.attn_kernel != "single":
                 self._attn_split(lib, blk, hq, hkv, code, st)
+            elif self.kv_pages is not None:
+                check(lib.hqq_b200_glue_rope_attn_decode_batch_paged(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin),
+                                                                     ptr(blk["k_cache"]), ptr(blk["v_cache"]), ptr(self.page_table), ptr(self.pos),
+                                                                     ptr(b["a"]), hq, hkv, self.cache_len, hd, B, self.kv_pages, code, st))
             else:
                 fn = lib.hqq_b200_glue_rope_attn_decode_batch_seqpos if self.ragged else lib.hqq_b200_glue_rope_attn_decode_batch
                 check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
@@ -739,6 +979,8 @@ class DecodeModel:
         chunk = min(int(chunk), 65535)
         if chunk < 1:
             raise ValueError("chunk must be >= 1")
+        if self.kv_pages is not None:  # back every row the prompts write (fresh pages, copy-on-write of a shared partial page)
+            self._apply_pages(self.pages.prefill({b: (starts[b], int(toks[b].numel())) for b in slots}))
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         last = {}
         with torch.no_grad():
@@ -794,6 +1036,9 @@ class DecodeModel:
         norm = lambda d, w: check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(d), ptr(w), ptr(x), M, s.hidden, s.rms_eps, code, st))
         delta = None
         kv8 = self.kv_bits == 8
+        paged = self.kv_pages is not None
+        if paged:
+            pt, npg = ptr(self.page_table), self.kv_pages
         if kv8 and self._kv8_stage is None:  # one staging pair for all layers: [batch, n_kv, cache_len, 128] each
             self._kv8_stage = tuple(torch.zeros(B, hkv, self.cache_len, hd, device=self.device, dtype=self.dtype) for _ in range(2))
         for blk in self.blocks:
@@ -803,14 +1048,22 @@ class DecodeModel:
                 # staging rows [0, p0) dequantised from the 8-bit cache, rows [p0, p0 + n) written by the rows kernel; the attention
                 # kernel is the one of the fp16 cache, reading the staging pair
                 kst, vst = self._kv8_stage
-                for bi in range(B):
+                for bi in range(0 if paged else B):
                     sp0 = p0 if varlen is None else (varlen[0][bi] if varlen[1][bi] else 0)  # slots outside the chunk: nothing
                     for hh in range(hkv):
                         for c, dst in (("k", kst), ("v", vst)):
                             if sp0 > 0:
                                 check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][bi, hh]), ptr(blk[c + "_scale"][bi, hh]), ptr(blk[c + "_zero"][bi, hh]),
                                                               ptr(dst[bi, hh]), sp0, hd, self.kv_group_size, 8, 1, code, st))
-                if varlen is not None:
+                if paged:  # one launch refills the staging rows [0, pos0) of the slots in the chunk, through the table
+                    check(lib.hqq_b200_glue_kv8_stage_paged(ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]),
+                                                            ptr(blk["v_scale"]), ptr(blk["v_zero"]), pt, ptr(kst), ptr(vst), vp0, vnt, hkv, self.cache_len, hd,
+                                                            self.kv_group_size, B, npg, code, st))
+                    check(lib.hqq_b200_glue_rope_append_rows_kv8_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                                       ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
+                                                                       ptr(blk["v_zero"]), pt, ptr(kst), ptr(vst), ptr(qr), vp0, vnt, hq, hkv, self.cache_len,
+                                                                       hd, self.kv_group_size, B, npg, code, st))
+                elif varlen is not None:
                     check(lib.hqq_b200_glue_rope_append_rows_kv8_varlen(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
                                                                         ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
                                                                         ptr(blk["v_zero"]), ptr(kst), ptr(vst), ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd,
@@ -820,6 +1073,10 @@ class DecodeModel:
                                                                  ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(kst),
                                                                  ptr(vst), ptr(qr), p0, n, hq, hkv, self.cache_len, hd, self.kv_group_size, B, code, st))
                 kc, vc = kst, vst
+            elif paged:
+                check(lib.hqq_b200_glue_rope_append_rows_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
+                                                               pt, ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd, B, npg, code, st))
+                kc, vc = blk["k_cache"], blk["v_cache"]
             elif varlen is not None:
                 check(lib.hqq_b200_glue_rope_append_rows_varlen(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
                                                                 ptr(blk["v_cache"]), ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd, B, code, st))
@@ -828,7 +1085,9 @@ class DecodeModel:
                 check(lib.hqq_b200_glue_rope_append_rows(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
                                                          ptr(qr), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
                 kc, vc = blk["k_cache"], blk["v_cache"]
-            if varlen is not None:
+            if paged and not kv8:
+                check(lib.hqq_b200_glue_attn_prefill_paged(ptr(qr), ptr(kc), ptr(vc), pt, ptr(a), vp0, vnt, hq, hkv, self.cache_len, hd, B, npg, code, st))
+            elif varlen is not None:
                 check(lib.hqq_b200_glue_attn_prefill_varlen(ptr(qr), ptr(kc), ptr(vc), ptr(a), vp0, vnt, hq, hkv, self.cache_len, hd, B, code, st))
             else:
                 check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(kc), ptr(vc), ptr(a), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
@@ -845,7 +1104,8 @@ class DecodeModel:
         return h, delta
 
     def _prefill_chunk_ref(self, ids, p0, hd, hq, hkv, slot=None):
-        """The same chunk on framework ops (fused=False); slot: ids [1, n] of that slot only, on that slot's caches."""
+        """The same chunk on framework ops (fused=False); slot: ids [1, n] of that slot only, on that slot's caches (kv_pages: gathered
+        through the table, and the chunk's rows stored back through it)."""
         s = self.shape
         B, n = ids.shape
         M = B * n
@@ -855,7 +1115,12 @@ class DecodeModel:
         mask = torch.arange(end, device=self.device).view(1, end) <= torch.arange(p0, end, device=self.device).view(n, 1)  # [n, end]
         delta = None
         for blk in self.blocks:
-            cb = blk if slot is None else {n: t[slot:slot + 1] for n, t in blk.items() if n.startswith(("k_", "v_"))}
+            if slot is None:
+                cb = blk
+            elif self.kv_pages is None:
+                cb = {n: t[slot:slot + 1] for n, t in blk.items() if n.startswith(("k_", "v_"))}
+            else:
+                cb = {n: t[slot:slot + 1].clone() for n, t in self.cache_view(blk).items()}
             if delta is not None:
                 h = h + delta
             x = F.rms_norm(h, (s.hidden,), blk["norm1"], s.rms_eps)
@@ -869,6 +1134,11 @@ class DecodeModel:
                 cb["k_cache"][:, :, p0:end] = k.transpose(1, 2)
                 cb["v_cache"][:, :, p0:end] = v.view(B, n, hkv, hd).transpose(1, 2)
                 kc, vc = cb["k_cache"][:, :, :end], cb["v_cache"][:, :, :end]
+            if slot is not None and self.kv_pages is not None:  # the chunk's rows into their pages
+                rows = torch.arange(p0, end, device=self.device)
+                at = (self.page_table[slot, rows // KV_PAGE].long(), slice(None), rows % KV_PAGE)
+                for name, t in cb.items():
+                    blk[name][at] = t[0, :, p0:end].transpose(0, 1)
             a = F.scaled_dot_product_attention(q.transpose(1, 2), kc, vc, attn_mask=mask, enable_gqa=True)
             o = blk["o"](a.transpose(1, 2).reshape(M, hq * hd))
             if self.tp > 1:
@@ -966,6 +1236,8 @@ class DecodeModel:
         torch.cuda.current_stream(self.device).wait_stream(st)
         torch.cuda.synchronize(self.device)
         self.pos.zero_()
+        if self.kv_pages is not None:
+            self.pages.pos = [0] * self.batch
         self.graph = torch.cuda.CUDAGraph()
         with torch.no_grad(), torch.cuda.graph(self.graph):
             step()
@@ -976,6 +1248,9 @@ class DecodeModel:
         self.tok.fill_(token)
         self.pos.zero_()
         self._sample_ctr.zero_()
+        if self.kv_pages is not None:  # every page free, every entry the sink, every slot active at position 0
+            self.pages.reset()
+            self.page_table.fill_(self.kv_pages)
         for blk in self.blocks:
             for name in ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero"):
                 if name in blk:
@@ -985,7 +1260,11 @@ class DecodeModel:
                 t.zero_()
 
     def decode(self, feed_back: bool = True):
-        """Replay one step; with feed_back the produced token becomes the next input (device-side copy)."""
+        """Replay one step; with feed_back the produced token becomes the next input (device-side copy).  With kv_pages, callers
+        must step through decode(), not a bare graph.replay(): before the replay a slot about to enter a page gets it here (stream-
+        ordered table writes, no sync).  A bare replay cannot address outside the pools, but its writes at a page edge go to the sink."""
+        if self.kv_pages is not None:
+            self._apply_pages(self.pages.step())
         self.graph.replay()
         if feed_back:
             self.tok.copy_(self.next_tok)

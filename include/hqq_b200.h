@@ -345,6 +345,51 @@ int hqq_b200_glue_rope_append_rows_kv8_varlen(const void* q, const void* k, cons
 int hqq_b200_glue_attn_prefill_varlen(const void* q_rot, const void* k_cache, const void* v_cache, void* out,
                                       const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads, int cache_len,
                                       int head_dim, int batch, int dtype, void* stream);
+/* Paged KV cache: the _seqpos decode and _varlen prefill entry points over page pools.  A page holds 64 positions of one sequence
+ * for every kv head: the pools are [n_pages + 1, n_kv_heads, 64, head_dim] (fp16 / bf16 rows, or uint8 levels) and, for the 8-bit
+ * cache, [n_pages + 1, n_kv_heads, 64, head_dim / group_size] meta.  table is a device int32 [batch, cache_len / 64]: position p of
+ * sequence b, kv head h lives at pool row (table[b][p / 64] * n_kv_heads + h) * 64 + p % 64.  Every entry must lie in
+ * [0, n_pages]; page n_pages is conventionally the sink the unbacked entries point at.  Nothing else differs from the contiguous
+ * entry points: a sequence's output, tickets and written rows are bit for bit theirs on the cache gathered through the table.
+ * Needs cache_len % 64 == 0 and n_pages >= 1.  The table entries, like pos, are read BEFORE the programmatic-dependency wait: they
+ * must have been written by an earlier, completed launch, not by the kernel directly in front of this one.  The 8-bit prefill keeps
+ * its staging pair [batch, n_kv_heads, cache_len, head_dim]; hqq_b200_glue_kv8_stage_paged refills staging rows [0, pos0[b]) of
+ * every slot with n_tok[b] > 0 from the pools, bit for bit the rows hqq_b200_dequantize gives. */
+int hqq_b200_glue_rope_attn_decode_batch_paged(const void* q, const void* k, const void* v,
+                                               const void* cos_table, const void* sin_table,
+                                               void* k_pool, void* v_pool, const int* table, const int64_t* pos, void* out,
+                                               int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                               int batch, int n_pages, int dtype, void* stream);
+int hqq_b200_glue_rope_attn_decode_split_paged(const void* q, const void* k, const void* v,
+                                               const void* cos_table, const void* sin_table,
+                                               void* k_pool, void* v_pool, const int* table, const int64_t* pos, void* out, void* workspace,
+                                               int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                               int batch, int n_pages, int dtype, void* stream);
+int hqq_b200_glue_rope_attn_decode_split_kv8_paged(const void* q, const void* k, const void* v,
+                                                   const void* cos_table, const void* sin_table,
+                                                   void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                   const int* table, const int64_t* pos, void* out, void* workspace,
+                                                   int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                                   int batch, int n_pages, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_paged(const void* q, const void* k, const void* v,
+                                         const void* cos_table, const void* sin_table,
+                                         void* k_pool, void* v_pool, const int* table, void* q_out, const int* pos0, const int* n_tok,
+                                         int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                         int batch, int n_pages, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_kv8_paged(const void* q, const void* k, const void* v,
+                                             const void* cos_table, const void* sin_table,
+                                             void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                             const int* table, void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok,
+                                             int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                             int batch, int n_pages, int dtype, void* stream);
+int hqq_b200_glue_kv8_stage_paged(const void* k_q, const void* k_scale, const void* k_zero,
+                                  const void* v_q, const void* v_scale, const void* v_zero, const int* table,
+                                  void* k_stage, void* v_stage, const int* pos0, const int* n_tok,
+                                  int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                  int batch, int n_pages, int dtype, void* stream);
+int hqq_b200_glue_attn_prefill_paged(const void* q_rot, const void* k_pool, const void* v_pool, const int* table, void* out,
+                                     const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads, int cache_len,
+                                     int head_dim, int batch, int n_pages, int dtype, void* stream);
 /* out[0] = argmax(logits[0..n)) (first index on ties) */
 int hqq_b200_glue_argmax(const void* logits, int n, int64_t* out, int dtype, void* stream);
 /* Vocabulary-sharded lm_head (tensor parallel decode): out_key[0] = a signed 64-bit key {ordered(max) : 0xFFFFFFFF - (index_offset +
