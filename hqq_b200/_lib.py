@@ -78,6 +78,17 @@ SIGNATURES = {
     "hqq_b200_glue_rope_append_rows_kv8_paged": (c_int, [c_void_p] * 17 + [c_int] * 8 + [c_void_p]),
     "hqq_b200_glue_kv8_stage_paged": (c_int, [c_void_p] * 11 + [c_int] * 7 + [c_void_p]),
     "hqq_b200_glue_attn_prefill_paged": (c_int, [c_void_p] * 7 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_devpos": (c_int, [c_void_p] * 9 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_devpos_paged": (c_int, [c_void_p] * 10 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_attn_verify_split_workspace_bytes": (c_size_t, [c_int] * 5),
+    "hqq_b200_glue_rope_append_rows_kv8_devpos": (c_int, [c_void_p] * 13 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv8_devpos_paged": (c_int, [c_void_p] * 14 + [c_int] * 9 + [c_void_p]),
+    "hqq_b200_glue_attn_verify_split_kv8": (c_int, [c_void_p] * 10 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_attn_verify_split_kv8_paged": (c_int, [c_void_p] * 11 + [c_int] * 9 + [c_void_p]),
+    "hqq_b200_glue_attn_verify_split": (c_int, [c_void_p] * 6 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_attn_verify_split_paged": (c_int, [c_void_p] * 7 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_ngram_draft": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
+    "hqq_b200_glue_spec_accept": (c_int, [c_void_p] * 8 + [c_int] * 3 + [c_void_p]),
     "hqq_b200_glue_argmax": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_key": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_tp": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),

@@ -968,6 +968,343 @@ int split_count(int n_kv, int cache_len) {
   return max(1, min(by_sm, by_len));
 }
 
+// Speculative verify attention (DESIGN.md 3.5): slot b feeds T = K + 1 rows at positions pos[b] .. pos[b] + T - 1, of which the
+// n[b] = min(T, L - pos[b]) that fit in the cache are valid; row t attends over cache rows 0 .. pos[b] + t.  The schedule is
+// rope_attn_decode_split_kernel's -- grid (S, ., batch) with S fixed at launch, 16-position tiles through per-warp 3-stage cp.async
+// rings, K.Q^T and V^T.P^T on mma.sync m16n8k16, online softmax in fp32, a ticketed merge in split order -- with three changes:
+//   - the MMA n dimension is the (t, h) columns of one GQA group, column c = t G + h (T G <= 64), in n-tiles of 8.  A CTA holds
+//     kVerTiles n-tiles; the column groups of a kv head are spread over grid.y = n_kv * n_cg, each re-reading the same chunk;
+//   - every attended row comes from the cache (the DEVPOS append writes rows pos .. pos + n - 1 just before this launch).  Rows < pos
+//     may be staged before griddepcontrol.wait; rows pos .. are loaded after it.  Each chunk covers [0, pos + n);
+//   - column (t, h) masks key positions > pos + t.  A tile can lie wholly past a column's last key, so the running max is guarded
+//     (a column with no key yet keeps m = -inf, l = 0, o = 0).
+// q / out [batch T, n_q 128] (row b T + t, q rotated), caches [batch, n_kv, L, 128] or (PAGED) pools [pages, n_kv, 64, 128].
+// part [batch, n_kv, n_cg, S, 8 kVerTiles, 2 + 128] floats, tickets [batch, n_kv, n_cg] uint32, zero between launches.
+// KV8: the caches hold HQQ 8-bit levels (uint8, same layout) with meta [.., 128 / gs] T; each staged 16-byte chunk is the
+// dequantisation T(T(q - z) * s) of 8 levels (kv8_deq2, what hqq_b200_dequantize gives), loaded and stored synchronously instead of
+// through cp.async; the tile layout, the MMAs and everything after them are those of the 16-bit cache.
+constexpr int kVerTiles = 2;                     // n-tiles per CTA (no spills at 2: DESIGN.md 3.5)
+constexpr int kVerCols = 8 * kVerTiles;          // columns per CTA
+constexpr int kVerMaxCols = 64;                  // T G
+constexpr int kVerMaxT = 8;                      // K + 1
+static_assert(kSplitWarps * kVerCols * kPartFloats * 4 <= kRingBytes, "the warp partials reuse the ring");
+template <typename T> struct Kv8Meta { const T* k_s; const T* k_z; const T* v_s; const T* v_z; int gs; };
+struct NoKv8 {};
+template <typename T, bool KV8> using Kv8Arg = typename std::conditional<KV8, Kv8Meta<T>, NoKv8>::type;
+template <typename T, bool KV8> using CacheT = typename std::conditional<KV8, uint8_t, T>::type;
+
+template <typename T, bool PAGED = false, bool KV8 = false>
+__global__ void __launch_bounds__(kSplitThreads, 1)
+    attn_verify_split_kernel(const T* __restrict__ q, const CacheT<T, KV8>* __restrict__ k_cache, const CacheT<T, KV8>* __restrict__ v_cache,
+                             const long long* __restrict__ pos_p, T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q,
+                             int n_kv, int L, int TQ, float scale_log2, const PageArg<PAGED> pg, Kv8Arg<T, KV8> m8) {
+  extern __shared__ __align__(16) char smem[];
+  constexpr int NW = kSplitWarps, ST = kSplitStages, NT = kVerTiles, NC = kVerCols;
+  const int G = n_q / n_kv, C = TQ * G, n_cg = (C + NC - 1) / NC;
+  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y / n_cg, cg = (int)blockIdx.y % n_cg, b = (int)blockIdx.z;
+  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  const int* tab = nullptr;
+  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
+  {
+    const long long kv = (long long)b * n_kv + kvh;
+    if constexpr (!PAGED) {
+      k_cache += kv * L * kHd; v_cache += kv * L * kHd;
+      if constexpr (KV8) {
+        const int ng = kHd / m8.gs;
+        m8.k_s += kv * L * ng; m8.k_z += kv * L * ng; m8.v_s += kv * L * ng; m8.v_z += kv * L * ng;
+      }
+    }
+    part += (kv * n_cg + cg) * S * NC * kPartFloats;
+    tickets += kv * n_cg + cg;
+  }
+  char* ring = smem + warp * ST * kStageBytes;
+  int* last = reinterpret_cast<int*>(smem + kRingBytes);
+
+  // *pos was written by a completed launch (the previous step's accept kernel): it may be read before the wait
+  const int pos = (int)pos_p[b], end = pos + min(TQ, L - pos);
+  const int chunk = (((end + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
+  const int c0 = min(split * chunk, end), c1 = min(c0 + chunk, end);
+  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
+  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;
+  pdl_launch_dependents();
+
+  // 16-byte chunk c of cache row `row` (K or V) into dst: cp.async, or (KV8) 8 levels dequantised with their group's meta
+  auto stage16 = [&](char* dst, int isv, long long row, int c, bool async) {
+    if constexpr (KV8) {
+      const uint2 w = *reinterpret_cast<const uint2*>((isv ? v_cache : k_cache) + row * kHd + c * 8);
+      const long long mi = row * (kHd / m8.gs) + (c * 8) / m8.gs;
+      typename Pair<T>::type s2, z2;
+      s2.x = s2.y = (isv ? m8.v_s : m8.k_s)[mi];
+      z2.x = z2.y = (isv ? m8.v_z : m8.k_z)[mi];
+      uint4 o;
+      o.x = kv8_deq2<T, 0>(w.x, z2, s2); o.y = kv8_deq2<T, 1>(w.x, z2, s2);
+      o.z = kv8_deq2<T, 0>(w.y, z2, s2); o.w = kv8_deq2<T, 1>(w.y, z2, s2);
+      *reinterpret_cast<uint4*>(dst) = o;
+    } else if (async) {
+      split_cp16(dst, (isv ? v_cache : k_cache) + row * kHd + c * 8);
+    } else {
+      *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>((isv ? v_cache : k_cache) + row * kHd + c * 8);
+    }
+  };
+  // Stage local tile i into its ring slot: rows below lim from the cache (cp.async), rows past the chunk zero (finite, P = 0).
+  // Before the wait lim = pos; rows pos .. c1 - 1 of those tiles are filled in after it.
+  auto issue = [&](int i, int lim) {
+    if (i < my_tiles) {
+      const int t0 = c0 + (warp + i * NW) * kSplitTile;
+      char* st = ring + (i % ST) * kStageBytes;
+      long long rt = 0;
+      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
+#pragma unroll 4
+      for (int j = lane; j < 2 * kSplitTile * 16; j += 32) {
+        const int isv = j >> 8, r = (j >> 4) & 15, c = j & 15, p = t0 + r;
+        char* dst = st + isv * kTileBytes + swz(r, c);
+        if (p < c1) {
+          if (p < lim) stage16(dst, isv, rt + p, c, true);
+        } else {
+          uint4 z;
+          z.x = z.y = z.z = z.w = 0u;
+          *reinterpret_cast<uint4*>(dst) = z;
+        }
+      }
+    }
+    split_commit();
+  };
+#pragma unroll
+  for (int i = 0; i < ST - 1; ++i) issue(i, pos);
+  pdl_wait();
+  for (int i = 0; i < ST - 1 && i < my_tiles; ++i) {  // rows pos .. of the tiles staged before the wait, written by the append
+    const int t0 = c0 + (warp + i * NW) * kSplitTile;
+    if (t0 + kSplitTile <= pos) continue;
+    char* st = ring + (i % ST) * kStageBytes;
+    long long rt = 0;
+    if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
+    for (int j = lane; j < 2 * kSplitTile * 16; j += 32) {
+      const int isv = j >> 8, r = (j >> 4) & 15, c = j & 15, p = t0 + r;
+      if (p >= pos && p < c1) stage16(st + isv * kTileBytes + swz(r, c), isv, rt + p, c, false);
+    }
+  }
+  // Q^T fragments of n-tile j: column cg NC + 8 j + g = (t, h); columns past T G are zero.  Lane (g, qd) owns the scores of columns
+  // 8 j + 2 qd + {0, 1}; lim[j][u] is the first key position such a column does not see.
+  uint32_t qb[NT][8][2];
+  int lim[NT][2];
+#pragma unroll
+  for (int j = 0; j < NT; ++j) {
+    const int col = cg * NC + 8 * j + g;
+    const bool ok = col < C;
+    const T* qr = q + (((long long)b * TQ + (ok ? col / G : 0)) * n_q + (long long)kvh * G + (ok ? col % G : 0)) * kHd + 2 * qd;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      qb[j][kk][0] = ok ? *reinterpret_cast<const uint32_t*>(qr + kk * 16) : 0u;
+      qb[j][kk][1] = ok ? *reinterpret_cast<const uint32_t*>(qr + kk * 16 + 8) : 0u;
+    }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int cu = cg * NC + 8 * j + 2 * qd + u;
+      lim[j][u] = cu < C ? min(pos + cu / G + 1, c1) : c1;
+    }
+  }
+
+  float o[NT][8][4];
+  float m[NT][2], l[NT][2];
+#pragma unroll
+  for (int j = 0; j < NT; ++j) {
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) o[j][mt][0] = o[j][mt][1] = o[j][mt][2] = o[j][mt][3] = 0.f;
+    m[j][0] = m[j][1] = -INFINITY;
+    l[j][0] = l[j][1] = 0.f;
+  }
+  const int kr = (lane & 7) + ((lane >> 3) & 1) * 8, kc = lane >> 4;
+  const int vr = (lane & 7) + ((lane >> 4) & 1) * 8, vc = (lane >> 3) & 1;
+  for (int i = 0; i < my_tiles; ++i) {
+    __syncwarp();
+    issue(i + ST - 1, c1);
+    split_wait<ST - 1>();
+    __syncwarp();
+    const char* kt = ring + (i % ST) * kStageBytes;
+    const char* vt = kt + kTileBytes;
+    float s[NT][4];
+#pragma unroll
+    for (int j = 0; j < NT; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t a[4];
+      ldsm4<false>(a, kt + swz(kr, 2 * kk + kc));
+#pragma unroll
+      for (int j = 0; j < NT; ++j) mma16816<T>(s[j], a, qb[j][kk][0], qb[j][kk][1]);
+    }
+    const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
+    uint32_t pb[NT][2];
+#pragma unroll
+    for (int j = 0; j < NT; ++j) {
+      const float x0 = p0 < lim[j][0] ? s[j][0] * scale_log2 : -INFINITY, x1 = p0 < lim[j][1] ? s[j][1] * scale_log2 : -INFINITY;
+      const float x2 = p0 + 8 < lim[j][0] ? s[j][2] * scale_log2 : -INFINITY, x3 = p0 + 8 < lim[j][1] ? s[j][3] * scale_log2 : -INFINITY;
+      float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
+#pragma unroll
+      for (int off = 4; off < 32; off <<= 1) {
+        t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
+        t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
+      }
+      const float n0 = fmaxf(m[j][0], t0), n1 = fmaxf(m[j][1], t1);
+      const float r0 = n0 == -INFINITY ? 0.f : n0, r1 = n1 == -INFINITY ? 0.f : n1;  // no key of the column yet: everything stays 0
+      const float a0 = exp2f(m[j][0] - r0), a1 = exp2f(m[j][1] - r1);
+      m[j][0] = n0; m[j][1] = n1;
+      const T p00 = from_f32<T>(exp2f(x0 - r0)), p01 = from_f32<T>(exp2f(x1 - r1));
+      const T p10 = from_f32<T>(exp2f(x2 - r0)), p11 = from_f32<T>(exp2f(x3 - r1));
+      l[j][0] = l[j][0] * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
+      l[j][1] = l[j][1] * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
+#pragma unroll
+      for (int mt = 0; mt < 8; ++mt) { o[j][mt][0] *= a0; o[j][mt][1] *= a1; o[j][mt][2] *= a0; o[j][mt][3] *= a1; }
+      const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
+      const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
+      const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
+      const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
+      pb[j][0] = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
+      pb[j][1] = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
+    }
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) {
+      uint32_t a[4];
+      ldsm4<true>(a, vt + swz(vr, 2 * mt + vc));
+#pragma unroll
+      for (int j = 0; j < NT; ++j) mma16816<T>(o[j][mt], a, pb[j][0], pb[j][1]);
+    }
+  }
+  split_wait<0>();
+#pragma unroll
+  for (int j = 0; j < NT; ++j) {
+#pragma unroll
+    for (int off = 4; off < 32; off <<= 1) {
+      l[j][0] += __shfl_xor_sync(0xffffffffu, l[j][0], off);
+      l[j][1] += __shfl_xor_sync(0xffffffffu, l[j][1], off);
+    }
+  }
+  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][NC][m, l, o[128]]
+  float* wp = reinterpret_cast<float*>(smem);
+#pragma unroll
+  for (int j = 0; j < NT; ++j) {
+    float* w0 = wp + (warp * NC + 8 * j + 2 * qd) * kPartFloats;
+    float* w1 = w0 + kPartFloats;
+    if (g == 0) { w0[0] = m[j][0]; w0[1] = l[j][0]; w1[0] = m[j][1]; w1[1] = l[j][1]; }
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) {
+      w0[2 + 16 * mt + g] = o[j][mt][0]; w1[2 + 16 * mt + g] = o[j][mt][1];
+      w0[2 + 16 * mt + g + 8] = o[j][mt][2]; w1[2 + 16 * mt + g + 8] = o[j][mt][3];
+    }
+  }
+  __syncthreads();
+  const int nc = min(NC, C - cg * NC);  // this CTA's real columns
+  for (int i = tid; i < nc * kHd; i += kSplitThreads) {
+    const int c = i >> 7, d = i & (kHd - 1);
+    float M = -INFINITY;
+    for (int w = 0; w < NW; ++w) M = fmaxf(M, wp[(w * NC + c) * kPartFloats]);
+    float lsum = 0.f, osum = 0.f;
+    if (M != -INFINITY) {
+      for (int w = 0; w < NW; ++w) {
+        const float* e = wp + (w * NC + c) * kPartFloats;
+        const float f = exp2f(e[0] - M);
+        lsum += f * e[1];
+        osum += f * e[2 + d];
+      }
+    }
+    float* dst = part + ((long long)split * NC + c) * kPartFloats;
+    if (d == 0) { dst[0] = M; dst[1] = lsum; }
+    dst[2 + d] = osum;
+  }
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) *last = atomicAdd(tickets, 1u) == (unsigned)(S - 1);
+  __syncthreads();
+  if (!*last) return;
+  __threadfence();
+  for (int i = tid; i < nc * kHd; i += kSplitThreads) {  // split 0 holds key 0, which every column sees: M is finite
+    const int c = i >> 7, d = i & (kHd - 1), col = cg * NC + c;
+    float M = -INFINITY;
+    for (int sp = 0; sp < S; ++sp) M = fmaxf(M, __ldcg(part + ((long long)sp * NC + c) * kPartFloats));
+    float lsum = 0.f, osum = 0.f;
+    for (int sp = 0; sp < S; ++sp) {
+      const float* e = part + ((long long)sp * NC + c) * kPartFloats;
+      const float f = exp2f(__ldcg(e) - M);
+      lsum += f * __ldcg(e + 1);
+      osum += f * __ldcg(e + 2 + d);
+    }
+    out[(((long long)b * TQ + col / G) * n_q + (long long)kvh * G + col % G) * kHd + d] = from_f32<T>(osum / lsum);
+  }
+  if (tid == 0) *tickets = 0u;
+}
+
+// Prompt-lookup drafts (DESIGN.md 3.5).  Slot b knows n = pos[b] + 1 tokens: hist[b][0 .. pos - 1] and tok[b] at pos.  Take the
+// longest g in {3, 2, 1} for which some j with j + g <= n - 1 has hist[j .. j + g - 1] == the last g known tokens, the largest such
+// j, and draft d_{i+1} = token j + g + i while j + g + i < n, else -1; no match: every draft -1.  grid = batch, block = kNgramThreads:
+// one pass over j with the three match lengths, then block max reductions.
+constexpr int kNgramThreads = 512;
+__global__ void __launch_bounds__(kNgramThreads) ngram_draft_kernel(const int* __restrict__ hist, const long long* __restrict__ pos_p,
+                                                                    const long long* __restrict__ tok, long long* __restrict__ drafts, int L, int K) {
+  __shared__ int red[3][kNgramThreads / 32];
+  __shared__ int best[3];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = (int)blockIdx.x, tid = (int)threadIdx.x;
+  const int* h = hist + (long long)b * L;
+  const int pos = (int)pos_p[b], n = pos + 1, last = (int)tok[b];
+  const int s2 = n >= 2 ? h[n - 2] : 0, s3 = n >= 3 ? h[n - 3] : 0;
+  int j1 = -1, j2 = -1, j3 = -1;  // every compared token lies below pos: from hist
+  for (int j = tid; j + 1 <= n - 1; j += kNgramThreads) {
+    const int a0 = h[j];
+    if (a0 == last) j1 = j;
+    if (j + 2 <= n - 1) {
+      const int a1 = h[j + 1];
+      if (a0 == s2 && a1 == last) j2 = j;
+      if (j + 3 <= n - 1 && a0 == s3 && a1 == s2 && h[j + 2] == last) j3 = j;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    j1 = max(j1, __shfl_xor_sync(0xffffffffu, j1, o));
+    j2 = max(j2, __shfl_xor_sync(0xffffffffu, j2, o));
+    j3 = max(j3, __shfl_xor_sync(0xffffffffu, j3, o));
+  }
+  if ((tid & 31) == 0) { red[0][tid >> 5] = j1; red[1][tid >> 5] = j2; red[2][tid >> 5] = j3; }
+  __syncthreads();
+  if (tid < 3) {
+    int v = -1;
+    for (int w = 0; w < kNgramThreads / 32; ++w) v = max(v, red[tid][w]);
+    best[tid] = v;
+  }
+  __syncthreads();
+  const int gl = best[2] >= 0 ? 3 : best[1] >= 0 ? 2 : best[0] >= 0 ? 1 : 0;
+  const int j = gl ? best[gl - 1] : 0;
+  for (int i = tid; i < K; i += kNgramThreads) {
+    const int at = j + gl + i;
+    drafts[(long long)b * K + i] = (gl && at < n) ? (at == pos ? (long long)last : (long long)h[at]) : -1ll;
+  }
+}
+
+// Greedy accept (DESIGN.md 3.5): slot b verified the window [tok, d1 .. dK] at pos .. pos + K with targets t_r = argmax of row r.
+// n = min(K + 1, L - pos); a = the largest r < n with d_i == t_{i-1} for every i <= r.  Emits d1 .. da, t_a (tokens [batch, K + 1],
+// -1 padded), n_new = a + 1; hist[pos .. pos + a] = the accepted window; pos = (pos + a + 1) mod L; tok = next_tok = t_a.
+// grid = ceil(batch / 128), block = 128: one thread per slot.
+__global__ void __launch_bounds__(128) spec_accept_kernel(const long long* __restrict__ targets, const long long* __restrict__ drafts,
+                                                          long long* __restrict__ pos_p, long long* __restrict__ tok, long long* __restrict__ next_tok,
+                                                          int* __restrict__ hist, long long* __restrict__ tokens, long long* __restrict__ n_new, int batch,
+                                                          int K, int L) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  if (b >= batch) return;
+  const int T = K + 1, pos = (int)pos_p[b], n = min(T, L - pos);
+  const long long* tg = targets + (long long)b * T;
+  const long long* d = drafts + (long long)b * K;
+  int a = 0;
+  while (a + 1 < n && d[a] == tg[a]) ++a;
+  int* hr = hist + (long long)b * L;
+  hr[pos] = (int)tok[b];
+  for (int i = 1; i <= a; ++i) hr[pos + i] = (int)d[i - 1];
+  for (int i = 0; i < T; ++i) tokens[(long long)b * T + i] = i < a ? d[i] : (i == a ? tg[a] : -1ll);
+  pos_p[b] = (pos + a + 1) % L;
+  tok[b] = next_tok[b] = tg[a];
+  n_new[b] = a + 1;
+}
+
 // Prompt prefill (DESIGN.md 3.5): a chunk of T positions pos0 .. pos0 + T - 1 of every sequence.
 //
 // rope_append_rows_kernel writes rope(k) and v into cache rows [pos0, pos0 + T) and rope(q) into q_out, rounding exactly as
@@ -1005,22 +1342,32 @@ struct VarlenRows {
 };
 struct NoVarlen {};  // the fixed-length instantiations: their uniform pos0 / T are the scalar arguments
 template <bool VARLEN> using VarlenArg = typename std::conditional<VARLEN, VarlenRows, NoVarlen>::type;
+// Device positions (DEVPOS instantiations, the speculative verify step): slot b's T rows b T + t go to positions pos[b] + t, and only
+// the n[b] = min(T, L - pos[b]) rows that fit in the cache are rotated and written.  pos is read before griddepcontrol.wait, so it
+// must have been written by an earlier, completed launch (the previous step's accept kernel).
+struct DevPos { const long long* pos; };
+template <bool VARLEN, bool DEVPOS> using RowsArg = typename std::conditional<DEVPOS, DevPos, VarlenArg<VARLEN>>::type;
 
 // grid = (T, batch), block = 256.  q / q_out [batch T, n_q 128], k / v [batch T, n_kv 128] (row b T + t), caches [batch, n_kv, L, 128].
-// VARLEN: grid = (max T, batch), rows as VarlenRows lays them out.  PAGED (VARLEN only): page pools, the CTA's position found with one
-// table read.
-template <typename T, bool VARLEN = false, bool PAGED = false>
+// VARLEN: grid = (max T, batch), rows as VarlenRows lays them out.  PAGED (VARLEN or DEVPOS): page pools, the CTA's position found with
+// one table read.  DEVPOS: grid = (T, batch), positions from the device (see DevPos).
+template <typename T, bool VARLEN = false, bool PAGED = false, bool DEVPOS = false>
 __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                                const T* __restrict__ cos_t, const T* __restrict__ sin_t, T* __restrict__ k_cache,
                                                                T* __restrict__ v_cache, T* __restrict__ q_out, int pos0, int n_tok, int n_q,
-                                                               int n_kv, int L, const VarlenArg<VARLEN> vl, const PageArg<PAGED> pg) {
-  static_assert(VARLEN || !PAGED, "a paged cache needs the variable-length layout");
+                                                               int n_kv, int L, const RowsArg<VARLEN, DEVPOS> vl, const PageArg<PAGED> pg) {
+  static_assert(VARLEN || DEVPOS || !PAGED, "a paged cache needs per-slot positions");
+  static_assert(!(VARLEN && DEVPOS), "one row layout");
   const int t = (int)blockIdx.x, b = (int)blockIdx.y;
   long long row = (long long)b * n_tok + t;
   if constexpr (VARLEN) {
     if (t >= vl.n_tok[b]) return;  // past this slot's rows
     pos0 = vl.pos0[b];
     row = (long long)vl.row0[b] + t;
+  }
+  if constexpr (DEVPOS) {
+    pos0 = (int)vl.pos[b];
+    if (t >= L - pos0) return;  // past the end of the cache: neither written nor rotated
   }
   const int p = pos0 + t;
   {
@@ -1057,14 +1404,17 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
 // grid = (T, batch), block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position (k and v of each kv head).
 // Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.  VARLEN as
 // rope_append_rows_kernel.  PAGED as there: levels and meta in the page pools, the staging pair stays [batch, n_kv, L, 128].
-template <typename T, bool VARLEN = false, bool PAGED = false>
+// DEVPOS as rope_append_rows_kernel (positions from the device, rows past the cache end skipped); it writes no staging rows (k_st /
+// v_st unused): the verify attention dequantises the cache itself.
+template <typename T, bool VARLEN = false, bool PAGED = false, bool DEVPOS = false>
 __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                                    const T* __restrict__ cos_t, const T* __restrict__ sin_t, uint8_t* __restrict__ k_q,
                                                                    T* __restrict__ k_s, T* __restrict__ k_z, uint8_t* __restrict__ v_q,
                                                                    T* __restrict__ v_s, T* __restrict__ v_z, T* __restrict__ k_st, T* __restrict__ v_st,
                                                                    T* __restrict__ q_out, int pos0, int n_tok, int n_q, int n_kv, int L, int gs,
-                                                                   const VarlenArg<VARLEN> vl, const PageArg<PAGED> pg) {
-  static_assert(VARLEN || !PAGED, "a paged cache needs the variable-length layout");
+                                                                   const RowsArg<VARLEN, DEVPOS> vl, const PageArg<PAGED> pg) {
+  static_assert(VARLEN || DEVPOS || !PAGED, "a paged cache needs per-slot positions");
+  static_assert(!(VARLEN && DEVPOS), "one row layout");
   const int t = (int)blockIdx.x, b = (int)blockIdx.y, ng = kHd / gs;
   long long row = (long long)b * n_tok + t;
   if constexpr (VARLEN) {
@@ -1072,17 +1422,20 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
     pos0 = vl.pos0[b];
     row = (long long)vl.row0[b] + t;
   }
+  if constexpr (DEVPOS) {
+    pos0 = (int)vl.pos[b];
+    if (t >= L - pos0) return;  // past the end of the cache: neither written nor rotated
+  }
   const int p = pos0 + t;
   {
     const long long kv = (long long)b * n_kv;
     q += row * n_q * kHd; q_out += row * n_q * kHd;
     k += row * n_kv * kHd; v += row * n_kv * kHd;
     if constexpr (!PAGED) {
-      k_q += kv * L * kHd; v_q += kv * L * kHd; k_st += kv * L * kHd; v_st += kv * L * kHd;
+      k_q += kv * L * kHd; v_q += kv * L * kHd;
       k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
-    } else {
-      k_st += kv * L * kHd; v_st += kv * L * kHd;
     }
+    if constexpr (!DEVPOS) { k_st += kv * L * kHd; v_st += kv * L * kHd; }
   }
   long long c0 = 0;  // PAGED: pool row of position p of kv head 0
   if constexpr (PAGED) c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
@@ -1130,7 +1483,7 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
     uint2 y;
     y.x = kv8_deq2<T, 0>(lv, z2, s2);
     y.y = kv8_deq2<T, 1>(lv, z2, s2);
-    *reinterpret_cast<uint2*>((isv ? v_st : k_st) + row * kHd + 4 * lane) = y;
+    if constexpr (!DEVPOS) *reinterpret_cast<uint2*>((isv ? v_st : k_st) + row * kHd + 4 * lane) = y;
   }
 }
 
@@ -2161,6 +2514,205 @@ extern "C" int hqq_b200_glue_attn_prefill_paged(const void* q_rot, const void* k
                       (const E*)k_pool, (const E*)v_pool, (E*)out, 0, 0, n_q_heads, n_kv_heads, cache_len, scale_log2, vl, PageTable{table});
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+// ---- speculative decoding (DESIGN.md 3.5)
+// The checks of the device-position entry points: the prefill shape checks, 1 <= T <= 8 rows per slot, T G <= 64 columns.
+static int spec_args(const char* name, int T, int n_q, int n_kv, int L, int hd, int batch, int dtype) {
+  if (int rc = prefill_args(name, 0, 1, n_q, n_kv, L, hd, batch, dtype)) return rc;
+  HQQ_REQUIRE(T >= 1 && T <= kVerMaxT && T <= L, HQQ_E_INVALID, "%s: needs 1 <= T <= %d and T <= cache_len (T=%d)", name, kVerMaxT, T);
+  HQQ_REQUIRE(T * (n_q / n_kv) <= kVerMaxCols, HQQ_E_UNSUPPORTED, "%s: T * n_q_heads / n_kv_heads must be <= %d", name, kVerMaxCols);
+  return HQQ_OK;
+}
+
+// table == nullptr: contiguous caches; else page pools
+static int rope_append_rows_devpos(const char* name, const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                   void* k_cache, void* v_cache, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                   int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && q_out && pos, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const DevPos dp{(const long long*)pos};
+  auto go = [&](auto tag, auto kernel, auto pg) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows_devpos", kernel, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k, (const E*)v,
+                      (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, 0, T, n_q_heads, n_kv_heads, cache_len, dp, pg);
+  };
+  if (table) {
+    const PageTable pt{table};
+    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kernel<__half, false, true, true>, pt)
+                            : go(__nv_bfloat16(), rope_append_rows_kernel<__nv_bfloat16, false, true, true>, pt);
+  }
+  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kernel<__half, false, false, true>, NoPages())
+                          : go(__nv_bfloat16(), rope_append_rows_kernel<__nv_bfloat16, false, false, true>, NoPages());
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                     void* k_cache, void* v_cache, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                                     int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_append_rows_devpos("hqq_b200_glue_rope_append_rows_devpos", q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, q_out, pos, T,
+                                 n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                           void* k_pool, void* v_pool, const int* table, void* q_out, const int64_t* pos, int T,
+                                                           int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
+                                                           void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_devpos_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_append_rows_devpos(name, q, k, v, cos_table, sin_table, k_pool, v_pool, table, q_out, pos, T, n_q_heads, n_kv_heads, cache_len, head_dim,
+                                 batch, dtype, stream);
+}
+
+// table == nullptr: contiguous 8-bit caches; else page pools
+static int rope_append_rows_kv8_devpos(const char* name, const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                       void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table, void* q_out,
+                                       const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int batch,
+                                       int dtype, void* stream) {
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && q_out && pos, HQQ_E_INVALID,
+              "%s: null pointer", name);
+  if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
+  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  cudaStream_t st = (cudaStream_t)stream;
+  const DevPos dp{(const long long*)pos};
+  auto go = [&](auto tag, auto kernel, auto pg) {
+    using E = decltype(tag);
+    return launch_pdl("rope_append_rows_kv8_devpos", kernel, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k,
+                      (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q, (E*)v_scale,
+                      (E*)v_zero, (E*)nullptr, (E*)nullptr, (E*)q_out, 0, T, n_q_heads, n_kv_heads, cache_len, group_size, dp, pg);
+  };
+  if (table) {
+    const PageTable pt{table};
+    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, true, true>, pt)
+                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, true, true>, pt);
+  }
+  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, false, true>, NoPages())
+                          : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, false, true>, NoPages());
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* q_out,
+                                                         const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                         int group_size, int batch, int dtype, void* stream) {
+  return rope_append_rows_kv8_devpos("hqq_b200_glue_rope_append_rows_kv8_devpos", q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
+                                     v_zero, nullptr, q_out, pos, T, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                               const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
+                                                               void* v_zero, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                                               int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages,
+                                                               int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_kv8_devpos_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_append_rows_kv8_devpos(name, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, q_out, pos, T, n_q_heads,
+                                     n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+}
+
+// column groups of one kv head in the verify attention
+static int verify_groups(int n_q_heads, int n_kv_heads, int T) { return (int)cdiv((int64_t)T * (n_q_heads / n_kv_heads), kVerCols); }
+
+extern "C" size_t hqq_b200_glue_attn_verify_split_workspace_bytes(int n_q_heads, int n_kv_heads, int head_dim, int T, int batch) {
+  if (n_kv_heads <= 0 || n_q_heads <= 0 || n_q_heads % n_kv_heads || head_dim <= 0 || T < 1 || batch <= 0) return 0;
+  const size_t s_max = (size_t)max(1, sm_count() / n_kv_heads);
+  const size_t groups = (size_t)batch * n_kv_heads * verify_groups(n_q_heads, n_kv_heads, T);
+  return groups * s_max * kVerCols * (size_t)(head_dim + 2) * sizeof(float) + groups * sizeof(unsigned);
+}
+
+// table == nullptr: contiguous caches; meta == nullptr: 16-bit caches, else the 8-bit cache's {k_scale, k_zero, v_scale, v_zero}
+static int attn_verify_split(const char* name, const void* q_rot, const void* k_cache, const void* v_cache, const void* const* meta, int gs,
+                             const int* table, const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
+                             int head_dim, int T, int batch, int dtype, void* stream) {
+  HQQ_REQUIRE(q_rot && k_cache && v_cache && pos && out && workspace, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
+  if (meta) {
+    HQQ_REQUIRE(meta[0] && meta[1] && meta[2] && meta[3], HQQ_E_INVALID, "%s: null pointer", name);
+    HQQ_REQUIRE(gs == 64 || gs == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, gs);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int S = split_count(n_kv_heads, cache_len), n_cg = verify_groups(n_q_heads, n_kv_heads, T);
+  const size_t part_bytes = (size_t)batch * n_kv_heads * n_cg * max(1, sm_count() / n_kv_heads) * kVerCols * kPartFloats * sizeof(float);
+  float* part = (float*)workspace;
+  unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
+  const dim3 grid((unsigned)S, (unsigned)(n_kv_heads * n_cg), (unsigned)batch);
+  constexpr int smem = kRingBytes + 16;
+  auto run = [&](auto tag, auto pg, auto paged, auto kv8) -> int {
+    using E = decltype(tag);
+    constexpr bool PG = decltype(paged)::value, K8 = decltype(kv8)::value;
+    using C = CacheT<E, K8>;
+    Kv8Arg<E, K8> m8;
+    if constexpr (K8) m8 = Kv8Meta<E>{(const E*)meta[0], (const E*)meta[1], (const E*)meta[2], (const E*)meta[3], gs};
+    if (int rc = reserve_smem<attn_verify_split_kernel<E, PG, K8>>(smem)) return rc;
+    return launch_pdl(K8 ? "attn_verify_split_kv8" : "attn_verify_split", attn_verify_split_kernel<E, PG, K8>, grid, dim3(kSplitThreads), smem, st,
+                      (const E*)q_rot, (const C*)k_cache, (const C*)v_cache, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads,
+                      cache_len, T, scale_log2, pg, m8);
+  };
+  auto by_dtype = [&](auto pg, auto paged, auto kv8) {
+    return dtype == HQQ_F16 ? run(__half(), pg, paged, kv8) : run(__nv_bfloat16(), pg, paged, kv8);
+  };
+  const PageTable pt{table};
+  if (meta) return table ? by_dtype(pt, std::true_type(), std::true_type()) : by_dtype(NoPages(), std::false_type(), std::true_type());
+  return table ? by_dtype(pt, std::true_type(), std::false_type()) : by_dtype(NoPages(), std::false_type(), std::false_type());
+}
+
+extern "C" int hqq_b200_glue_attn_verify_split(const void* q_rot, const void* k_cache, const void* v_cache, const int64_t* pos, void* out,
+                                               void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int T, int batch, int dtype,
+                                               void* stream) {
+  return attn_verify_split("hqq_b200_glue_attn_verify_split", q_rot, k_cache, v_cache, nullptr, 0, nullptr, pos, out, workspace, n_q_heads, n_kv_heads,
+                           cache_len, head_dim, T, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_attn_verify_split_paged(const void* q_rot, const void* k_pool, const void* v_pool, const int* table, const int64_t* pos,
+                                                     void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int T,
+                                                     int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_attn_verify_split_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return attn_verify_split(name, q_rot, k_pool, v_pool, nullptr, 0, table, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, T, batch,
+                           dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_attn_verify_split_kv8(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero, const void* v_q,
+                                                   const void* v_scale, const void* v_zero, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                   int n_kv_heads, int cache_len, int head_dim, int group_size, int T, int batch, int dtype,
+                                                   void* stream) {
+  const void* meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return attn_verify_split("hqq_b200_glue_attn_verify_split_kv8", q_rot, k_q, v_q, meta, group_size, nullptr, pos, out, workspace, n_q_heads,
+                           n_kv_heads, cache_len, head_dim, T, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_attn_verify_split_kv8_paged(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero, const void* v_q,
+                                                         const void* v_scale, const void* v_zero, const int* table, const int64_t* pos, void* out,
+                                                         void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                                         int T, int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_attn_verify_split_kv8_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  const void* meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return attn_verify_split(name, q_rot, k_q, v_q, meta, group_size, table, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, T, batch,
+                           dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_ngram_draft(const int32_t* hist, const int64_t* pos, const int64_t* tok, int64_t* drafts, int cache_len, int K, int batch,
+                                         void* stream) {
+  const char* name = "hqq_b200_glue_ngram_draft";
+  HQQ_REQUIRE(hist && pos && tok && drafts, HQQ_E_INVALID, "%s: null pointer", name);
+  HQQ_REQUIRE(cache_len > 0 && cache_len <= kSplitMaxLen && K >= 1 && K < kVerMaxT && batch > 0 && batch <= 65535, HQQ_E_INVALID,
+              "%s: needs 0 < cache_len <= %d, 1 <= K <= %d, 0 < batch <= 65535 (cache_len=%d K=%d batch=%d)", name, kSplitMaxLen, kVerMaxT - 1, cache_len,
+              K, batch);
+  return launch_pdl("ngram_draft", ngram_draft_kernel, dim3((unsigned)batch), dim3(kNgramThreads), 0, (cudaStream_t)stream, (const int*)hist,
+                    (const long long*)pos, (const long long*)tok, (long long*)drafts, cache_len, K);
+}
+
+extern "C" int hqq_b200_glue_spec_accept(const int64_t* targets, const int64_t* drafts, int64_t* pos, int64_t* tok, int64_t* next_tok, int32_t* hist,
+                                         int64_t* tokens, int64_t* n_new, int cache_len, int K, int batch, void* stream) {
+  const char* name = "hqq_b200_glue_spec_accept";
+  HQQ_REQUIRE(targets && drafts && pos && tok && next_tok && hist && tokens && n_new, HQQ_E_INVALID, "%s: null pointer", name);
+  HQQ_REQUIRE(cache_len > 0 && cache_len <= kSplitMaxLen && K >= 1 && K < kVerMaxT && batch > 0 && batch <= 65535, HQQ_E_INVALID,
+              "%s: needs 0 < cache_len <= %d, 1 <= K <= %d, 0 < batch <= 65535 (cache_len=%d K=%d batch=%d)", name, kSplitMaxLen, kVerMaxT - 1, cache_len,
+              K, batch);
+  return launch_pdl("spec_accept", spec_accept_kernel, dim3((unsigned)cdiv(batch, 128)), dim3(128), 0, (cudaStream_t)stream, (const long long*)targets,
+                    (const long long*)drafts, (long long*)pos, (long long*)tok, (long long*)next_tok, (int*)hist, (long long*)tokens, (long long*)n_new,
+                    batch, K, cache_len);
 }
 
 extern "C" int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,

@@ -266,6 +266,38 @@ class PageAllocator:
         self.pos = [(p + 1) % self.cache_len for p in self.pos]
         return ops
 
+    def spec_window(self, k: int):
+        """Pages for one speculative verify step (before it runs): an active slot writes rows pos .. pos + n - 1, n = min(k + 1,
+        cache_len - pos).  Every entry the window enters at the page's first row gets a fresh page (the entry the window starts in
+        mid-page is the slot's current page, backed already); at pos == 0 (the wrap) the previous lap's pages are returned first.
+        Positions do not move: spec_advance does that once the accepted counts are known."""
+        spans = {b: (self.pos[b], min(k + 1, self.cache_len - self.pos[b])) for b in range(self.batch) if self.active[b]}
+
+        def run():
+            w, fresh = [], []
+            for b, (p, n) in spans.items():  # every reference is given up before any page is taken
+                if p == 0:
+                    self._clear(w, b)
+                for j in range(p // KV_PAGE, (p + n - 1) // KV_PAGE + 1):
+                    if j * KV_PAGE >= p:
+                        self._drop(self.table[b][j])
+                        fresh.append((b, j))
+            for b, j in fresh:
+                self._set(w, b, j, self._take())
+            return w, []
+        return self._atomic(run)
+
+    def spec_advance(self, n_new):
+        """After a verify step: every slot's position moves by its n_new[b] accepted tokens (mod cache_len), and an active slot's
+        pages that lie wholly at or past its new position (they hold only rejected rows) go back to the pool.  Restores the
+        invariant: entries past the page of the slot's last written row are the sink."""
+        w = []
+        for b in range(self.batch):
+            self.pos[b] = (self.pos[b] + int(n_new[b])) % self.cache_len
+            if self.active[b]:
+                self._clear(w, b, -(-self.pos[b] // KV_PAGE))
+        return w, []
+
     def prefill(self, spans):
         """Back the rows a prefill writes.  spans: {slot: (start, T)}, rows start .. start + T - 1.  A page the prompt enters at its
         first row gets a fresh page; the page it enters mid-page must be backed already and is copied first if shared.  Entries past
@@ -345,7 +377,7 @@ class DecodeModel:
                  device="cuda", cache_len: int = 256, tp: int = 1, rank: int = 0, seed: int = 0, process_group=None,
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
                  kv_bits: int = 16, kv_group_size: int = 64, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
-                 top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None):
+                 top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None, spec_k: int | None = None):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
         # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
         # top-k, top-p, then a Gumbel race on Philox numbers keyed by sample_seed and countered by _sample_ctr -- instead of the argmax.
@@ -388,6 +420,17 @@ class DecodeModel:
             if not self.ragged:
                 raise ValueError("kv_pages needs ragged=True")
             self.pages = PageAllocator(kv_pages, self.batch, cache_len)
+        # spec_k K (ragged, greedy): decode_spec() verifies the window [tok, d1 .. dK] of every slot in one captured pass and emits
+        # the accepted drafts plus one target (include/hqq_b200.h states the rule); the drafts come from prompt lookup over the
+        # device token history `hist` [batch, cache_len] or from the caller.
+        self.spec_k = spec_k
+        if spec_k is not None:
+            if not self.ragged:
+                raise ValueError("spec_k needs ragged=True")
+            if do_sample:
+                raise ValueError("spec_k verifies greedy targets: it cannot be combined with do_sample")
+            if not (isinstance(spec_k, int) and 1 <= spec_k <= 7):
+                raise ValueError(f"spec_k must be an int in [1, 7] (got {spec_k!r})")
         if (self.batch > 1 or self.ragged) and fused:
             fused = True  # the 8-launch path with the batched glue kernels; the one-token kernels (fused=5) and their exchange are M = 1 only
         self.fused = fused
@@ -464,6 +507,14 @@ class DecodeModel:
         self._sample_ctr = torch.zeros(1, dtype=torch.long, device=self.device)  # Philox counter: + 1 per sampled token
         if kv_pages is not None:
             self.page_table = torch.full((self.batch, cache_len // KV_PAGE), kv_pages, dtype=torch.int32, device=self.device)
+        if spec_k is not None:  # hist[b][p] = the token fed at position p; the verify step's static I/O
+            self.hist = torch.zeros(self.batch, cache_len, dtype=torch.int32, device=self.device)
+            self._spec_drafts = torch.full((self.batch, spec_k), -1, dtype=torch.long, device=self.device)
+            self._spec_targets = torch.zeros(self.batch * (spec_k + 1), dtype=torch.long, device=self.device)
+            self._spec_tokens = torch.full((self.batch, spec_k + 1), -1, dtype=torch.long, device=self.device)
+            self._spec_n_new = torch.zeros(self.batch, dtype=torch.long, device=self.device)
+            self.spec_graph = None
+            self.spec_logits = None  # [batch, K + 1, vocab / tp]: the last verify step's logits
         self.graph = None
         self.last_logits = None  # set by prefill(): logits of the last prompt position of each sequence
 
@@ -520,6 +571,8 @@ class DecodeModel:
         self._apply_pages(self.pages.fork(src, dst))
         self.pos[dst].copy_(self.pos[src])
         self.tok[dst].copy_(self.tok[src])
+        if self.spec_k is not None:
+            self.hist[dst].copy_(self.hist[src])
 
     def _paged_only(self, what):
         if self.kv_pages is None:
@@ -584,6 +637,7 @@ class DecodeModel:
         s = self.shape
         B = self.batch
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
+        self._hist_write()
         h = self.embed.index_select(0, self.tok)  # [B, hidden]
         if self.ragged:  # sequence b at position pos[b]: its own RoPE row and causal mask
             cos = self.cos.index_select(0, self.pos).view(B, 1, hd)
@@ -646,6 +700,11 @@ class DecodeModel:
         else:
             self.next_tok.copy_(torch.argmax(logits, dim=-1))
         self.pos.add_(1).remainder_(self.cache_len)
+
+    def _hist_write(self):
+        """spec_k: a decode step records its input token in the prompt-lookup history, hist[b][pos[b]] = tok[b]."""
+        if self.spec_k is not None:
+            self.hist.scatter_(1, self.pos.view(-1, 1), self.tok.view(-1, 1).to(torch.int32))
 
     def _kv8_write(self, blk, k, v, idx):
         """kv_bits 8 on framework ops: rows k, v [batch, n_kv, n, 128] quantised into cache positions idx [n]."""
@@ -715,16 +774,8 @@ class DecodeModel:
         if self.do_sample:
             self._sample(lib, self._sample_rows(b["logits"], b), self.next_tok, code, st)
             return
-        if self.batch > 1:  # a row per sequence: framework ops (with tp > 1: the global maximum, then the lowest index that attains it)
-            if self.tp == 1:
-                self.next_tok.copy_(torch.argmax(b["logits"], dim=-1))
-                return
-            val, idx = torch.max(b["logits"].float(), dim=-1)
-            gmax = val.clone()
-            torch.distributed.all_reduce(gmax, op=torch.distributed.ReduceOp.MAX, group=self.pg)
-            cand = torch.where(val == gmax, idx + self.rank * self.vocab_shard, torch.full_like(idx, self.shape.vocab))
-            torch.distributed.all_reduce(cand, op=torch.distributed.ReduceOp.MIN, group=self.pg)
-            self.next_tok.copy_(cand)
+        if self.batch > 1:  # a row per sequence: framework ops
+            self.next_tok.copy_(self._greedy(b["logits"]))
             return
         if self.tp == 1:
             check(lib.hqq_b200_glue_argmax(ptr(b["logits"]), self.vocab_shard, ptr(self.next_tok), code, st))
@@ -763,6 +814,7 @@ class DecodeModel:
         inter = s.inter // self.tp
         b = self._bufs
         B = self.batch
+        self._hist_write()
         torch.index_select(self.embed, 0, self.tok, out=b["h"])  # [B, hidden]
         delta = None
         norm = lambda d, w: check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(b["h"]), ptr(d), ptr(w), ptr(b["x"]), B, s.hidden, s.rms_eps, code, st))
@@ -981,6 +1033,9 @@ class DecodeModel:
             raise ValueError("chunk must be >= 1")
         if self.kv_pages is not None:  # back every row the prompts write (fresh pages, copy-on-write of a shared partial page)
             self._apply_pages(self.pages.prefill({b: (starts[b], int(toks[b].numel())) for b in slots}))
+        if self.spec_k is not None:  # the prompt joins the prompt-lookup history
+            for b in slots:
+                self.hist[b, starts[b]:starts[b] + toks[b].numel()] = toks[b].to(torch.int32)
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         last = {}
         with torch.no_grad():
@@ -1014,10 +1069,11 @@ class DecodeModel:
         self.pos.index_copy_(0, idx, torch.tensor([(starts[b] + int(toks[b].numel())) % L for b in slots], device=self.device))
         return self.tok.clone()
 
-    def _prefill_chunk_fused(self, ids, p0, hd, hq, hkv, varlen=None):
+    def _prefill_chunk_fused(self, ids, p0, hd, hq, hkv, varlen=None, attn=None):
         """One chunk on the package's kernels; returns the residual stream h [M, hidden] before the last block's MLP delta, and
         that delta (the final norm adds them for the rows it needs).  varlen = (pos0, n_tok) host lists of the ragged batch's slots:
-        ids [1, M] packed in slot order and the _varlen kernels (p0 unused)."""
+        ids [1, M] packed in slot order and the _varlen kernels (p0 unused).  attn(blk, q, k, v, q_rot, out): the cache append and
+        attention step in place of the prefill kernels (the speculative verify pass)."""
         from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
         lib, s = load(), self.shape
         st = stream_ptr(self.device)
@@ -1039,12 +1095,14 @@ class DecodeModel:
         paged = self.kv_pages is not None
         if paged:
             pt, npg = ptr(self.page_table), self.kv_pages
-        if kv8 and self._kv8_stage is None:  # one staging pair for all layers: [batch, n_kv, cache_len, 128] each
+        if kv8 and attn is None and self._kv8_stage is None:  # one staging pair for all layers: [batch, n_kv, cache_len, 128] each
             self._kv8_stage = tuple(torch.zeros(B, hkv, self.cache_len, hd, device=self.device, dtype=self.dtype) for _ in range(2))
         for blk in self.blocks:
             norm(delta, blk["norm1"])
             self._lin(x, (blk["q"], blk["k"], blk["v"]), [q, k, v])
-            if kv8:
+            if attn is not None:
+                attn(blk, q, k, v, qr, a)
+            elif kv8:
                 # staging rows [0, p0) dequantised from the 8-bit cache, rows [p0, p0 + n) written by the rows kernel; the attention
                 # kernel is the one of the fp16 cache, reading the staging pair
                 kst, vst = self._kv8_stage
@@ -1085,7 +1143,9 @@ class DecodeModel:
                 check(lib.hqq_b200_glue_rope_append_rows(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
                                                          ptr(qr), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
                 kc, vc = blk["k_cache"], blk["v_cache"]
-            if paged and not kv8:
+            if attn is not None:
+                pass  # the hook's attention output is in a already
+            elif paged and not kv8:
                 check(lib.hqq_b200_glue_attn_prefill_paged(ptr(qr), ptr(kc), ptr(vc), pt, ptr(a), vp0, vnt, hq, hkv, self.cache_len, hd, B, npg, code, st))
             elif varlen is not None:
                 check(lib.hqq_b200_glue_attn_prefill_varlen(ptr(qr), ptr(kc), ptr(vc), ptr(a), vp0, vnt, hq, hkv, self.cache_len, hd, B, code, st))
@@ -1251,6 +1311,8 @@ class DecodeModel:
         if self.kv_pages is not None:  # every page free, every entry the sink, every slot active at position 0
             self.pages.reset()
             self.page_table.fill_(self.kv_pages)
+        if self.spec_k is not None:
+            self.hist.zero_()
         for blk in self.blocks:
             for name in ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero"):
                 if name in blk:
@@ -1268,6 +1330,205 @@ class DecodeModel:
         self.graph.replay()
         if feed_back:
             self.tok.copy_(self.next_tok)
+
+    # ---- speculative decoding (spec_k)
+    def _spec_window_ids(self):
+        """The verify rows [batch, K + 1]: tok, then the drafts (a -1 sentinel embeds as token 0: it never matches, so no row
+        after it is accepted)."""
+        return torch.cat([self.tok.view(-1, 1), self._spec_drafts.clamp_min(0)], dim=1)
+
+    def _greedy(self, logits):
+        """Targets of logits rows [M, vocab / tp], first index on ties: torch.argmax at tp = 1, else the global maximum and then
+        the lowest global index that attains it (two small all-reduces), as the batched head does."""
+        if self.tp == 1:
+            return torch.argmax(logits, dim=-1)
+        val, idx = torch.max(logits.float(), dim=-1)
+        gmax = val.clone()
+        torch.distributed.all_reduce(gmax, op=torch.distributed.ReduceOp.MAX, group=self.pg)
+        cand = torch.where(val == gmax, idx + self.rank * self.vocab_shard, torch.full_like(idx, self.shape.vocab))
+        torch.distributed.all_reduce(cand, op=torch.distributed.ReduceOp.MIN, group=self.pg)
+        return cand
+
+    def verify_fused(self):
+        """One speculative verify step on the package's kernels: the window [tok, d1 .. dK] of every slot runs the prefill block walk
+        (_prefill_chunk_fused) at M = batch (K + 1) rows, with the device-position append and the verify attention as its attention
+        step; every row goes through the final norm and the lm_head, the targets are the rows' greedy picks, and one
+        hqq_b200_glue_spec_accept launch emits the accepted tokens and advances pos, tok, next_tok and hist on the device."""
+        from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
+        lib, s = load(), self.shape
+        st = stream_ptr(self.device)
+        code = DTYPE_CODE[self.dtype]
+        B, K, L = self.batch, self.spec_k, self.cache_len
+        T = K + 1
+        hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
+        ws = self._bufs["verify_ws"]
+
+        def attn(blk, q, k, v, qr, a):
+            if self.kv_bits == 8:
+                c8 = [ptr(blk[n]) for n in ("k_cache", "k_scale", "k_zero", "v_cache", "v_scale", "v_zero")]
+                gs = self.kv_group_size
+                if self.kv_pages is None:
+                    check(lib.hqq_b200_glue_rope_append_rows_kv8_devpos(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, ptr(qr), ptr(self.pos), T,
+                                                                        hq, hkv, L, hd, gs, B, code, st))
+                    check(lib.hqq_b200_glue_attn_verify_split_kv8(ptr(qr), *c8, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B, code, st))
+                    return
+                pt = ptr(self.page_table)
+                check(lib.hqq_b200_glue_rope_append_rows_kv8_devpos_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, pt, ptr(qr),
+                                                                          ptr(self.pos), T, hq, hkv, L, hd, gs, B, self.kv_pages, code, st))
+                check(lib.hqq_b200_glue_attn_verify_split_kv8_paged(ptr(qr), *c8, pt, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B,
+                                                                    self.kv_pages, code, st))
+                return
+            if self.kv_pages is None:
+                check(lib.hqq_b200_glue_rope_append_rows_devpos(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                                ptr(blk["v_cache"]), ptr(qr), ptr(self.pos), T, hq, hkv, L, hd, B, code, st))
+                check(lib.hqq_b200_glue_attn_verify_split(ptr(qr), ptr(blk["k_cache"]), ptr(blk["v_cache"]), ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L,
+                                                          hd, T, B, code, st))
+                return
+            pt = ptr(self.page_table)
+            check(lib.hqq_b200_glue_rope_append_rows_devpos_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                                                                  ptr(blk["v_cache"]), pt, ptr(qr), ptr(self.pos), T, hq, hkv, L, hd, B, self.kv_pages,
+                                                                  code, st))
+            check(lib.hqq_b200_glue_attn_verify_split_paged(ptr(qr), ptr(blk["k_cache"]), ptr(blk["v_cache"]), pt, ptr(self.pos), ptr(a), ptr(ws), hq,
+                                                            hkv, L, hd, T, B, self.kv_pages, code, st))
+
+        h, delta = self._prefill_chunk_fused(self._spec_window_ids(), 0, hd, hq, hkv, attn=attn)
+        x = torch.empty_like(h)
+        check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(delta), ptr(self.final_norm), ptr(x), B * T, s.hidden, s.rms_eps, code, st))
+        logits = self._bufs["verify_logits"]
+        torch.matmul(x, self.lm_head.t(), out=logits)
+        self._spec_targets.copy_(self._greedy(logits))
+        check(lib.hqq_b200_glue_spec_accept(ptr(self._spec_targets), ptr(self._spec_drafts), ptr(self.pos), ptr(self.tok), ptr(self.next_tok),
+                                            ptr(self.hist), ptr(self._spec_tokens), ptr(self._spec_n_new), L, K, B, st))
+
+    def verify(self):
+        """The same verify step on framework ops (fused=False), the reference: per-row RoPE, the window's valid rows (t < n[b]) written
+        into the caches (through the page table when paged; kv_bits 8: quantised by kv8_quantize_rows, attention over the
+        dequantised cache), SDPA with the per-slot causal masks key <= pos[b] + t, the head, and
+        the accept rule restated with tensor ops."""
+        s, B, K, L = self.shape, self.batch, self.spec_k, self.cache_len
+        T = K + 1
+        hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
+        dev = self.device
+        ids = self._spec_window_ids()
+        rows = self.pos.view(B, 1) + torch.arange(T, device=dev).view(1, T)  # [B, T] positions
+        n = torch.clamp(L - self.pos, max=T)
+        valid = torch.arange(T, device=dev).view(1, T) < n.view(B, 1)
+        at_rows = torch.where(valid, rows, torch.zeros_like(rows))  # rows past the cache: any RoPE row, never written
+        cos, sin = self.cos[at_rows].view(B, T, 1, hd), self.sin[at_rows].view(B, T, 1, hd)
+        mask = (self.arange.view(1, 1, L) <= rows.view(B, T, 1)).view(B, 1, T, L)
+        bi, ti = valid.nonzero(as_tuple=True)
+        p = rows[bi, ti]
+        at = (bi, slice(None), p) if self.kv_pages is None else (self.page_table[bi, p // KV_PAGE].long(), slice(None), p % KV_PAGE)
+        h = self.embed.index_select(0, ids.reshape(-1))
+        for blk in self.blocks:
+            x = F.rms_norm(h, (s.hidden,), blk["norm1"], s.rms_eps)
+            q, k, v = self._multi(x, (blk["q"], blk["k"], blk["v"]))
+            q = self._rope(q.view(B, T, hq, hd), cos, sin)
+            k = self._rope(k.view(B, T, hkv, hd), cos, sin)
+            for name, x in (("k", k[bi, ti]), ("v", v.view(B, T, hkv, hd)[bi, ti])):
+                if self.kv_bits == 8:
+                    for suffix, val in zip(("_cache", "_scale", "_zero"), kv8_quantize_rows(x, self.kv_group_size)):
+                        blk[name + suffix][at] = val
+                else:
+                    blk[name + "_cache"][at] = x
+            cv = self.cache_view(blk)
+            kc, vc = self._kv8_read(cv, L) if self.kv_bits == 8 else (cv["k_cache"], cv["v_cache"])
+            a = F.scaled_dot_product_attention(q.transpose(1, 2), kc, vc, attn_mask=mask, enable_gqa=True)
+            o = blk["o"](a.transpose(1, 2).reshape(B * T, hq * hd))
+            if self.tp > 1:
+                torch.distributed.all_reduce(o, group=self.pg)
+            h = h + o
+            x = F.rms_norm(h, (s.hidden,), blk["norm2"], s.rms_eps)
+            g, u = self._multi(x, (blk["gate"], blk["up"]))
+            y = blk["down"](F.silu(g) * u)
+            if self.tp > 1:
+                torch.distributed.all_reduce(y, group=self.pg)
+            h = h + y
+        h = F.rms_norm(h, (s.hidden,), self.final_norm, s.rms_eps)
+        logits = torch.matmul(h, self.lm_head.t())
+        self.spec_logits = logits.view(B, T, -1)
+        tg = self._greedy(logits).view(B, T)
+        d = self._spec_drafts
+        ok = (d == tg[:, :K]) & (torch.arange(1, T, device=dev).view(1, K) < n.view(B, 1))
+        a = torch.cumprod(ok.long(), dim=1).sum(dim=1)  # accepted drafts
+        i = torch.arange(T, device=dev).view(1, T)
+        t_a = tg.gather(1, a.view(B, 1))
+        self._spec_tokens.copy_(torch.where(i < a.view(B, 1), torch.cat([d, d[:, :1]], 1), torch.where(i == a.view(B, 1), t_a, -1)))
+        window = torch.cat([self.tok.view(B, 1), d], 1)
+        for r in range(T):  # hist[pos + r] = window[r] for r <= a
+            idx = (self.pos + r).clamp(max=L - 1).view(B, 1)
+            cur = self.hist.gather(1, idx)
+            self.hist.scatter_(1, idx, torch.where((r <= a).view(B, 1), window[:, r:r + 1].to(torch.int32), cur))
+        self._spec_targets.copy_(tg.view(-1))
+        self._spec_n_new.copy_(a + 1)
+        self.pos.copy_((self.pos + a + 1) % L)
+        self.tok.copy_(t_a.view(B))
+        self.next_tok.copy_(t_a.view(B))
+
+    def capture_spec(self, warmup: int = 3):
+        """Capture one verify step (verify_fused) into self.spec_graph.  The warm-up runs on the current state and puts back pos,
+        tok, next_tok and hist afterwards; the cache rows it wrote lie past the slots' positions, where no step reads.  fused=False
+        needs no capture: decode_spec() runs verify() eagerly."""
+        if self.spec_k is None:
+            raise ValueError("capture_spec needs spec_k")
+        if not self.fused:
+            raise ValueError("capture_spec needs a fused model (fused=False runs verify() eagerly in decode_spec)")
+        if not hasattr(self, "_bufs"):
+            self._alloc_bufs()
+        if "verify_ws" not in self._bufs:
+            from ._lib import load
+            s, tp, T = self.shape, self.tp, self.spec_k + 1
+            with torch.cuda.device(self.device):
+                nbytes = load().hqq_b200_glue_attn_verify_split_workspace_bytes(s.n_heads // tp, s.n_kv_heads // tp, s.head_dim, T, self.batch)
+            self._bufs["verify_ws"] = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+            self._bufs["verify_logits"] = torch.zeros(self.batch * T, self.vocab_shard, dtype=self.dtype, device=self.device)
+        self.spec_logits = self._bufs["verify_logits"].view(self.batch, self.spec_k + 1, -1)
+        saved = [t.clone() for t in (self.pos, self.tok, self.next_tok, self.hist, self._spec_drafts)]
+        self._spec_drafts.fill_(-1)
+        st = torch.cuda.Stream(device=self.device)
+        st.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(st), torch.no_grad():
+            for _ in range(warmup):
+                self.verify_fused()
+        torch.cuda.current_stream(self.device).wait_stream(st)
+        torch.cuda.synchronize(self.device)
+        for t, v in zip((self.pos, self.tok, self.next_tok, self.hist, self._spec_drafts), saved):
+            t.copy_(v)
+        self.spec_graph = torch.cuda.CUDAGraph()
+        with torch.no_grad(), torch.cuda.graph(self.spec_graph):
+            self.verify_fused()
+        return self.spec_graph
+
+    def decode_spec(self, drafts: torch.Tensor | None = None):
+        """One speculative step for every slot: drafts from prompt lookup (hqq_b200_glue_ngram_draft over hist, launched in front of
+        the replay) or the caller's device int64 [batch, K] (-1 for none), then the captured verify step (fused=False: verify()).
+        Caller drafts outside [0, vocab) count as -1 (mapped on the device).
+        Returns (tokens [batch, K + 1] with -1 after the emitted ones, n_new [batch]) as device tensors; tok / next_tok hold the last
+        emitted token, so decode() and decode_spec() may be interleaved.  No synchronisation, except with kv_pages: the pages past
+        the accepted tokens are returned by spec_advance, which reads n_new to the host once per call."""
+        from ._lib import check, load, ptr, stream_ptr
+        if self.spec_k is None:
+            raise ValueError("decode_spec needs spec_k")
+        B, K = self.batch, self.spec_k
+        if drafts is None:
+            check(load().hqq_b200_glue_ngram_draft(ptr(self.hist), ptr(self.pos), ptr(self.tok), ptr(self._spec_drafts), self.cache_len, K, B,
+                                                   stream_ptr(self.device)))
+        else:
+            if not (torch.is_tensor(drafts) and drafts.shape == (B, K) and drafts.device == self.device and not drafts.is_floating_point()):
+                raise ValueError(f"drafts must be an integer tensor [batch={B}, K={K}] on {self.device}")
+            self._spec_drafts.copy_(torch.where((drafts >= 0) & (drafts < self.shape.vocab), drafts, -1))
+        if self.kv_pages is not None:
+            self._apply_pages(self.pages.spec_window(K))
+        with torch.no_grad():
+            if self.fused:
+                if self.spec_graph is None:
+                    raise RuntimeError("decode_spec on a fused model needs capture_spec() first")
+                self.spec_graph.replay()
+            else:
+                self.verify()
+        if self.kv_pages is not None:
+            self._apply_pages(self.pages.spec_advance(self._spec_n_new.tolist()))
+        return self._spec_tokens.clone(), self._spec_n_new.clone()
 
 
 # ---------------------------------------------------------------------------------------------- quantise-only sharding (SURVEY 8e)

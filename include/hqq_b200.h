@@ -390,6 +390,70 @@ int hqq_b200_glue_kv8_stage_paged(const void* k_q, const void* k_scale, const vo
 int hqq_b200_glue_attn_prefill_paged(const void* q_rot, const void* k_pool, const void* v_pool, const int* table, void* out,
                                      const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads, int cache_len,
                                      int head_dim, int batch, int n_pages, int dtype, void* stream);
+
+/* Speculative decoding (greedy, DecodeModel(ragged=True, spec_k=K), 1 <= K <= 7).  Slot b sits at position pos[b] with next input
+ * tok[b].  One verify step feeds the window [tok, d1 .. dK] at positions pos .. pos + K (row b T + t, T = K + 1); only the
+ * n[b] = min(T, cache_len - pos[b]) rows that fit in the cache are valid.  Row r's target is t_r = argmax(logits_r) (first index on
+ * ties).  a = the largest r < n[b] with d_i == t_{i-1} for every i <= r; the slot emits d1 .. da, t_a (a + 1 tokens), then
+ * pos <- (pos + a + 1) mod cache_len, tok <- t_a, next_tok <- t_a.  Cache rows past the new position may hold rejected rows; they
+ * are never read.  A draft of -1 matches no target.
+ *
+ * rope_append_rows_devpos: the rows kernel with device positions: row b T + t goes to position pos[b] + t; rows t >= n[b] are
+ * neither written nor rotated into q_out.  Written rows are bit for bit those of the _varlen entry point called with pos0 = pos.
+ * pos is read before the programmatic wait: it must come from an earlier, completed launch.  1 <= T <= 8, T * n_q / n_kv <= 64.
+ * The _paged twin writes through the page table. */
+int hqq_b200_glue_rope_append_rows_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                          void* k_cache, void* v_cache, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                          int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                const void* sin_table, void* k_pool, void* v_pool, const int* table, void* q_out,
+                                                const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                int batch, int n_pages, int dtype, void* stream);
+/* Verify attention: out row b T + t, head h = softmax over cache rows 0 .. pos[b] + t of q_rot row b T + t (rotated, as the
+ * rows kernel leaves it) against the cache, every row read from the cache (the devpos append writes rows pos .. just before).
+ * Split-KV like rope_attn_decode_split (grid (S, n_kv * n_cg, batch), S = max(1, min(SMs / n_kv, ceil(cache_len / 16)))); the
+ * (t, head) pairs of a GQA group are the MMA columns, 16 per CTA, n_cg = ceil(T * n_q / n_kv / 16) column groups per kv head.
+ * Rows t >= n[b] are undefined (their q_rot rows are not written).  workspace: hqq_b200_glue_attn_verify_split_workspace_bytes() =
+ * batch * n_kv * n_cg * max(1, SMs / n_kv) * 16 * (head_dim + 2) * 4 bytes of partials, one per column, then
+ * batch * n_kv * n_cg uint32 tickets, zeroed once (every launch leaves them at zero).  1 <= T <= 8, T * n_q / n_kv <= 64. */
+size_t hqq_b200_glue_attn_verify_split_workspace_bytes(int n_q_heads, int n_kv_heads, int head_dim, int T, int batch);
+int hqq_b200_glue_attn_verify_split(const void* q_rot, const void* k_cache, const void* v_cache, const int64_t* pos, void* out,
+                                    void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int T, int batch,
+                                    int dtype, void* stream);
+int hqq_b200_glue_attn_verify_split_paged(const void* q_rot, const void* k_pool, const void* v_pool, const int* table,
+                                          const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
+                                          int head_dim, int T, int batch, int n_pages, int dtype, void* stream);
+/* 8-bit HQQ cache (levels uint8 and meta [.., 128 / gs] T, as hqq_b200_glue_rope_append_rows_kv8): the devpos append quantises
+ * the valid rows into the cache exactly as the _varlen kv8 append does and writes no staging rows; the verify attention
+ * dequantises every attended row, T(T(q - z) * s) as hqq_b200_dequantize gives it, into the 16-bit tile the 16-bit form uses.
+ * Same workspace.  group_size 64 or 128. */
+int hqq_b200_glue_rope_append_rows_kv8_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                              void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                              void* q_out, const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len,
+                                              int head_dim, int group_size, int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_kv8_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                    const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q,
+                                                    void* v_scale, void* v_zero, const int* table, void* q_out, const int64_t* pos, int T,
+                                                    int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int batch,
+                                                    int n_pages, int dtype, void* stream);
+int hqq_b200_glue_attn_verify_split_kv8(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero, const void* v_q,
+                                        const void* v_scale, const void* v_zero, const int64_t* pos, void* out, void* workspace,
+                                        int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int T, int batch,
+                                        int dtype, void* stream);
+int hqq_b200_glue_attn_verify_split_kv8_paged(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero,
+                                              const void* v_q, const void* v_scale, const void* v_zero, const int* table,
+                                              const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
+                                              int cache_len, int head_dim, int group_size, int T, int batch, int n_pages, int dtype,
+                                              void* stream);
+/* Prompt-lookup drafts: slot b knows L = pos[b] + 1 tokens, hist[b][0 .. pos - 1] (int32 [batch, cache_len]) and tok[b] at pos.
+ * Take the longest g in {3, 2, 1} for which some j with j + g <= L - 1 has hist[j .. j+g-1] == the last g tokens, the largest such
+ * j, and write drafts[b][i] = token j + g + i while j + g + i < L, else -1 (int64 [batch, K]); no match: every draft -1. */
+int hqq_b200_glue_ngram_draft(const int32_t* hist, const int64_t* pos, const int64_t* tok, int64_t* drafts, int cache_len, int K,
+                              int batch, void* stream);
+/* Accept and advance: from targets int64 [batch, K + 1] and drafts int64 [batch, K], as defined above: tokens int64 [batch, K + 1]
+ * (d1 .. da, t_a, then -1), n_new[b] = a + 1, hist[b][pos .. pos + a] = the accepted window, and pos, tok, next_tok advanced. */
+int hqq_b200_glue_spec_accept(const int64_t* targets, const int64_t* drafts, int64_t* pos, int64_t* tok, int64_t* next_tok,
+                              int32_t* hist, int64_t* tokens, int64_t* n_new, int cache_len, int K, int batch, void* stream);
 /* out[0] = argmax(logits[0..n)) (first index on ties) */
 int hqq_b200_glue_argmax(const void* logits, int n, int64_t* out, int dtype, void* stream);
 /* Vocabulary-sharded lm_head (tensor parallel decode): out_key[0] = a signed 64-bit key {ordered(max) : 0xFFFFFFFF - (index_offset +
