@@ -41,6 +41,8 @@ SIGNATURES = {
                                      c_size_t, c_void_p]),
     "hqq_b200_linear_fwd_workspace_bytes": (c_size_t, [c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int]),
     "hqq_b200_dense_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p]),
+    "hqq_b200_lm_logprob_workspace_bytes": (c_size_t, [c_int64, c_int64]),
+    "hqq_b200_lm_logprob": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "hqq_b200_linear_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
                                     c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "hqq_b200_linear_fwd_multi": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,

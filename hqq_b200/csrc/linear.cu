@@ -15,6 +15,9 @@ int linear_gemm(const void* x, const void* Wq, const void* scale, const void* ze
                 int64_t N, int64_t K, int gs, int nbits, int dtype, void* ws, size_t ws_bytes, cudaStream_t st);
 bool dense_route_ok(int64_t M, int64_t N, int64_t K, int dtype);
 int linear_dense(const void* x, const void* W, const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, cudaStream_t st);
+size_t lm_logprob_ws_bytes(int64_t M, int64_t N);
+int lm_logprob(const void* x, const void* W, const int64_t* targets, float* lse, float* tgt, void* ws, int64_t M, int64_t N, int64_t K,
+               int64_t index_offset, int dtype, cudaStream_t st);
 }  // namespace hqq
 
 using namespace hqq;
@@ -89,6 +92,13 @@ extern "C" int hqq_b200_linear_fwd(const void* x, const void* W_q, const void* s
 extern "C" int hqq_b200_dense_gemm(const void* x, const void* W, const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
                                    void* stream) {
   return linear_dense(x, W, bias, y, M, N, K, dtype, (cudaStream_t)stream);
+}
+
+extern "C" size_t hqq_b200_lm_logprob_workspace_bytes(int64_t M, int64_t N) { return lm_logprob_ws_bytes(M, N); }
+
+extern "C" int hqq_b200_lm_logprob(const void* x, const void* W, const int64_t* targets, float* lse, float* tgt, void* workspace, int64_t M,
+                                   int64_t N, int64_t K, int64_t index_offset, int dtype, void* stream) {
+  return lm_logprob(x, W, targets, lse, tgt, workspace, M, N, K, index_offset, dtype, (cudaStream_t)stream);
 }
 
 extern "C" int hqq_b200_linear_fwd_multi(const void* x, int count, const void* const* W_q, const void* const* scale,

@@ -61,6 +61,12 @@ struct Args {
   int step;  // packed rows = N / F
   int Gk;    // groups per row = K / GS
   Sched sched;
+  // LSE epilogue only (hqq_b200_lm_logprob): targets int64 [M], this shard's first vocabulary row, tgt fp32 [M] (written where the
+  // target lies in the shard), part [n_row][M] = (max, sum of exp) of each vocabulary tile and position
+  const int64_t* targets;
+  long long index_offset;
+  float* tgt;
+  float2* part;
 };
 
 struct Item { int tile_n, m0, un, kb0, kb1, slice, tile; bool valid; };
@@ -254,16 +260,20 @@ struct Smem {
   static constexpr int A_STAGE = kTileRows * 128;  // 128 rows x 128 B
   static constexpr int B_STAGE = kUN * 128;
   static constexpr int BYTES = kStages * (A_STAGE + B_STAGE) + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int XCH = kMmaThreads / 32 * kUN * 8;  // LSE epilogue: (max, sum) of each MMA warp's 16 rows per token column
 };
 
 // NBITS = 16 ("dense"): the A operand is an ordinary [N, K] fp16/bf16 matrix fetched by TMA like B -- the dequant warps idle.  It is
 // the second half of the routes no fused expansion exists for (3-bit's 10-field int32 slabs, axis = 0 groups, other group sizes,
 // the backward pass): our dequantize kernel writes W_r once, this kernel multiplies (hqq_b200_linear_fwd route 3).
-template <typename T, int NBITS, int GS>
+// LSE (dense only, W = an lm_head shard): the epilogue reduces each [128 vocabulary rows x UN tokens] tile of T-rounded logits to a
+// per-token (max, sum of exp) and picks out the target's logit (hqq_b200_lm_logprob); the logits never reach memory.
+template <typename T, int NBITS, int GS, bool LSE = false>
 __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_constant__ CUtensorMap xmap_full,
                                                                   const __grid_constant__ CUtensorMap xmap_half,
                                                                   const __grid_constant__ CUtensorMap amap, const Args a) {
   constexpr bool DENSE = NBITS == 16;
+  static_assert(!LSE || DENSE, "the LSE epilogue is an instantiation of the dense kernel");
   constexpr int F = DENSE ? 1 : 8 / NBITS;  // slabs per byte
   constexpr int PR = kTileRows / F;        // packed rows per tile
   constexpr int BPT = DENSE ? 32 : 64 * PR / kDequantThreads;  // packed bytes per dequant thread and k-block (32 / F)
@@ -370,6 +380,53 @@ __global__ void __launch_bounds__(kThreads, 1) linear_gemm_kernel(const __grid_c
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[(it - 1) % kStages]);
+      if constexpr (LSE) {
+        // ---- LSE epilogue: per token column, the tile's T-rounded logits of rows < N -> (max, sum of exp(l - max)) in fp32 ----
+        // A warp holds 16 rows (r0, r0 + 8 over its 8 lane quads): shuffles over the quads, then the 8 warps' partials meet in
+        // shared memory and one thread per column merges them in warp order.  No atomics: every value has one fixed order.
+        float2* xch = reinterpret_cast<float2*>(smem + kStages * (S::A_STAGE + S::B_STAGE) + 256);  // [8 warps][kUN columns]
+        const int mw = warp - kMmaWarp0;
+        const int row0 = im.tile_n * kTileRows;
+        const float ninf = __uint_as_float(0xff800000u);
+        const bool ok0 = row0 + r0 < a.N, ok1 = row0 + r0 + 8 < a.N;  // rows past the ragged edge (TMA zero-filled) are masked
+#pragma unroll
+        for (int jj = 0; jj < kUN / 8; ++jj) {
+          if (8 * jj >= im.un) break;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * jj + c0 + e, m = im.m0 + col;
+            const float v0 = ok0 ? to_f32<T>(cvt_out<T>(acc[4 * jj + e])) : ninf;
+            const float v1 = ok1 ? to_f32<T>(cvt_out<T>(acc[4 * jj + 2 + e])) : ninf;
+            if (m < a.M) {
+              const long long tr = (long long)a.targets[m] - a.index_offset - row0;
+              if (tr == r0 && ok0) a.tgt[m] = v0;
+              if (tr == r0 + 8 && ok1) a.tgt[m] = v1;
+            }
+            float mx = fmaxf(v0, v1);
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 4));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 8));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 16));
+            float sm = mx == ninf ? 0.0f : expf(v0 - mx) + expf(v1 - mx);
+            sm += __shfl_xor_sync(0xffffffffu, sm, 4);
+            sm += __shfl_xor_sync(0xffffffffu, sm, 8);
+            sm += __shfl_xor_sync(0xffffffffu, sm, 16);
+            if (lane < 4) xch[mw * kUN + col] = make_float2(mx, sm);
+          }
+        }
+        HQQ_NAMED_BAR_SYNC(1, kMmaThreads);
+        const int col = threadIdx.x - kDequantThreads;
+        if (col < im.un && im.m0 + col < a.M) {
+          float mx = xch[col].x;  // warp 0 holds tile row 0 < N: mx ends finite
+#pragma unroll
+          for (int w = 1; w < kMmaThreads / 32; ++w) mx = fmaxf(mx, xch[w * kUN + col].x);
+          float sm = 0.0f;
+#pragma unroll
+          for (int w = 0; w < kMmaThreads / 32; ++w) { const float2 p = xch[w * kUN + col]; sm += p.y * expf(p.x - mx); }
+          a.part[(size_t)im.tile_n * a.M + im.m0 + col] = make_float2(mx, sm);
+        }
+        HQQ_NAMED_BAR_SYNC(1, kMmaThreads);  // the exchange area is free for the next tile
+        continue;
+      }
       // ---- epilogue: accumulators -> (bias) -> y, or the fp32 partial of this k-slice ----
       const int prow0 = im.tile_n * PR;
 #pragma unroll
@@ -564,6 +621,25 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
   }
 }
 
+// LSE second pass: per position, the vocabulary tiles' (max, sum) merged in tile order (include/hqq_b200.h states the numbers).
+// tgt[m] = -inf where the target is not in this shard; the epilogue has written the others.
+__global__ void __launch_bounds__(256) lse_merge_kernel(const float2* __restrict__ part, const int64_t* __restrict__ targets, float* __restrict__ lse,
+                                                        float* __restrict__ tgt, int M, int n_row, int N, long long index_offset) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  pdl_wait();  // launched as a programmatic dependent of the GEMM: reads only after that grid has completed
+  if (m >= M) return;
+  float mx = part[m].x;
+  for (int j = 1; j < n_row; ++j) mx = fmaxf(mx, part[(size_t)j * M + m].x);
+  float s = 0.0f;
+  for (int j = 0; j < n_row; ++j) {
+    const float2 p = part[(size_t)j * M + m];
+    s += p.y * expf(p.x - mx);
+  }
+  lse[m] = mx + logf(s);
+  const long long t = (long long)targets[m] - index_offset;
+  if (t < 0 || t >= N) tgt[m] = __uint_as_float(0xff800000u);
+}
+
 // ---- host side ------------------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -642,7 +718,7 @@ static size_t splitk_ws_bytes(const Sched& s) {
   return s.ksplit > 1 ? (size_t)s.ksplit * (size_t)s.n_row * s.n_tok * kUN * kTileRows * sizeof(float) : 0;
 }
 
-template <typename T, int NBITS, int GS>
+template <typename T, int NBITS, int GS, bool LSE = false>
 static int launch(const void* x, Args& a, cudaStream_t st, const void* dense_W = nullptr, void* ws = nullptr, size_t ws_bytes = 0) {
   CUtensorMap xmap_full, xmap_half, amap;
   const CUtensorMapDataType dt = std::is_same<T, __half>::value ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -667,11 +743,18 @@ static int launch(const void* x, Args& a, cudaStream_t st, const void* dense_W =
     a.ws = reinterpret_cast<float*>(ws);
   }
   const int grid = a.sched.n_items < P ? a.sched.n_items : P;
-  rc = reserve_smem<linear_gemm_kernel<T, NBITS, GS>>(Smem::BYTES);
+  constexpr int smem = Smem::BYTES + (LSE ? Smem::XCH : 0);
+  rc = reserve_smem<linear_gemm_kernel<T, NBITS, GS, LSE>>(smem);
   if (rc) return rc;
-  rc = launch_pdl("hqq_b200_linear_fwd/wgmma", linear_gemm_kernel<T, NBITS, GS>, dim3((unsigned)grid), dim3(kThreads), Smem::BYTES, st, xmap_full,
-                  xmap_half, amap, a);
-  if (rc || a.sched.ksplit <= 1) return rc;
+  rc = launch_pdl(LSE ? "hqq_b200_lm_logprob/wgmma-lse" : "hqq_b200_linear_fwd/wgmma", linear_gemm_kernel<T, NBITS, GS, LSE>, dim3((unsigned)grid),
+                  dim3(kThreads), smem, st, xmap_full, xmap_half, amap, a);
+  if (rc) return rc;
+  if (LSE) {
+    const float2* part = a.part;
+    return launch_pdl("hqq_b200_lm_logprob/merge", lse_merge_kernel, dim3((unsigned)cdiv(a.M, 256)), dim3(256), 0, st, part, a.targets,
+                      reinterpret_cast<float*>(a.y), a.tgt, a.M, a.sched.n_row, a.N, a.index_offset);
+  }
+  if (a.sched.ksplit <= 1) return rc;
   const long long total = (long long)a.M * a.N;
   const bool vec = a.step % 4 == 0 && PR % 4 == 0 && aligned(a.y, 8);
   const dim3 rgrid((unsigned)cdiv(vec ? total / 4 : total, 256));
@@ -735,6 +818,27 @@ int linear_dense(const void* x, const void* W, const void* bias, void* y, int64_
   a.Gk = 0;
   if (dtype == HQQ_F16) return gemm::launch<__half, 16, 64>(x, a, st, W);
   return gemm::launch<__nv_bfloat16, 16, 64>(x, a, st, W);
+}
+
+size_t lm_logprob_ws_bytes(int64_t M, int64_t N) { return M > 0 && N > 0 ? (size_t)cdiv(N, gemm::kTileRows) * (size_t)M * sizeof(float2) : 0; }
+
+// lse / tgt of every position over the rows of an lm_head shard W [N, K]: the dense kernel with the LSE epilogue, then the tile merge
+int lm_logprob(const void* x, const void* W, const int64_t* targets, float* lse, float* tgt, void* ws, int64_t M, int64_t N, int64_t K,
+               int64_t index_offset, int dtype, cudaStream_t st) {
+  HQQ_REQUIRE(x && W && targets && lse && tgt && ws, HQQ_E_INVALID, "hqq_b200_lm_logprob: null pointer");
+  HQQ_REQUIRE(aligned(x, 16) && aligned(W, 16) && aligned(targets, 8) && aligned(lse, 4) && aligned(tgt, 4) && aligned(ws, 8), HQQ_E_INVALID,
+              "hqq_b200_lm_logprob: x and W must be 16-byte aligned, targets and workspace 8-byte, lse and tgt 4-byte");
+  HQQ_REQUIRE(M >= 1 && N >= 1 && K >= 8 && K % 8 == 0 && M <= (1 << 28) && N <= (1 << 28) && K <= (1 << 28), HQQ_E_INVALID,
+              "hqq_b200_lm_logprob: bad shape M=%lld N=%lld K=%lld (K a multiple of 8)", (long long)M, (long long)N, (long long)K);
+  HQQ_REQUIRE(dtype == HQQ_F16 || dtype == HQQ_BF16, HQQ_E_UNSUPPORTED, "hqq_b200_lm_logprob: dtype %d: fp16 / bf16 only", dtype);
+  gemm::Args a;
+  a.Wq = nullptr; a.scale = nullptr; a.zero = nullptr; a.bias = nullptr; a.y = lse;
+  a.M = (int)M; a.N = (int)N; a.K = (int)K;
+  a.step = (int)N;
+  a.Gk = 0;
+  a.targets = targets; a.index_offset = (long long)index_offset; a.tgt = tgt; a.part = reinterpret_cast<float2*>(ws);
+  if (dtype == HQQ_F16) return gemm::launch<__half, 16, 64, true>(x, a, st, W);
+  return gemm::launch<__nv_bfloat16, 16, 64, true>(x, a, st, W);
 }
 
 int linear_gemm(const void* x, const void* Wq, const void* scale, const void* zero, const void* bias, void* y, int64_t M, int64_t N,

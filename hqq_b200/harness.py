@@ -53,6 +53,7 @@ LLAMA31_8B = LlamaShape(rope_scaling={"rope_type": "llama3", "factor": 8.0, "low
 # Above this many cache positions the fused steps run the split-KV attention kernel (csrc/decode_glue.cu): the one-CTA-per-head
 # kernel keeps a score per position in shared memory and stops here.  At or below it they run that kernel as before.
 SINGLE_ATTN_MAX_LEN = 8192
+LOGPROB_ROWS = 4096  # rows per hqq_b200_lm_logprob call in score(): 33 MB of tile partials at vocabulary 128256
 
 
 def rope_inv_freq(shape: LlamaShape, device) -> torch.Tensor:
@@ -964,8 +965,63 @@ class DecodeModel:
         pair.  fused=False quantises into the cache and attends over its dequantisation.
 
         ragged: see _prefill_ragged (`tokens` is a list of per-slot prompts or None)."""
+        return self._prefill(tokens, start, chunk)
+
+    def score(self, prompts, start: int = 0, chunk: int = 2048):
+        """prefill() with the same arguments, checks and resulting state (caches, pos, tok, last_logits, the sample counter, pages,
+        hist), which also returns the prompt's log-probabilities: entry i is log p(prompt[i + 1] | prompt[0 .. i] and the cache rows
+        before the prompt), fp32; the first prompt token is not scored.  Lock-step: a [batch, T - 1] tensor; ragged: one 1-D tensor
+        of T_b - 1 entries per slot (None for slots without a prompt).
+
+        After the last block of each chunk every row goes through the final norm (hqq_b200_glue_add_rmsnorm_rows on a copy of the
+        residual stream) and the LSE head (hqq_b200_lm_logprob, blocks of at most LOGPROB_ROWS rows; the target of a row is the
+        slot's next prompt token, -1 at its last position): log p = tgt - lse, and the logits never reach memory.  The last
+        positions also go through prefill's own head, unchanged.  With tensor parallelism each rank's (lse, tgt) meet in one
+        all_gather_into_tensor and are merged in rank order, so every rank returns the same values.  fused=False: torch.matmul
+        logits, F.log_softmax in fp32 and a gather (the logits of all ranks gathered first) -- the reference."""
+        logp = {}
+        self._prefill(prompts, start, chunk, score=logp)
+        return logp["out"]
+
+    def _score_rows(self, h, delta, targets):
+        """log p(targets | rows) fp32 [R] for the residual stream h, delta [R, hidden] after the last block; h is not modified.
+        Rows whose target is -1 get an arbitrary value (the callers drop them)."""
+        s, R = self.shape, h.shape[0]
+        if not self.fused:
+            x = F.rms_norm(h + delta, (s.hidden,), self.final_norm, s.rms_eps)
+            logits = torch.matmul(x, self.lm_head.t())
+            if self.tp > 1:
+                g = torch.empty(self.tp, R, self.vocab_shard, dtype=logits.dtype, device=logits.device)
+                torch.distributed.all_gather_into_tensor(g, logits.contiguous(), group=self.pg)
+                logits = g.permute(1, 0, 2).reshape(R, -1)
+            lp = F.log_softmax(logits.float(), dim=-1)
+            return lp.gather(1, targets.clamp_min(0).view(-1, 1)).view(-1)
+        from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
+        lib, st, code = load(), stream_ptr(self.device), DTYPE_CODE[self.dtype]
+        hs, x = h.clone(), torch.empty_like(h)
+        check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(hs), ptr(delta), ptr(self.final_norm), ptr(x), R, s.hidden, s.rms_eps, code, st))
+        n = self.vocab_shard
+        lse = torch.empty(2, R, dtype=torch.float32, device=self.device)  # [lse; tgt]
+        rows = min(R, LOGPROB_ROWS)
+        ws = torch.empty(lib.hqq_b200_lm_logprob_workspace_bytes(rows, n), dtype=torch.uint8, device=self.device)
+        for r0 in range(0, R, rows):
+            m = min(rows, R - r0)
+            check(lib.hqq_b200_lm_logprob(ptr(x[r0:]), ptr(self.lm_head), ptr(targets[r0:]), ptr(lse[0, r0:]), ptr(lse[1, r0:]), ptr(ws), m, n,
+                                          s.hidden, self.rank * n, code, st))
+        if self.tp > 1:  # lse = M + log(sum_r exp(lse_r - M)) in rank order; tgt is finite on the one rank whose shard holds it
+            g = torch.empty(self.tp, 2, R, dtype=torch.float32, device=self.device)
+            torch.distributed.all_gather_into_tensor(g, lse, group=self.pg)
+            mx = g[:, 0].max(dim=0).values
+            acc = torch.zeros_like(mx)
+            for r in range(self.tp):
+                acc += torch.exp(g[r, 0] - mx)
+            lse = torch.stack([mx + torch.log(acc), g[:, 1].max(dim=0).values])
+        return lse[1] - lse[0]
+
+    def _prefill(self, tokens, start=0, chunk=2048, score=None):
+        """prefill(); score: a dict that receives the log-probabilities of score() under "out"."""
         if self.ragged:
-            return self._prefill_ragged(tokens, start, chunk)
+            return self._prefill_ragged(tokens, start, chunk, score)
         s, B = self.shape, self.batch
         tokens = torch.as_tensor(tokens, device=self.device)
         if tokens.dim() == 1 and B == 1:
@@ -981,10 +1037,16 @@ class DecodeModel:
         tokens = tokens.to(torch.long)
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         h_last = d_last = None
+        if score is not None:
+            score["out"] = torch.empty(B, T - 1, dtype=torch.float32, device=self.device)
+            nxt = torch.cat([tokens[:, 1:], torch.full((B, 1), -1, dtype=torch.long, device=self.device)], dim=1)  # row t's target
         with torch.no_grad():
             for c0 in range(0, T, chunk):
                 n = min(chunk, T - c0)
                 h, delta = (self._prefill_chunk_fused if self.fused else self._prefill_chunk_ref)(tokens[:, c0:c0 + n], start + c0, hd, hq, hkv)
+                if score is not None and min(n, T - 1 - c0) > 0:
+                    lp = self._score_rows(h, delta, nxt[:, c0:c0 + n].reshape(-1)).view(B, n)
+                    score["out"][:, c0:c0 + n] = lp[:, :min(n, T - 1 - c0)]
                 if c0 + n == T:
                     h_last, d_last = h.view(B, n, s.hidden)[:, -1].contiguous(), delta.view(B, n, s.hidden)[:, -1].contiguous()
             tok = self._prefill_head(h_last, d_last)
@@ -992,7 +1054,7 @@ class DecodeModel:
         self.pos.fill_((start + T) % self.cache_len)
         return self.tok.clone()
 
-    def _prefill_ragged(self, prompts, start=0, chunk=2048) -> torch.Tensor:
+    def _prefill_ragged(self, prompts, start=0, chunk=2048, score=None) -> torch.Tensor:
         """Prefill of a ragged batch: `prompts` holds `batch` entries, each a 1-D token tensor or None (that slot's pos, tok and
         caches stay as they are); a [batch, T] tensor stands for the equal-length list.  `start` is an int or one per slot.  Slot b
         takes in its prompt at positions start_b .. start_b + T_b - 1.  Each chunk takes up to `chunk` tokens from every slot that
@@ -1038,6 +1100,17 @@ class DecodeModel:
                 self.hist[b, starts[b]:starts[b] + toks[b].numel()] = toks[b].to(torch.int32)
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         last = {}
+        if score is not None:  # slot b's rows t0 .. t0 + n - 1 score entries t0 .. (the last position has no target)
+            out = score["out"] = [None if t is None else torch.empty(t.numel() - 1, dtype=torch.float32, device=self.device) for t in toks]
+            nxt = [None if t is None else torch.cat([t[1:], t.new_full((1,), -1)]) for t in toks]
+
+            def scored(h, delta, segs):  # segs: (slot, t0, n) in row order
+                lp = self._score_rows(h, delta, torch.cat([nxt[b][t0:t0 + n] for b, t0, n in segs]))
+                r = 0
+                for b, t0, n in segs:
+                    k = max(0, min(n, out[b].numel() - t0))
+                    out[b][t0:t0 + k] = lp[r:r + k]
+                    r += n
         with torch.no_grad():
             if not self.fused:
                 for b in slots:
@@ -1045,6 +1118,8 @@ class DecodeModel:
                     for c0 in range(0, T, chunk):
                         n = min(chunk, T - c0)
                         h, delta = self._prefill_chunk_ref(toks[b][c0:c0 + n].view(1, n), starts[b] + c0, hd, hq, hkv, slot=b)
+                        if score is not None:
+                            scored(h, delta, [(b, c0, n)])
                     last[b] = (h[-1], delta[-1])
             else:
                 done = [0] * B
@@ -1056,6 +1131,8 @@ class DecodeModel:
                         budget -= n_tok[b]
                     ids = torch.cat([toks[b][done[b]:done[b] + n_tok[b]] for b in slots if n_tok[b]])
                     h, delta = self._prefill_chunk_fused(ids.view(1, -1), 0, hd, hq, hkv, varlen=(pos0, n_tok))
+                    if score is not None:
+                        scored(h, delta, [(b, done[b], n_tok[b]) for b in slots if n_tok[b]])
                     r = 0
                     for b in range(B):
                         r += n_tok[b]

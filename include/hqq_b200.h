@@ -153,6 +153,22 @@ int hqq_b200_linear_fwd(const void* x, const void* W_q, const void* scale, const
 int hqq_b200_dense_gemm(const void* x, const void* W, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
                         int dtype, void* stream);
 
+/* Log-probabilities over an lm_head shard without materialising the logits (prompt scoring, perplexity).  x [M, K] and the shard
+ * W [N, K] (vocabulary rows index_offset .. index_offset + N - 1) of `dtype` (f16/bf16); targets int64 [M]: a vocabulary index or -1.
+ *   l[m][v] = T(sum_k x[m][k] * W[v][k])   -- fp32 accumulation, one rounding to T: what hqq_b200_dense_gemm stores (no bias)
+ *   per vocabulary tile j (rows 128 j .. 128 j + 127 that are < N) and position m, in fp32:
+ *     m_j = max_v l[m][v],  s_j = sum_v expf(l[m][v] - m_j)                      (the wgmma kernel's epilogue; logits never stored)
+ *   then over the tiles, in tile order:  M = max_j m_j,  S = sum_j s_j * expf(m_j - M),  lse[m] = M + logf(S)      (fp32)
+ *   tgt[m] = l[m][targets[m] - index_offset] when that row lies in the shard, else -inf                          (fp32)
+ * log p(target | x) = tgt - lse on one shard; shards merge their lse the same way (max, then sum of exp in rank order).  The
+ * value of a position depends on its x row alone: not on M, the other rows or the schedule.  No atomics.
+ * workspace: hqq_b200_lm_logprob_workspace_bytes(M, N) = ceil(N / 128) * M * 8 bytes (8-byte aligned) of tile partials; the
+ * caller bounds M per call (4096 rows at vocabulary 128256: 33 MB).  HQQ_E_INVALID for null or unaligned pointers (x, W 16 bytes;
+ * targets, workspace 8; lse, tgt 4) or K % 8 != 0; HQQ_E_UNSUPPORTED outside f16 / bf16.                                      */
+size_t hqq_b200_lm_logprob_workspace_bytes(int64_t M, int64_t N);
+int hqq_b200_lm_logprob(const void* x, const void* W, const int64_t* targets, float* lse, float* tgt, void* workspace, int64_t M,
+                        int64_t N, int64_t K, int64_t index_offset, int dtype, void* stream);
+
 /* Several HQQLinear layers that consume the SAME activation (q/k/v, gate/up) in one launch of the small-M kernel:
  * the 16-row tiles of all `count` (<= 4) matrices form one stream-K work list, so small matrices no longer pay a
  * launch each.  Arrays hold `count` device pointers / sizes; bias may be NULL or hold NULL entries; all matrices share
