@@ -87,6 +87,18 @@ SIGNATURES = {
     "hqq_b200_glue_rope_append_rows_kv8_devpos_paged": (c_int, [c_void_p] * 14 + [c_int] * 9 + [c_void_p]),
     "hqq_b200_glue_attn_verify_split_kv8": (c_int, [c_void_p] * 10 + [c_int] * 8 + [c_void_p]),
     "hqq_b200_glue_attn_verify_split_kv8_paged": (c_int, [c_void_p] * 11 + [c_int] * 9 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_kv4": (c_int, [c_void_p] * 14 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_kv4_seqpos": (c_int, [c_void_p] * 14 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_attn_decode_split_kv4_paged": (c_int, [c_void_p] * 15 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv4": (c_int, [c_void_p] * 14 + [c_int] * 9 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv4_varlen": (c_int, [c_void_p] * 16 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv4_paged": (c_int, [c_void_p] * 17 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_kv4_stage": (c_int, [c_void_p] * 10 + [c_int] * 6 + [c_void_p]),
+    "hqq_b200_glue_kv4_stage_paged": (c_int, [c_void_p] * 11 + [c_int] * 7 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv4_devpos": (c_int, [c_void_p] * 13 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_rope_append_rows_kv4_devpos_paged": (c_int, [c_void_p] * 14 + [c_int] * 9 + [c_void_p]),
+    "hqq_b200_glue_attn_verify_split_kv4": (c_int, [c_void_p] * 10 + [c_int] * 8 + [c_void_p]),
+    "hqq_b200_glue_attn_verify_split_kv4_paged": (c_int, [c_void_p] * 11 + [c_int] * 9 + [c_void_p]),
     "hqq_b200_glue_attn_verify_split": (c_int, [c_void_p] * 6 + [c_int] * 7 + [c_void_p]),
     "hqq_b200_glue_attn_verify_split_paged": (c_int, [c_void_p] * 7 + [c_int] * 8 + [c_void_p]),
     "hqq_b200_glue_ngram_draft": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),

@@ -640,8 +640,9 @@ __device__ __forceinline__ void split_merge(const float* wp, float* __restrict__
 //
 // kv8_quant4: a 128-element row held four per lane (lane l: elements 4 l .. 4 l + 3).  Group min / max over gs / 4 lanes, then
 // init_group (maxv 255, zero not rounded) and quant_level as quantize.cu does for an 8-bit layer without the solver.  Returns the
-// four levels (byte j: element 4 l + j) and the scale (1 / s) and zero of the lane's group rounded to T.
-template <typename T>
+// four levels (byte j: element 4 l + j) and the scale (1 / s) and zero of the lane's group rounded to T.  MAXV 15 is the 4-bit
+// cache's quantiser (levels in [0, 15], one per byte, unpacked).
+template <typename T, int MAXV = 255>
 __device__ __forceinline__ uint32_t kv8_quant4(const float (&x)[4], int gs, T& scale, T& zero) {
   float mn = fminf(fminf(x[0], x[1]), fminf(x[2], x[3])), mx = fmaxf(fmaxf(x[0], x[1]), fmaxf(x[2], x[3]));
 #pragma unroll
@@ -652,10 +653,10 @@ __device__ __forceinline__ uint32_t kv8_quant4(const float (&x)[4], int gs, T& s
     }
   }
   GroupState st;
-  init_group(mn, mx, 255, 0, st);
+  init_group(mn, mx, MAXV, 0, st);
   uint32_t q = 0;
 #pragma unroll
-  for (int j = 0; j < 4; ++j) q |= (uint32_t)quant_level(x[j], st.s, st.z, 255.0f) << (8 * j);
+  for (int j = 0; j < 4; ++j) q |= (uint32_t)quant_level(x[j], st.s, st.z, (float)MAXV) << (8 * j);
   scale = from_f32<T>(__frcp_rn(st.s));  // quantize.py:154 scale = 1.0 / scale, then the meta cast to T
   zero = from_f32<T>(st.z);
   return q;
@@ -962,6 +963,309 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
   split_merge<T>(wp, part, tickets, out, last, S, split, G, tid);
 }
 
+// 4-bit HQQ KV cache (DESIGN.md 3.5).  A cache row of one kv head is Quantizer.quantize(row, nbits=4, group_size=gs, axis=1,
+// optimize=False) with gs 32 or 64, packed as the reference's 4bit_u8 packing of that row: 64 bytes, byte d = q[d] << 4 | q[d + 64];
+// meta [128 / gs] T.  The attended row is T(T(q - z) * s), what oracle.dequantize gives.  16-byte chunk c of a row holds dims
+// 16 c .. 16 c + 15 (high nibbles) and 64 + 16 c .. (low nibbles), each half inside one group.
+//
+// kv4_pack: the levels of kv8_quant4<T, 15> (lane l: elements 4 l .. 4 l + 3, one per byte) -> the packed bytes 4 l .. 4 l + 3 of
+// the row in lanes 0..15 (lanes 16..31 hold elements 64 .. 127, whose levels are the low nibbles).  Every lane must call it.
+__device__ __forceinline__ uint32_t kv4_pack(uint32_t q) { return (q << 4) | __shfl_xor_sync(0xffffffffu, q, 16); }
+// kv4_unpack: packed bytes 4 l' .. 4 l' + 3 -> the levels (one per byte) of elements 4 l' .. (hi) or 64 + 4 l' .. (lo)
+__device__ __forceinline__ uint32_t kv4_unpack(uint32_t w, bool hi) { return (hi ? w >> 4 : w) & 0x0F0F0F0Fu; }
+
+// The levels in bits 0..3 and 16..19 of t (other bits ignored) -> T(T(q - z) * s) each, packed as a T2 (bits 0..3 in the low half):
+// T(q) exactly, then one rounded T subtraction and one rounded T product per element, as kv8_deq2.  fp16: half2(1024 + q) by bit
+// pattern (0x640q), minus 1024 exactly; bf16: bf16(128 + q) by bit pattern (0x430q), minus 128 exactly.
+template <typename T>
+__device__ __forceinline__ uint32_t kv4_deq2(uint32_t t, typename Pair<T>::type z, typename Pair<T>::type s) {
+  using T2 = typename Pair<T>::type;
+  const uint32_t m = std::is_same<T, __half>::value ? 0x64006400u : 0x43004300u;
+  const uint32_t h = (t & 0x000F000Fu) | m;
+  const T2 q = __hsub2(*reinterpret_cast<const T2*>(&h), *reinterpret_cast<const T2*>(&m));
+  const T2 r = __hmul2(__hsub2(q, z), s);
+  return *reinterpret_cast<const uint32_t*>(&r);
+}
+
+// Split-KV decode attention over a 4-bit cache: rope_attn_decode_split_kv8_kernel's grid, chunks, ticket, merge, RoPE and
+// pre-wait staging, with a 6-stage ring of 2560-byte stages (K and V levels [16][64], 16-byte chunks swizzled so that the 16 rows
+// of a tile fill 8 lines of 128 bytes with line l = r / 2 holding chunk (4 (r & 1) + c) ^ 2 (l & 3) -- conflict-free for the K reads
+// (16 bytes a lane) and the V reads (8 bytes a lane) below -- then k scale | k zero | v scale | v zero [16][<= 4]).  The head dim is
+// permuted the same way for both operands of a product: lane (g, qd) takes K chunk qd of positions g, g + 8 (k slot
+// 2 qd + {0, 1, 8, 9} of step kk is dim 16 qd + 4 kk + {0..3} for kk < 4, the high nibbles, and 64 + 16 qd + 4 (kk - 4) + {0..3}
+// for kk >= 4, the low nibbles), and V bytes 8 g .. 8 g + 7 of positions 2 qd + {0, 1, 8, 9} (O^T row g of step mt is dim 8 g + mt,
+// the high nibble of byte 8 g + mt; row g + 8 is dim 64 + 8 g + mt, its low nibble).  Each lane's K half-row and V half-row span
+// two groups, one per nibble.  Row pos is this launch's quantisation of the fresh k / v in every CTA that holds it; split 0 writes
+// it to the cache.
+constexpr int kKv4Stages = 6;
+constexpr int kKv4LvlBytes = kSplitTile * kHd / 2;                                // one K or V level tile, 1 KB
+constexpr int kKv4MetaBytes = kSplitTile * 4 * 2;                                 // one meta array of a tile: [16][<= 4] T
+constexpr int kKv4StageBytes = 2 * kKv4LvlBytes + 4 * kKv4MetaBytes;
+constexpr int kKv4RingBytes = kSplitWarps * kKv4Stages * kKv4StageBytes;           // 120 KB
+// + rotated q [8][128] T, fresh k, v [128] T, their packed levels [2][64] and meta [4][4] T, the last-CTA flag
+constexpr int kKv4SmemBytes = kKv4RingBytes + (kSplitMaxGroup + 2) * kHd * 2 + kHd + 32 + 16;
+static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kKv4RingBytes, "the warp partials reuse the ring");
+
+__device__ __forceinline__ int swz4(int r, int c) { return (r >> 1) * 128 + (((((r & 1) << 2) | c) ^ (((r >> 1) & 3) << 1)) << 4); }
+
+// grid = (S, n_kv, batch), block = 256.  As rope_attn_decode_split_kv8_kernel, with packed levels [batch, n_kv, L, 64] uint8 and meta
+// [batch, n_kv, L, 128 / gs] T (paged: [pages, n_kv, 64, 64] and [pages, n_kv, 64, 128 / gs]), gs 32 or 64.
+template <typename T, bool SEQPOS = false, bool PAGED = false>
+__global__ void __launch_bounds__(kSplitThreads, 1)
+    rope_attn_decode_split_kv4_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
+                                      const T* __restrict__ sin_t, uint8_t* __restrict__ k_q, T* __restrict__ k_s, T* __restrict__ k_z,
+                                      uint8_t* __restrict__ v_q, T* __restrict__ v_s, T* __restrict__ v_z, const long long* __restrict__ pos_p,
+                                      T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
+                                      int gs, float scale_log2, const PageArg<PAGED> pg) {
+  extern __shared__ __align__(16) char smem[];
+  constexpr int NW = kSplitWarps, ST = kKv4Stages, LB = kHd / 2;
+  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
+  const int G = n_q / n_kv, ng = kHd / gs;
+  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
+  const int* tab = nullptr;
+  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
+  {
+    const long long kv = (long long)b * n_kv + kvh;
+    if constexpr (!PAGED) {
+      k_q += kv * L * LB; v_q += kv * L * LB;
+      k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+    }
+    k_in += kv * kHd; v_in += kv * kHd;
+    q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
+    part += kv * S * G * kPartFloats;
+    tickets += kv;
+  }
+  char* ring = smem + warp * ST * kKv4StageBytes;
+  T* qs = reinterpret_cast<T*>(smem + kKv4RingBytes);  // rotated q [8][128]
+  T* kf = qs + kSplitMaxGroup * kHd;                   // rotated k and v of position pos
+  T* vf = kf + kHd;
+  uint8_t* fq = reinterpret_cast<uint8_t*>(vf + kHd);  // their packed levels: k [64], v [64]
+  T* fm = reinterpret_cast<T*>(fq + 2 * LB);           // their meta: k scale, k zero, v scale, v zero [4] each
+  int* last = reinterpret_cast<int*>(fm + 16);
+
+  // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
+  const int pos = (int)pos_p[SEQPOS ? b : 0], n_pos = pos + 1;
+  const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
+  const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
+  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
+  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;
+  pdl_launch_dependents();
+
+  // Stage local tile i as the 8-bit kernel does: rows < pos from the cache, row pos from this launch's quantisation once `fresh`,
+  // rows past pos zero (levels and meta: they dequantise to 0).  A meta chunk of 16 bytes spans 8 / ng rows; one that reaches row pos
+  // (or sits on a misaligned address) is staged row by row.
+  auto issue = [&](int i, bool fresh) {
+    if (i < my_tiles) {
+      const int t0 = c0 + (warp + i * NW) * kSplitTile;
+      char* st = ring + (i % ST) * kKv4StageBytes;
+      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
+      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
+#pragma unroll
+      for (int j = lane; j < 2 * kSplitTile * 4; j += 32) {
+        const int isv = j >> 6, r = (j >> 2) & 15, c = j & 3, p = t0 + r;
+        char* dst = st + isv * kKv4LvlBytes + swz4(r, c);
+        if (p < pos) {
+          split_cp16(dst, (isv ? v_q : k_q) + (rt + p) * LB + c * 16);
+        } else if (p > pos || fresh) {
+          uint4 val;
+          val.x = val.y = val.z = val.w = 0u;
+          if (p == pos) val = *reinterpret_cast<const uint4*>(fq + isv * LB + c * 16);
+          *reinterpret_cast<uint4*>(dst) = val;
+        }
+      }
+      if (lane < 8 * ng) {  // 4 arrays x 2 ng chunks
+        const int a = lane / (2 * ng), j = lane % (2 * ng), rows = 8 / ng, r0 = j * rows;
+        const T* src = (a == 0 ? k_s : a == 1 ? k_z : a == 2 ? v_s : v_z) + (rt + (t0 + r0)) * ng;
+        char* dst = st + 2 * kKv4LvlBytes + a * kKv4MetaBytes + j * 16;
+        if (t0 + r0 + rows <= pos && ((uintptr_t)src & 15) == 0) {
+          split_cp16(dst, src);
+        } else {
+          for (int e = 0; e < 8; ++e) {
+            const int p = t0 + r0 + e / ng;
+            if (p < pos) reinterpret_cast<T*>(dst)[e] = src[e];
+            else if (p > pos) reinterpret_cast<T*>(dst)[e] = from_f32<T>(0.f);
+            else if (fresh) reinterpret_cast<T*>(dst)[e] = fm[4 * a + e % ng];
+          }
+        }
+      }
+    }
+    split_commit();  // always (possibly empty): every iteration waits on the same group count
+  };
+#pragma unroll
+  for (int i = 0; i < ST - 1; ++i) issue(i, false);
+  pdl_wait();
+
+  // RoPE exactly as rope_attn_decode_kernel: x*cos + rotate_half(x)*sin, each product and the sum rounded to T
+  for (int i = tid; i < (G + 1) * kHd; i += kSplitThreads) {
+    const int h = i >> 7, d = i & (kHd - 1), half = kHd / 2;
+    const float c = to_f32<T>(cos_t[(long long)pos * kHd + d]), s = to_f32<T>(sin_t[(long long)pos * kHd + d]);
+    const T* x = h < G ? q_in + h * kHd : k_in;
+    const float xv = to_f32<T>(x[d]);
+    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
+    const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
+    if (h < G) {
+      qs[h * kHd + d] = r;
+    } else {
+      kf[d] = r;
+      vf[d] = v_in[d];
+    }
+  }
+  __syncthreads();
+  if (warp < 2) {  // warp 0 quantises the rotated k row, warp 1 the v row; split 0 writes them to the cache
+    const T* src = warp ? vf : kf;
+    float x[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) x[j] = to_f32<T>(src[4 * lane + j]);
+    T sc, ze;
+    const uint32_t q = kv4_pack(kv8_quant4<T, 15>(x, gs, sc, ze));
+    if (lane < 16) *reinterpret_cast<uint32_t*>(fq + warp * LB + 4 * lane) = q;
+    const int grp = 4 * lane / gs;
+    if ((4 * lane) % gs == 0) { fm[8 * warp + grp] = sc; fm[8 * warp + 4 + grp] = ze; }
+    if (split == 0) {
+      long long pr = pos;
+      if constexpr (PAGED) pr = page_row(tab, n_kv, kvh, pos);
+      if (lane < 16) *reinterpret_cast<uint32_t*>((warp ? v_q : k_q) + pr * LB + 4 * lane) = q;
+      if ((4 * lane) % gs == 0) {
+        (warp ? v_s : k_s)[pr * ng + grp] = sc;
+        (warp ? v_z : k_z)[pr * ng + grp] = ze;
+      }
+    }
+  }
+  __syncthreads();
+  if (pos >= c0 && pos < c1) {  // row pos in a tile staged before the wait: its owner fills it in now
+    const int ti = (pos - c0) / kSplitTile, i = ti / NW;
+    if (ti % NW == warp && i < ST - 1) {
+      const int r = pos - (c0 + ti * kSplitTile);
+      char* st = ring + (i % ST) * kKv4StageBytes;
+      if (lane < 8) {
+        const int isv = lane >> 2, c = lane & 3;
+        *reinterpret_cast<uint4*>(st + isv * kKv4LvlBytes + swz4(r, c)) = *reinterpret_cast<const uint4*>(fq + isv * LB + c * 16);
+      } else if (lane >= 16 && lane < 16 + 4 * ng) {
+        const int a = (lane - 16) / ng, e = (lane - 16) % ng;
+        reinterpret_cast<T*>(st + 2 * kKv4LvlBytes + a * kKv4MetaBytes)[r * ng + e] = fm[4 * a + e];
+      }
+    }
+  }
+  // Q^T fragments in the permuted dims: k slots 2 qd + {0, 1} / + {8, 9} of step kk are dims dk + {0, 1} / + {2, 3}
+  uint32_t qb[8][2];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+    const T* qr = qs + g * kHd + (kk < 4 ? 16 * qd + 4 * kk : 64 + 16 * qd + 4 * (kk - 4));
+    qb[kk][0] = g < G ? *reinterpret_cast<const uint32_t*>(qr) : 0u;
+    qb[kk][1] = g < G ? *reinterpret_cast<const uint32_t*>(qr + 2) : 0u;
+  }
+
+  float o[8][4];
+#pragma unroll
+  for (int mt = 0; mt < 8; ++mt) o[mt][0] = o[mt][1] = o[mt][2] = o[mt][3] = 0.f;
+  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+  const int gkh = 16 * qd / gs, gkl = (64 + 16 * qd) / gs;  // the groups of the lane's K dims (high, low nibbles)
+  const int gvh = 8 * g / gs, gvl = (64 + 8 * g) / gs;      // and of its V dims
+  for (int i = 0; i < my_tiles; ++i) {
+    __syncwarp();  // every lane is done with the slot the next issue overwrites
+    issue(i + ST - 1, true);
+    split_wait<ST - 1>();
+    __syncwarp();  // this tile's copies and plain stores of every lane are visible to the warp
+    const char* st = ring + (i % ST) * kKv4StageBytes;
+    const T* ms = reinterpret_cast<const T*>(st + 2 * kKv4LvlBytes);
+    constexpr int MA = kKv4MetaBytes / 2;  // T elements per meta array
+    float s[4] = {0.f, 0.f, 0.f, 0.f};
+    {
+      const uint4 ka = *reinterpret_cast<const uint4*>(st + swz4(g, qd)), kb = *reinterpret_cast<const uint4*>(st + swz4(g + 8, qd));
+      typename Pair<T>::type sah, sal, sbh, sbl, zah, zal, zbh, zbl;  // rows g (a) and g + 8 (b), high and low nibbles
+      sah.x = sah.y = ms[g * ng + gkh]; sal.x = sal.y = ms[g * ng + gkl];
+      sbh.x = sbh.y = ms[(g + 8) * ng + gkh]; sbl.x = sbl.y = ms[(g + 8) * ng + gkl];
+      zah.x = zah.y = ms[MA + g * ng + gkh]; zal.x = zal.y = ms[MA + g * ng + gkl];
+      zbh.x = zbh.y = ms[MA + (g + 8) * ng + gkh]; zbl.x = zbl.y = ms[MA + (g + 8) * ng + gkl];
+      const uint32_t wa[4] = {ka.x, ka.y, ka.z, ka.w}, wb[4] = {kb.x, kb.y, kb.z, kb.w};
+#pragma unroll
+      for (int w = 0; w < 4; ++w) {
+        // bytes 4 w, 4 w + 1 (dims +0, +1) and 4 w + 2, 4 w + 3 (dims +2, +3) of each row, one byte per 16-bit half
+        const uint32_t a01 = prmt(wa[w], 0u, 0x4140u), a23 = prmt(wa[w], 0u, 0x4342u);
+        const uint32_t b01 = prmt(wb[w], 0u, 0x4140u), b23 = prmt(wb[w], 0u, 0x4342u);
+        uint32_t a[4];
+        a[0] = kv4_deq2<T>(a01 >> 4, zah, sah); a[1] = kv4_deq2<T>(b01 >> 4, zbh, sbh);
+        a[2] = kv4_deq2<T>(a23 >> 4, zah, sah); a[3] = kv4_deq2<T>(b23 >> 4, zbh, sbh);
+        mma16816<T>(s, a, qb[w][0], qb[w][1]);
+        a[0] = kv4_deq2<T>(a01, zal, sal); a[1] = kv4_deq2<T>(b01, zbl, sbl);
+        a[2] = kv4_deq2<T>(a23, zal, sal); a[3] = kv4_deq2<T>(b23, zbl, sbl);
+        mma16816<T>(s, a, qb[w + 4][0], qb[w + 4][1]);
+      }
+    }
+    const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
+    const float x0 = p0 < c1 ? s[0] * scale_log2 : -INFINITY, x1 = p0 < c1 ? s[1] * scale_log2 : -INFINITY;
+    const float x2 = p0 + 8 < c1 ? s[2] * scale_log2 : -INFINITY, x3 = p0 + 8 < c1 ? s[3] * scale_log2 : -INFINITY;
+    float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
+#pragma unroll
+    for (int off = 4; off < 32; off <<= 1) {
+      t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
+      t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
+    }
+    const float n0 = fmaxf(m0, t0), n1 = fmaxf(m1, t1);  // finite: every tile holds position c0 + 16 j < c1
+    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
+    m0 = n0; m1 = n1;
+    const T p00 = from_f32<T>(exp2f(x0 - n0)), p01 = from_f32<T>(exp2f(x1 - n1));
+    const T p10 = from_f32<T>(exp2f(x2 - n0)), p11 = from_f32<T>(exp2f(x3 - n1));
+    l0 = l0 * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
+    l1 = l1 * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) { o[mt][0] *= a0; o[mt][1] *= a1; o[mt][2] *= a0; o[mt][3] *= a1; }
+    // P^T fragment (k = position, n = head g), as in rope_attn_decode_split_kernel
+    const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
+    const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
+    const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
+    const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
+    const uint32_t b0 = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
+    const uint32_t b1 = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
+    {
+      // V^T: positions r = 2 qd + {0, 1, 8, 9}, bytes 8 g .. 8 g + 7 (half of chunk g / 2)
+      const char* vt = st + kKv4LvlBytes;
+      const int r0 = 2 * qd, cb = 8 * (g & 1);
+      const uint2 v0 = *reinterpret_cast<const uint2*>(vt + swz4(r0, g >> 1) + cb), v1 = *reinterpret_cast<const uint2*>(vt + swz4(r0 + 1, g >> 1) + cb);
+      const uint2 v8 = *reinterpret_cast<const uint2*>(vt + swz4(r0 + 8, g >> 1) + cb), v9 = *reinterpret_cast<const uint2*>(vt + swz4(r0 + 9, g >> 1) + cb);
+      const T* vs = ms + 2 * MA;
+      const T* vz = ms + 3 * MA;
+      typename Pair<T>::type s01h, s01l, s89h, s89l, z01h, z01l, z89h, z89l;  // positions r0, r0 + 1 / r0 + 8, r0 + 9; high / low nibbles
+      s01h.x = vs[r0 * ng + gvh]; s01h.y = vs[(r0 + 1) * ng + gvh]; s01l.x = vs[r0 * ng + gvl]; s01l.y = vs[(r0 + 1) * ng + gvl];
+      s89h.x = vs[(r0 + 8) * ng + gvh]; s89h.y = vs[(r0 + 9) * ng + gvh]; s89l.x = vs[(r0 + 8) * ng + gvl]; s89l.y = vs[(r0 + 9) * ng + gvl];
+      z01h.x = vz[r0 * ng + gvh]; z01h.y = vz[(r0 + 1) * ng + gvh]; z01l.x = vz[r0 * ng + gvl]; z01l.y = vz[(r0 + 1) * ng + gvl];
+      z89h.x = vz[(r0 + 8) * ng + gvh]; z89h.y = vz[(r0 + 9) * ng + gvh]; z89l.x = vz[(r0 + 8) * ng + gvl]; z89l.y = vz[(r0 + 9) * ng + gvl];
+      const uint32_t w0[2] = {v0.x, v0.y}, w1[2] = {v1.x, v1.y}, w8[2] = {v8.x, v8.y}, w9[2] = {v9.x, v9.y};
+#pragma unroll
+      for (int mt = 0; mt < 8; ++mt) {
+        // byte mt of each position: the two positions of a pair side by side (bits 0..7 and 16..23)
+        const uint32_t sel = (mt & 3) | ((4 + (mt & 3)) << 8);
+        const uint32_t t01 = prmt(w0[mt >> 2], w1[mt >> 2], sel), t89 = prmt(w8[mt >> 2], w9[mt >> 2], sel);
+        uint32_t a[4];
+        a[0] = kv4_deq2<T>(t01 >> 4, z01h, s01h); a[1] = kv4_deq2<T>(t01, z01l, s01l);
+        a[2] = kv4_deq2<T>(t89 >> 4, z89h, s89h); a[3] = kv4_deq2<T>(t89, z89l, s89l);
+        mma16816<T>(o[mt], a, b0, b1);
+      }
+    }
+  }
+  split_wait<0>();
+#pragma unroll
+  for (int off = 4; off < 32; off <<= 1) {
+    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+  }
+  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][8][m, l, o[128]]
+  float* wp = reinterpret_cast<float*>(smem);
+  {
+    float* w0 = wp + (warp * kSplitMaxGroup + 2 * qd) * kPartFloats;
+    float* w1 = w0 + kPartFloats;
+    if (g == 0) { w0[0] = m0; w0[1] = l0; w1[0] = m1; w1[1] = l1; }
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) {  // O^T rows g, g + 8 of step mt are dims 8 g + mt, 64 + 8 g + mt
+      w0[2 + 8 * g + mt] = o[mt][0]; w1[2 + 8 * g + mt] = o[mt][1];
+      w0[2 + 64 + 8 * g + mt] = o[mt][2]; w1[2 + 64 + 8 * g + mt] = o[mt][3];
+    }
+  }
+  __syncthreads();
+  split_merge<T>(wp, part, tickets, out, last, S, split, G, tid);
+}
+
 int split_count(int n_kv, int cache_len) {
   const int by_sm = sm_count() / n_kv;
   const int by_len = (int)cdiv(cache_len, kSplitTile);
@@ -982,7 +1286,8 @@ int split_count(int n_kv, int cache_len) {
 // part [batch, n_kv, n_cg, S, 8 kVerTiles, 2 + 128] floats, tickets [batch, n_kv, n_cg] uint32, zero between launches.
 // KV8: the caches hold HQQ 8-bit levels (uint8, same layout) with meta [.., 128 / gs] T; each staged 16-byte chunk is the
 // dequantisation T(T(q - z) * s) of 8 levels (kv8_deq2, what hqq_b200_dequantize gives), loaded and stored synchronously instead of
-// through cp.async; the tile layout, the MMAs and everything after them are those of the 16-bit cache.
+// through cp.async; the tile layout, the MMAs and everything after them are those of the 16-bit cache.  KV8 with BITS 4: the 4-bit
+// cache (packed levels [.., 64], gs 32 or 64); chunk c's 8 levels are the high (c < 8) or low nibbles of bytes 8 (c % 8) .. + 7.
 constexpr int kVerTiles = 2;                     // n-tiles per CTA (no spills at 2: DESIGN.md 3.5)
 constexpr int kVerCols = 8 * kVerTiles;          // columns per CTA
 constexpr int kVerMaxCols = 64;                  // T G
@@ -993,7 +1298,7 @@ struct NoKv8 {};
 template <typename T, bool KV8> using Kv8Arg = typename std::conditional<KV8, Kv8Meta<T>, NoKv8>::type;
 template <typename T, bool KV8> using CacheT = typename std::conditional<KV8, uint8_t, T>::type;
 
-template <typename T, bool PAGED = false, bool KV8 = false>
+template <typename T, bool PAGED = false, bool KV8 = false, int BITS = 8>
 __global__ void __launch_bounds__(kSplitThreads, 1)
     attn_verify_split_kernel(const T* __restrict__ q, const CacheT<T, KV8>* __restrict__ k_cache, const CacheT<T, KV8>* __restrict__ v_cache,
                              const long long* __restrict__ pos_p, T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q,
@@ -1003,12 +1308,13 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
   const int G = n_q / n_kv, C = TQ * G, n_cg = (C + NC - 1) / NC;
   const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y / n_cg, cg = (int)blockIdx.y % n_cg, b = (int)blockIdx.z;
   const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  constexpr int RW = KV8 ? kHd * BITS / 8 : kHd;  // cache elements a row
   const int* tab = nullptr;
   if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
   {
     const long long kv = (long long)b * n_kv + kvh;
     if constexpr (!PAGED) {
-      k_cache += kv * L * kHd; v_cache += kv * L * kHd;
+      k_cache += kv * L * RW; v_cache += kv * L * RW;
       if constexpr (KV8) {
         const int ng = kHd / m8.gs;
         m8.k_s += kv * L * ng; m8.k_z += kv * L * ng; m8.v_s += kv * L * ng; m8.v_z += kv * L * ng;
@@ -1031,7 +1337,14 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
   // 16-byte chunk c of cache row `row` (K or V) into dst: cp.async, or (KV8) 8 levels dequantised with their group's meta
   auto stage16 = [&](char* dst, int isv, long long row, int c, bool async) {
     if constexpr (KV8) {
-      const uint2 w = *reinterpret_cast<const uint2*>((isv ? v_cache : k_cache) + row * kHd + c * 8);
+      uint2 w;
+      if constexpr (BITS == 8) {
+        w = *reinterpret_cast<const uint2*>((isv ? v_cache : k_cache) + row * kHd + c * 8);
+      } else {
+        const uint2 p = *reinterpret_cast<const uint2*>((isv ? v_cache : k_cache) + row * RW + (c & 7) * 8);
+        w.x = kv4_unpack(p.x, c < 8);
+        w.y = kv4_unpack(p.y, c < 8);
+      }
       const long long mi = row * (kHd / m8.gs) + (c * 8) / m8.gs;
       typename Pair<T>::type s2, z2;
       s2.x = s2.y = (isv ? m8.v_s : m8.k_s)[mi];
@@ -1405,8 +1718,9 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
 // Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.  VARLEN as
 // rope_append_rows_kernel.  PAGED as there: levels and meta in the page pools, the staging pair stays [batch, n_kv, L, 128].
 // DEVPOS as rope_append_rows_kernel (positions from the device, rows past the cache end skipped); it writes no staging rows (k_st /
-// v_st unused): the verify attention dequantises the cache itself.
-template <typename T, bool VARLEN = false, bool PAGED = false, bool DEVPOS = false>
+// v_st unused): the verify attention dequantises the cache itself.  BITS 4: the 4-bit cache (rope_attn_decode_split_kv4_kernel's
+// quantisation and packing, levels [.., 64]).
+template <typename T, bool VARLEN = false, bool PAGED = false, bool DEVPOS = false, int BITS = 8>
 __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
                                                                    const T* __restrict__ cos_t, const T* __restrict__ sin_t, uint8_t* __restrict__ k_q,
                                                                    T* __restrict__ k_s, T* __restrict__ k_z, uint8_t* __restrict__ v_q,
@@ -1415,6 +1729,7 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
                                                                    const RowsArg<VARLEN, DEVPOS> vl, const PageArg<PAGED> pg) {
   static_assert(VARLEN || DEVPOS || !PAGED, "a paged cache needs per-slot positions");
   static_assert(!(VARLEN && DEVPOS), "one row layout");
+  constexpr int LB = kHd * BITS / 8;  // level bytes a row
   const int t = (int)blockIdx.x, b = (int)blockIdx.y, ng = kHd / gs;
   long long row = (long long)b * n_tok + t;
   if constexpr (VARLEN) {
@@ -1432,7 +1747,7 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
     q += row * n_q * kHd; q_out += row * n_q * kHd;
     k += row * n_kv * kHd; v += row * n_kv * kHd;
     if constexpr (!PAGED) {
-      k_q += kv * L * kHd; v_q += kv * L * kHd;
+      k_q += kv * L * LB; v_q += kv * L * LB;
       k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
     }
     if constexpr (!DEVPOS) { k_st += kv * L * kHd; v_st += kv * L * kHd; }
@@ -1468,11 +1783,16 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
       }
     }
     T sc, ze;
-    const uint32_t lv = kv8_quant4<T>(x, gs, sc, ze);
+    const uint32_t lv = kv8_quant4<T, (1 << BITS) - 1>(x, gs, sc, ze);
     const long long row = (long long)kvh * L + p;
     long long crow = row;
     if constexpr (PAGED) crow = c0 + (long long)kvh * kPage;
-    *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + crow * kHd + 4 * lane) = lv;
+    if constexpr (BITS == 8) {
+      *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + crow * kHd + 4 * lane) = lv;
+    } else {
+      const uint32_t pk = kv4_pack(lv);
+      if (lane < 16) *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + crow * LB + 4 * lane) = pk;
+    }
     if ((4 * lane) % gs == 0) {
       (isv ? v_s : k_s)[crow * ng + 4 * lane / gs] = sc;
       (isv ? v_z : k_z)[crow * ng + 4 * lane / gs] = ze;
@@ -1490,22 +1810,34 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
 // Prefill into a paged 8-bit cache: staging rows [0, pos0[b]) of every slot with n_tok[b] > 0, dequantised from the page pools through
 // the table with the rows kernel's arithmetic (kv8_deq2: T(T(q - z) * s), what hqq_b200_dequantize gives).  grid = (max pos0, batch),
 // block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position, four elements per lane.  The table is read before the
-// wait, the pools after it.
-template <typename T>
+// wait, the pools after it.  BITS 4: the 4-bit cache (lane l unpacks the high nibbles of bytes 4 l .. 4 l + 3, lane 16 + l their
+// low nibbles).  PAGED false (BITS 4 only): the contiguous caches [batch, n_kv, L, .], pg unused.
+template <typename T, int BITS = 8, bool PAGED = true>
 __global__ void __launch_bounds__(256) kv8_stage_paged_kernel(const uint8_t* __restrict__ k_q, const T* __restrict__ k_s, const T* __restrict__ k_z,
                                                               const uint8_t* __restrict__ v_q, const T* __restrict__ v_s, const T* __restrict__ v_z,
                                                               T* __restrict__ k_st, T* __restrict__ v_st, int n_kv, int L, int gs, const VarlenRows vl,
-                                                              const PageTable pg) {
+                                                              const PageArg<PAGED> pg) {
+  constexpr int LB = kHd * BITS / 8;  // level bytes a row
   const int p = (int)blockIdx.x, b = (int)blockIdx.y, ng = kHd / gs;
   if (vl.n_tok[b] == 0 || p >= vl.pos0[b]) return;  // slot outside the chunk, or a row the rows kernel writes
-  const long long c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
+  long long c0;  // cache row of position p of kv head 0; kv head h at c0 + h * rs
+  long long rs;
+  if constexpr (PAGED) {
+    c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
+    rs = kPage;
+  } else {
+    c0 = (long long)b * n_kv * L + p;
+    rs = L;
+  }
   pdl_launch_dependents();
   pdl_wait();
   const int warp = (int)threadIdx.x >> 5, lane = (int)threadIdx.x & 31;
   for (int r = warp; r < 2 * n_kv; r += (int)blockDim.x >> 5) {
     const int kvh = r >> 1, isv = r & 1, grp = 4 * lane / gs;
-    const long long crow = c0 + (long long)kvh * kPage;
-    const uint32_t lv = *reinterpret_cast<const uint32_t*>((isv ? v_q : k_q) + crow * kHd + 4 * lane);
+    const long long crow = c0 + (long long)kvh * rs;
+    uint32_t lv;
+    if constexpr (BITS == 8) lv = *reinterpret_cast<const uint32_t*>((isv ? v_q : k_q) + crow * kHd + 4 * lane);
+    else lv = kv4_unpack(*reinterpret_cast<const uint32_t*>((isv ? v_q : k_q) + crow * LB + 4 * (lane & 15)), lane < 16);
     typename Pair<T>::type s2, z2;
     s2.x = s2.y = (isv ? v_s : k_s)[crow * ng + grp];
     z2.x = z2.y = (isv ? v_z : k_z)[crow * ng + grp];
@@ -2244,19 +2576,30 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_paged(const void* q, const v
                                 head_dim, batch, dtype, stream);
 }
 
-// table == nullptr: contiguous caches; else page pools (seqpos only)
+// The group sizes of a quantised cache: 64 or 128 for 8 bits, 32 or 64 for 4 bits (a 4-bit row of one group has no 4bit_u8 packing)
+static int kv_group_args(const char* name, int bits, int group_size) {
+  if (bits == 8) {
+    HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  } else {
+    HQQ_REQUIRE(group_size == 32 || group_size == 64, HQQ_E_UNSUPPORTED, "%s: group_size must be 32 or 64 (got %d)", name, group_size);
+  }
+  return HQQ_OK;
+}
+
+// table == nullptr: contiguous caches; else page pools (seqpos only).  bits 8 or 4.
 static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
                                       const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
                                       const int* table, const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
-                                      int group_size, int batch, int dtype, void* stream) {
+                                      int group_size, int batch, int dtype, void* stream, int bits = 8) {
   HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && pos && out && workspace, HQQ_E_INVALID,
               "%s: null pointer", name);
   HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
   HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0 && ((uintptr_t)k_q & 15) == 0 && ((uintptr_t)v_q & 15) == 0, HQQ_E_INVALID,
               "%s: workspace must be 4-byte and the level caches 16-byte aligned", name);
   HQQ_REQUIRE(head_dim == kHd && n_kv_heads > 0 && n_kv_heads <= 65535 && n_q_heads % n_kv_heads == 0 && n_q_heads / n_kv_heads >= 1 &&
-                  n_q_heads / n_kv_heads <= kSplitMaxGroup && cache_len > 0 && cache_len <= kSplitMaxLen && (group_size == 64 || group_size == 128),
+                  n_q_heads / n_kv_heads <= kSplitMaxGroup && cache_len > 0 && cache_len <= kSplitMaxLen,
               HQQ_E_UNSUPPORTED, "%s: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072, group_size 64 or 128", name);
+  if (int rc = kv_group_args(name, bits, group_size)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int S = split_count(n_kv_heads, cache_len);
   const int G = n_q_heads / n_kv_heads;
@@ -2269,6 +2612,13 @@ static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void*
     using E = decltype(tag);
     constexpr bool SP = decltype(sp)::value;
     constexpr bool PG = std::is_same<decltype(pg), PageTable>::value;
+    if (bits == 4) {
+      if (int rc = reserve_smem<rope_attn_decode_split_kv4_kernel<E, SP, PG>>(kKv4SmemBytes)) return rc;
+      return launch_pdl("rope_attn_decode_split_kv4", rope_attn_decode_split_kv4_kernel<E, SP, PG>, grid, dim3(kSplitThreads), kKv4SmemBytes, st,
+                        (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
+                        (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, group_size,
+                        scale_log2, pg);
+    }
     if (int rc = reserve_smem<rope_attn_decode_split_kv8_kernel<E, SP, PG>>(kKv8SmemBytes)) return rc;
     return launch_pdl("rope_attn_decode_split_kv8", rope_attn_decode_split_kv8_kernel<E, SP, PG>, grid, dim3(kSplitThreads), kKv8SmemBytes, st,
                       (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
@@ -2314,46 +2664,98 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_paged(const void* q, con
                                     n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
 }
 
+extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                        const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
+                                                        int head_dim, int group_size, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv4", false, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
+                                    v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                               void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                               const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
+                                                               int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv4_seqpos", true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q,
+                                    v_scale, v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream,
+                                    4);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                              void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                                              const int* table, const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
+                                                              int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_attn_decode_split_kv4_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_attn_decode_split_kv8(name, true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, pos, out, workspace,
+                                    n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
+}
+
+// The fixed-length (pos0_v == nullptr: uniform pos0, T) and variable-length (host pos0_v / n_tok_v) appends into a quantised cache
+static int rope_append_rows_kvq(const char* name, int bits, const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage, void* v_stage, void* q_out,
+                                int pos0, int T, const int* pos0_v, const int* n_tok_v, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                int group_size, int batch, int dtype, void* stream) {
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
+              HQQ_E_INVALID, "%s: null pointer", name);
+  VarlenRows vl;
+  int max_t = 0;
+  if (pos0_v) {
+    if (int rc = varlen_args(name, pos0_v, n_tok_v, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  } else if (int rc = prefill_args(name, pos0, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) {
+    return rc;
+  }
+  if (int rc = kv_group_args(name, bits, group_size)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag, auto kernel, auto rows, dim3 grid) {
+    using E = decltype(tag);
+    return launch_pdl(name, kernel, grid, dim3(256), 0, st, (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table,
+                      (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0_v ? 0 : pos0,
+                      pos0_v ? 0 : T, n_q_heads, n_kv_heads, cache_len, group_size, rows, NoPages());
+  };
+  const dim3 gf((unsigned)T, (unsigned)batch), gv((unsigned)max_t, (unsigned)batch);
+  if (bits == 8) {
+    if (pos0_v) return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true>, vl, gv)
+                                        : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true>, vl, gv);
+    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half>, NoVarlen(), gf)
+                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16>, NoVarlen(), gf);
+  }
+  if (pos0_v) return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true, false, false, 4>, vl, gv)
+                                      : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true, false, false, 4>, vl, gv);
+  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, false, false, 4>, NoVarlen(), gf)
+                          : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, false, false, 4>, NoVarlen(), gf);
+}
+
 extern "C" int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_q,
                                                   void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage, void* v_stage,
                                                   void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                                   int group_size, int batch, int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_kv8";
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
-              HQQ_E_INVALID, "%s: null pointer", name);
-  if (int rc = prefill_args(name, pos0, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
-  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag) {
-    using E = decltype(tag);
-    return launch_pdl("rope_append_rows_kv8", rope_append_rows_kv8_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q,
-                      (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q,
-                      (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0, T, n_q_heads, n_kv_heads, cache_len, group_size, NoVarlen(),
-                      NoPages());
-  };
-  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv8", 8, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, k_stage,
+                              v_stage, q_out, pos0, T, nullptr, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows_kv8_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                          void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage,
                                                          void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads,
                                                          int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_kv8_varlen";
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
-              HQQ_E_INVALID, "%s: null pointer", name);
-  VarlenRows vl;
-  int max_t = 0;
-  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
-  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag) {
-    using E = decltype(tag);
-    return launch_pdl("rope_append_rows_kv8_varlen", rope_append_rows_kv8_kernel<E, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
-                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
-                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl,
-                      NoPages());
-  };
-  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv8_varlen", 8, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero,
+                              k_stage, v_stage, q_out, 0, 0, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv4(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_q,
+                                                  void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage, void* v_stage,
+                                                  void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                  int group_size, int batch, int dtype, void* stream) {
+  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv4", 4, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, k_stage,
+                              v_stage, q_out, pos0, T, nullptr, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv4_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage,
+                                                         void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads,
+                                                         int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
+  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv4_varlen", 4, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero,
+                              k_stage, v_stage, q_out, 0, 0, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache,
@@ -2447,28 +2849,78 @@ extern "C" int hqq_b200_glue_rope_append_rows_paged(const void* q, const void* k
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
 
-extern "C" int hqq_b200_glue_rope_append_rows_kv8_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
-                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
-                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
-                                                        void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_kv8_paged";
+static int rope_append_rows_kvq_paged(const char* name, int bits, const void* q, const void* k, const void* v, const void* cos_table,
+                                      const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                      const int* table, void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                      int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
   HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
               HQQ_E_INVALID, "%s: null pointer", name);
   if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
   VarlenRows vl;
   int max_t = 0;
   if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
-  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  if (int rc = kv_group_args(name, bits, group_size)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag) {
+  auto go = [&](auto tag, auto kernel) {
     using E = decltype(tag);
-    return launch_pdl("rope_append_rows_kv8_paged", rope_append_rows_kv8_kernel<E, true, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
-                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
-                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl,
-                      PageTable{table});
+    return launch_pdl(name, kernel, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k, (const E*)v,
+                      (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q, (E*)v_scale, (E*)v_zero,
+                      (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl, PageTable{table});
   };
-  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+  if (bits == 8)
+    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true, true>)
+                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true, true>);
+  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true, true, false, 4>)
+                          : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true, true, false, 4>);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
+                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
+                                                        void* stream) {
+  return rope_append_rows_kvq_paged("hqq_b200_glue_rope_append_rows_kv8_paged", 8, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
+                                    v_zero, table, k_stage, v_stage, q_out, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch,
+                                    n_pages, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv4_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
+                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
+                                                        void* stream) {
+  return rope_append_rows_kvq_paged("hqq_b200_glue_rope_append_rows_kv4_paged", 4, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
+                                    v_zero, table, k_stage, v_stage, q_out, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch,
+                                    n_pages, dtype, stream);
+}
+
+// Staging rows [0, pos0[b]) of the slots with n_tok[b] > 0 from a quantised cache: page pools through the table, or (table == nullptr,
+// 4 bits only) the contiguous caches
+static int kvq_stage(const char* name, int bits, const void* k_q, const void* k_scale, const void* k_zero, const void* v_q, const void* v_scale,
+                     const void* v_zero, const int* table, void* k_stage, void* v_stage, const int* pos0, const int* n_tok, int n_kv_heads, int cache_len,
+                     int head_dim, int group_size, int batch, int dtype, void* stream) {
+  HQQ_REQUIRE(k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage, HQQ_E_INVALID, "%s: null pointer", name);
+  VarlenRows vl;
+  int max_t = 0;
+  if (int rc = varlen_args(name, pos0, n_tok, n_kv_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  if (int rc = kv_group_args(name, bits, group_size)) return rc;
+  int max_p = 0;  // rows to refill: [0, pos0[b]) of the slots in the chunk
+  for (int b = 0; b < batch; ++b)
+    if (vl.n_tok[b] > 0) max_p = max(max_p, vl.pos0[b]);
+  if (max_p == 0) return HQQ_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  auto go = [&](auto tag, auto kernel, auto pg) {
+    using E = decltype(tag);
+    return launch_pdl(name, kernel, dim3((unsigned)max_p, (unsigned)batch), dim3(256), 0, st, (const uint8_t*)k_q, (const E*)k_scale, (const E*)k_zero,
+                      (const uint8_t*)v_q, (const E*)v_scale, (const E*)v_zero, (E*)k_stage, (E*)v_stage, n_kv_heads, cache_len, group_size, vl, pg);
+  };
+  const PageTable pt{table};
+  if (bits == 8)
+    return dtype == HQQ_F16 ? go(__half(), kv8_stage_paged_kernel<__half>, pt) : go(__nv_bfloat16(), kv8_stage_paged_kernel<__nv_bfloat16>, pt);
+  if (table)
+    return dtype == HQQ_F16 ? go(__half(), kv8_stage_paged_kernel<__half, 4>, pt) : go(__nv_bfloat16(), kv8_stage_paged_kernel<__nv_bfloat16, 4>, pt);
+  return dtype == HQQ_F16 ? go(__half(), kv8_stage_paged_kernel<__half, 4, false>, NoPages())
+                          : go(__nv_bfloat16(), kv8_stage_paged_kernel<__nv_bfloat16, 4, false>, NoPages());
 }
 
 extern "C" int hqq_b200_glue_kv8_stage_paged(const void* k_q, const void* k_scale, const void* k_zero, const void* v_q, const void* v_scale,
@@ -2477,22 +2929,25 @@ extern "C" int hqq_b200_glue_kv8_stage_paged(const void* k_q, const void* k_scal
   const char* name = "hqq_b200_glue_kv8_stage_paged";
   HQQ_REQUIRE(k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage, HQQ_E_INVALID, "%s: null pointer", name);
   if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  VarlenRows vl;
-  int max_t = 0;
-  if (int rc = varlen_args(name, pos0, n_tok, n_kv_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
-  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
-  int max_p = 0;  // rows to refill: [0, pos0[b]) of the slots in the chunk
-  for (int b = 0; b < batch; ++b)
-    if (vl.n_tok[b] > 0) max_p = max(max_p, vl.pos0[b]);
-  if (max_p == 0) return HQQ_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag) {
-    using E = decltype(tag);
-    return launch_pdl("kv8_stage_paged", kv8_stage_paged_kernel<E>, dim3((unsigned)max_p, (unsigned)batch), dim3(256), 0, st, (const uint8_t*)k_q,
-                      (const E*)k_scale, (const E*)k_zero, (const uint8_t*)v_q, (const E*)v_scale, (const E*)v_zero, (E*)k_stage, (E*)v_stage, n_kv_heads,
-                      cache_len, group_size, vl, PageTable{table});
-  };
-  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+  return kvq_stage(name, 8, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, k_stage, v_stage, pos0, n_tok, n_kv_heads, cache_len, head_dim,
+                   group_size, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_kv4_stage_paged(const void* k_q, const void* k_scale, const void* k_zero, const void* v_q, const void* v_scale,
+                                             const void* v_zero, const int* table, void* k_stage, void* v_stage, const int* pos0, const int* n_tok,
+                                             int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_kv4_stage_paged";
+  HQQ_REQUIRE(k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage, HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return kvq_stage(name, 4, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, k_stage, v_stage, pos0, n_tok, n_kv_heads, cache_len, head_dim,
+                   group_size, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_kv4_stage(const void* k_q, const void* k_scale, const void* k_zero, const void* v_q, const void* v_scale, const void* v_zero,
+                                       void* k_stage, void* v_stage, const int* pos0, const int* n_tok, int n_kv_heads, int cache_len, int head_dim,
+                                       int group_size, int batch, int dtype, void* stream) {
+  return kvq_stage("hqq_b200_glue_kv4_stage", 4, k_q, k_scale, k_zero, v_q, v_scale, v_zero, nullptr, k_stage, v_stage, pos0, n_tok, n_kv_heads, cache_len,
+                   head_dim, group_size, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_attn_prefill_paged(const void* q_rot, const void* k_pool, const void* v_pool, const int* table, void* out, const int* pos0,
@@ -2564,15 +3019,15 @@ extern "C" int hqq_b200_glue_rope_append_rows_devpos_paged(const void* q, const 
                                  batch, dtype, stream);
 }
 
-// table == nullptr: contiguous 8-bit caches; else page pools
+// table == nullptr: contiguous quantised caches; else page pools.  bits 8 or 4.
 static int rope_append_rows_kv8_devpos(const char* name, const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table, void* q_out,
                                        const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int batch,
-                                       int dtype, void* stream) {
+                                       int dtype, void* stream, int bits = 8) {
   HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && q_out && pos, HQQ_E_INVALID,
               "%s: null pointer", name);
   if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
-  HQQ_REQUIRE(group_size == 64 || group_size == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, group_size);
+  if (int rc = kv_group_args(name, bits, group_size)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const DevPos dp{(const long long*)pos};
   auto go = [&](auto tag, auto kernel, auto pg) {
@@ -2581,8 +3036,15 @@ static int rope_append_rows_kv8_devpos(const char* name, const void* q, const vo
                       (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q, (E*)v_scale,
                       (E*)v_zero, (E*)nullptr, (E*)nullptr, (E*)q_out, 0, T, n_q_heads, n_kv_heads, cache_len, group_size, dp, pg);
   };
+  const PageTable pt{table};
+  if (bits == 4) {
+    if (table)
+      return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, true, true, 4>, pt)
+                              : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, true, true, 4>, pt);
+    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, false, true, 4>, NoPages())
+                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, false, true, 4>, NoPages());
+  }
   if (table) {
-    const PageTable pt{table};
     return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, true, true>, pt)
                             : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, true, true>, pt);
   }
@@ -2609,6 +3071,25 @@ extern "C" int hqq_b200_glue_rope_append_rows_kv8_devpos_paged(const void* q, co
                                      n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
 }
 
+extern "C" int hqq_b200_glue_rope_append_rows_kv4_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* q_out,
+                                                         const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                         int group_size, int batch, int dtype, void* stream) {
+  return rope_append_rows_kv8_devpos("hqq_b200_glue_rope_append_rows_kv4_devpos", q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
+                                     v_zero, nullptr, q_out, pos, T, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv4_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                               const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
+                                                               void* v_zero, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                                               int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages,
+                                                               int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_rope_append_rows_kv4_devpos_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_append_rows_kv8_devpos(name, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, q_out, pos, T, n_q_heads,
+                                     n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
+}
+
 // column groups of one kv head in the verify attention
 static int verify_groups(int n_q_heads, int n_kv_heads, int T) { return (int)cdiv((int64_t)T * (n_q_heads / n_kv_heads), kVerCols); }
 
@@ -2619,15 +3100,16 @@ extern "C" size_t hqq_b200_glue_attn_verify_split_workspace_bytes(int n_q_heads,
   return groups * s_max * kVerCols * (size_t)(head_dim + 2) * sizeof(float) + groups * sizeof(unsigned);
 }
 
-// table == nullptr: contiguous caches; meta == nullptr: 16-bit caches, else the 8-bit cache's {k_scale, k_zero, v_scale, v_zero}
+// table == nullptr: contiguous caches; meta == nullptr: 16-bit caches, else the quantised cache's {k_scale, k_zero, v_scale, v_zero}
+// with `bits` 8 or 4
 static int attn_verify_split(const char* name, const void* q_rot, const void* k_cache, const void* v_cache, const void* const* meta, int gs,
                              const int* table, const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
-                             int head_dim, int T, int batch, int dtype, void* stream) {
+                             int head_dim, int T, int batch, int dtype, void* stream, int bits = 8) {
   HQQ_REQUIRE(q_rot && k_cache && v_cache && pos && out && workspace, HQQ_E_INVALID, "%s: null pointer", name);
   if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
   if (meta) {
     HQQ_REQUIRE(meta[0] && meta[1] && meta[2] && meta[3], HQQ_E_INVALID, "%s: null pointer", name);
-    HQQ_REQUIRE(gs == 64 || gs == 128, HQQ_E_UNSUPPORTED, "%s: group_size must be 64 or 128 (got %d)", name, gs);
+    if (int rc = kv_group_args(name, bits, gs)) return rc;
   }
   cudaStream_t st = (cudaStream_t)stream;
   const int S = split_count(n_kv_heads, cache_len), n_cg = verify_groups(n_q_heads, n_kv_heads, T);
@@ -2637,23 +3119,29 @@ static int attn_verify_split(const char* name, const void* q_rot, const void* k_
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
   const dim3 grid((unsigned)S, (unsigned)(n_kv_heads * n_cg), (unsigned)batch);
   constexpr int smem = kRingBytes + 16;
-  auto run = [&](auto tag, auto pg, auto paged, auto kv8) -> int {
+  auto run = [&](auto tag, auto pg, auto paged, auto kv8, auto nbits) -> int {
     using E = decltype(tag);
     constexpr bool PG = decltype(paged)::value, K8 = decltype(kv8)::value;
+    constexpr int NB = decltype(nbits)::value;
     using C = CacheT<E, K8>;
     Kv8Arg<E, K8> m8;
     if constexpr (K8) m8 = Kv8Meta<E>{(const E*)meta[0], (const E*)meta[1], (const E*)meta[2], (const E*)meta[3], gs};
-    if (int rc = reserve_smem<attn_verify_split_kernel<E, PG, K8>>(smem)) return rc;
-    return launch_pdl(K8 ? "attn_verify_split_kv8" : "attn_verify_split", attn_verify_split_kernel<E, PG, K8>, grid, dim3(kSplitThreads), smem, st,
-                      (const E*)q_rot, (const C*)k_cache, (const C*)v_cache, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads,
-                      cache_len, T, scale_log2, pg, m8);
+    if (int rc = reserve_smem<attn_verify_split_kernel<E, PG, K8, NB>>(smem)) return rc;
+    return launch_pdl(K8 ? (NB == 4 ? "attn_verify_split_kv4" : "attn_verify_split_kv8") : "attn_verify_split", attn_verify_split_kernel<E, PG, K8, NB>,
+                      grid, dim3(kSplitThreads), smem, st, (const E*)q_rot, (const C*)k_cache, (const C*)v_cache, (const long long*)pos, (E*)out, part,
+                      tickets, n_q_heads, n_kv_heads, cache_len, T, scale_log2, pg, m8);
   };
-  auto by_dtype = [&](auto pg, auto paged, auto kv8) {
-    return dtype == HQQ_F16 ? run(__half(), pg, paged, kv8) : run(__nv_bfloat16(), pg, paged, kv8);
+  using B8 = std::integral_constant<int, 8>;
+  auto by_dtype = [&](auto pg, auto paged, auto kv8, auto nbits) {
+    return dtype == HQQ_F16 ? run(__half(), pg, paged, kv8, nbits) : run(__nv_bfloat16(), pg, paged, kv8, nbits);
   };
   const PageTable pt{table};
-  if (meta) return table ? by_dtype(pt, std::true_type(), std::true_type()) : by_dtype(NoPages(), std::false_type(), std::true_type());
-  return table ? by_dtype(pt, std::true_type(), std::false_type()) : by_dtype(NoPages(), std::false_type(), std::false_type());
+  if (meta && bits == 4) {
+    using B4 = std::integral_constant<int, 4>;
+    return table ? by_dtype(pt, std::true_type(), std::true_type(), B4()) : by_dtype(NoPages(), std::false_type(), std::true_type(), B4());
+  }
+  if (meta) return table ? by_dtype(pt, std::true_type(), std::true_type(), B8()) : by_dtype(NoPages(), std::false_type(), std::true_type(), B8());
+  return table ? by_dtype(pt, std::true_type(), std::false_type(), B8()) : by_dtype(NoPages(), std::false_type(), std::false_type(), B8());
 }
 
 extern "C" int hqq_b200_glue_attn_verify_split(const void* q_rot, const void* k_cache, const void* v_cache, const int64_t* pos, void* out,
@@ -2690,6 +3178,26 @@ extern "C" int hqq_b200_glue_attn_verify_split_kv8_paged(const void* q_rot, cons
   const void* meta[4] = {k_scale, k_zero, v_scale, v_zero};
   return attn_verify_split(name, q_rot, k_q, v_q, meta, group_size, table, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, T, batch,
                            dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_attn_verify_split_kv4(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero, const void* v_q,
+                                                   const void* v_scale, const void* v_zero, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                   int n_kv_heads, int cache_len, int head_dim, int group_size, int T, int batch, int dtype,
+                                                   void* stream) {
+  const void* meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return attn_verify_split("hqq_b200_glue_attn_verify_split_kv4", q_rot, k_q, v_q, meta, group_size, nullptr, pos, out, workspace, n_q_heads,
+                           n_kv_heads, cache_len, head_dim, T, batch, dtype, stream, 4);
+}
+
+extern "C" int hqq_b200_glue_attn_verify_split_kv4_paged(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero, const void* v_q,
+                                                         const void* v_scale, const void* v_zero, const int* table, const int64_t* pos, void* out,
+                                                         void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size,
+                                                         int T, int batch, int n_pages, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_attn_verify_split_kv4_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  const void* meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return attn_verify_split(name, q_rot, k_q, v_q, meta, group_size, table, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, T, batch,
+                           dtype, stream, 4);
 }
 
 extern "C" int hqq_b200_glue_ngram_draft(const int32_t* hist, const int64_t* pos, const int64_t* tok, int64_t* drafts, int cache_len, int K, int batch,

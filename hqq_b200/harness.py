@@ -85,29 +85,37 @@ def rope_tables(shape: LlamaShape, cache_len: int, dtype, device):
     return torch.cat([fr.cos(), fr.cos()], dim=-1).to(dtype), torch.cat([fr.sin(), fr.sin()], dim=-1).to(dtype)
 
 
-def kv8_quantize_rows(x: torch.Tensor, group_size: int):
+def kv8_quantize_rows(x: torch.Tensor, group_size: int, bits: int = 8):
     """The 8-bit KV cache format on framework ops: rows x [..., 128] in T -> levels uint8 [..., 128] and scale, zero
     [..., 128 / group_size] in T.  HQQ's Quantizer.quantize(row, nbits=8, group_size, axis=1, optimize=False) (round_zero off, as for
     8-bit layers) in fp32 -- inverse scale reciprocal(max - min) * 255 (1 where max - min <= 1e-4, at most 2e4), zero -min * s,
     levels round(x * s + z) clamped to [0, 255] with the product and the sum rounded separately -- then scale = 1 / s and the zero
     cast to T.  The solver is not run: its early stop compares a mean over the whole tensor, so a row's levels would depend on
-    which rows were quantised with it."""
+    which rows were quantised with it.  bits 4: the 4-bit cache, nbits=4 (15 in place of 255, group_size 32 or 64), each row's levels
+    packed as the reference's 4bit_u8 packing of that row: uint8 [..., 64], byte d = q[d] << 4 | q[d + 64]."""
+    maxv = float((1 << bits) - 1)
     shape = x.shape
     w = x.float().reshape(-1, group_size)
     mn, mx = w.amin(dim=1, keepdim=True), w.amax(dim=1, keepdim=True)
     denom = mx - mn
-    s = torch.reciprocal(denom) * 255.0
+    s = torch.reciprocal(denom) * maxv
     s = torch.where(denom.abs() <= 1e-4, torch.ones_like(s), s)
     s = torch.clamp(s, max=2e4)
     z = -mn * s
-    q = torch.clamp(torch.round(w * s + z), 0, 255).to(torch.uint8)
+    q = torch.clamp(torch.round(w * s + z), 0, maxv).to(torch.uint8).reshape(shape)
+    if bits == 4:
+        half = shape[-1] // 2
+        q = (q[..., :half] << 4) | q[..., half:]
     meta = shape[:-1] + (shape[-1] // group_size,)
-    return q.reshape(shape), torch.reciprocal(s).to(x.dtype).reshape(meta), z.to(x.dtype).reshape(meta)
+    return q, torch.reciprocal(s).to(x.dtype).reshape(meta), z.to(x.dtype).reshape(meta)
 
 
-def kv8_dequantize(q: torch.Tensor, scale: torch.Tensor, zero: torch.Tensor) -> torch.Tensor:
+def kv8_dequantize(q: torch.Tensor, scale: torch.Tensor, zero: torch.Tensor, bits: int = 8) -> torch.Tensor:
     """Rows of the 8-bit KV cache back in T: (T(q) - zero) * scale with one rounding to T per operation (hqq_b200_dequantize,
-    Quantizer.dequantize).  q [..., 128] uint8, scale / zero [..., 128 / group_size] in T."""
+    Quantizer.dequantize).  q [..., 128] uint8, scale / zero [..., 128 / group_size] in T.  bits 4: q [..., 64] packed as
+    kv8_quantize_rows packs it, unpacked first."""
+    if bits == 4:
+        q = torch.cat([q >> 4, q & 15], dim=-1)
     ng = scale.shape[-1]
     qs = q.reshape(q.shape[:-1] + (ng, q.shape[-1] // ng)).to(scale.dtype)
     return ((qs - zero.unsqueeze(-1)) * scale.unsqueeze(-1)).reshape(q.shape)
@@ -377,7 +385,7 @@ class DecodeModel:
     def __init__(self, shape: LlamaShape = LLAMA3_8B, nbits: int = 4, group_size: int = 64, dtype=torch.float16,
                  device="cuda", cache_len: int = 256, tp: int = 1, rank: int = 0, seed: int = 0, process_group=None,
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
-                 kv_bits: int = 16, kv_group_size: int = 64, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
+                 kv_bits: int = 16, kv_group_size: int | None = None, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
                  top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None, spec_k: int | None = None):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
         # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
@@ -393,14 +401,24 @@ class DecodeModel:
         if not (isinstance(sample_seed, int) and 0 <= sample_seed < 2 ** 64):
             raise ValueError(f"sample_seed must be an int in [0, 2^64) (got {sample_seed!r})")
         self.do_sample, self.temperature, self.top_k, self.top_p, self.sample_seed = bool(do_sample), float(temperature), int(top_k), float(top_p), int(sample_seed)
-        # kv_bits 8: every layer's K and V cache in HQQ's 8-bit format (kv8_quantize_rows), groups of kv_group_size along the head dim
-        if kv_bits not in (16, 8):
-            raise ValueError(f"kv_bits must be 16 or 8 (got {kv_bits!r})")
-        if kv_group_size not in (64, 128):
+        # kv_bits 8: every layer's K and V cache in HQQ's 8-bit format (kv8_quantize_rows), groups of kv_group_size along the head dim;
+        # kv_bits 4: HQQ's 4-bit format, each row's levels packed by 4bit_u8 (kv8_quantize_rows(..., bits=4)), groups of 32 or 64.
+        # kv_group_size defaults to 64 for the 8-bit cache; the 4-bit cache takes it explicitly: at 4 bits the group size is the
+        # cache's accuracy / size trade-off (gs 32: 160 bytes per position and kv head, gs 64: 144), not a detail to default silently
+        if kv_bits not in (16, 8, 4):
+            raise ValueError(f"kv_bits must be 16, 8 or 4 (got {kv_bits!r})")
+        if kv_group_size is None:
+            if kv_bits == 4:
+                raise ValueError("kv_bits=4 needs an explicit kv_group_size, 32 or 64")
+            kv_group_size = 64
+        if kv_bits == 4 and kv_group_size not in (32, 64):
+            raise ValueError(f"kv_group_size must be 32 or 64 with kv_bits=4 (got {kv_group_size!r})")
+        if kv_bits != 4 and kv_group_size not in (64, 128):
             raise ValueError(f"kv_group_size must be 64 or 128 (got {kv_group_size!r})")
-        if kv_bits == 8 and shape.head_dim != 128:
-            raise ValueError("kv_bits=8 needs head_dim 128")
+        if kv_bits != 16 and shape.head_dim != 128:
+            raise ValueError(f"kv_bits={kv_bits} needs head_dim 128")
         self.kv_bits, self.kv_group_size = int(kv_bits), int(kv_group_size)
+        self._kvq = self.kv_bits != 16  # a quantised cache: levels plus scale and zero
         # batch > 1 (BASELINE configs[4], bs = 32): `batch` sequences decode in lock-step at the same position; the linears then
         # run the small-M kernel (M = batch <= 32; the wgmma kernel from 17 sequences on large matrices) between the batched glue
         # kernels -- the one-token kernels and their NVLink exchange are M = 1 only, so tensor-parallel partials are summed by NCCL
@@ -413,6 +431,8 @@ class DecodeModel:
         self.ragged = bool(ragged)
         if self.ragged and self.batch > 256:
             raise ValueError("ragged batches hold at most 256 sequences")
+        if self.kv_bits == 4 and self.batch > 256:  # the staging refill takes the batch as slots
+            raise ValueError("kv_bits=4 holds at most 256 sequences")
         # kv_pages N (ragged only): every layer's cache is a pool of N + 1 pages [N + 1, n_kv, 64, 128] (page N the sink) and the
         # slots reach their rows through one shared device page_table [batch, cache_len / 64]; PageAllocator hands out the pages.
         # The kernels are the ragged ones' PAGED twins: a paged model computes the unpaged ragged model's bits.
@@ -489,15 +509,16 @@ class DecodeModel:
             blk["norm1"] = torch.ones(shape.hidden, device=self.device, dtype=dtype)
             blk["norm2"] = torch.ones(shape.hidden, device=self.device, dtype=dtype)
             hkv = shape.n_kv_heads // tp
-            cdt = torch.uint8 if self.kv_bits == 8 else dtype
+            cdt = torch.uint8 if self._kvq else dtype
             rows = (self.batch, hkv, cache_len) if kv_pages is None else (kv_pages + 1, hkv, KV_PAGE)
-            blk["k_cache"] = torch.zeros(*rows, shape.head_dim, device=self.device, dtype=cdt)
-            blk["v_cache"] = torch.zeros(*rows, shape.head_dim, device=self.device, dtype=cdt)
-            if self.kv_bits == 8:
+            width = shape.head_dim * self.kv_bits // 8 if self._kvq else shape.head_dim  # level bytes or elements a row
+            blk["k_cache"] = torch.zeros(*rows, width, device=self.device, dtype=cdt)
+            blk["v_cache"] = torch.zeros(*rows, width, device=self.device, dtype=cdt)
+            if self._kvq:
                 for name in ("k_scale", "k_zero", "v_scale", "v_zero"):
                     blk[name] = torch.zeros(*rows, shape.head_dim // kv_group_size, device=self.device, dtype=dtype)
             self.blocks.append(blk)
-        self._kv8_stage = None  # kv_bits 8: dequantised fp16 / bf16 K and V for the prefill attention, allocated by the first fused prefill
+        self._kv8_stage = None  # kv_bits 8 / 4: dequantised fp16 / bf16 K and V for the prefill attention, allocated by the first fused prefill
         self.cos, self.sin = rope_tables(shape, cache_len, dtype, self.device)  # [cache_len, hd]
         self.arange = torch.arange(cache_len, device=self.device)
         # static I/O for graph capture
@@ -522,9 +543,9 @@ class DecodeModel:
     @property
     def attn_kernel(self) -> str:
         """Attention kernel of the fused steps: "single" (one CTA per query head, cache_len <= 8192), "split" (split-KV) or
-        "split_kv8" (split-KV over the 8-bit cache, at every cache_len)."""
-        if self.kv_bits == 8:
-            return "split_kv8"
+        "split_kv8" / "split_kv4" (split-KV over the 8-bit / 4-bit cache, at every cache_len)."""
+        if self._kvq:
+            return f"split_kv{self.kv_bits}"
         return "split" if self.cache_len > SINGLE_ATTN_MAX_LEN else "single"
 
     _CACHE_NAMES = ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero")
@@ -580,7 +601,7 @@ class DecodeModel:
             raise ValueError(f"{what} needs a paged KV cache (kv_pages)")
 
     def kv_cache_bytes(self) -> int:
-        """Bytes of every layer's KV cache on this rank: fp16 / bf16 rows, or levels plus scale and zero with kv_bits 8 (with
+        """Bytes of every layer's KV cache on this rank: fp16 / bf16 rows, or levels plus scale and zero with kv_bits 8 / 4 (with
         kv_pages: the page pools, sink included)."""
         names = ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero")
         return sum(blk[n].numel() * blk[n].element_size() for blk in self.blocks for n in names if n in blk)
@@ -589,8 +610,9 @@ class DecodeModel:
         from ._lib import check, ptr
         b = self._bufs
         paged = self.kv_pages is not None
-        if paged and self.kv_bits == 8:
-            check(lib.hqq_b200_glue_rope_attn_decode_split_kv8_paged(
+        kvq = f"kv{self.kv_bits}"
+        if paged and self._kvq:
+            check(getattr(lib, f"hqq_b200_glue_rope_attn_decode_split_{kvq}_paged")(
                 ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]),
                 ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(self.page_table), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq,
                 hkv, self.cache_len, self.shape.head_dim, self.kv_group_size, self.batch, self.kv_pages, code, st))
@@ -600,8 +622,8 @@ class DecodeModel:
                                                                  ptr(blk["v_cache"]), ptr(self.page_table), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq,
                                                                  hkv, self.cache_len, self.shape.head_dim, self.batch, self.kv_pages, code, st))
             return
-        if self.kv_bits == 8:
-            fn = lib.hqq_b200_glue_rope_attn_decode_split_kv8_seqpos if self.ragged else lib.hqq_b200_glue_rope_attn_decode_split_kv8
+        if self._kvq:
+            fn = getattr(lib, f"hqq_b200_glue_rope_attn_decode_split_{kvq}" + ("_seqpos" if self.ragged else ""))
             check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
                      ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
                      ptr(blk["v_zero"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
@@ -660,15 +682,15 @@ class DecodeModel:
                 else:
                     at = (self.page_table[self._slot_idx, self.pos // KV_PAGE].long(), slice(None), self.pos % KV_PAGE)
                 for name, x in (("k", k), ("v", v.view(B, hkv, hd))):
-                    if self.kv_bits == 8:
-                        lv, sc, ze = kv8_quantize_rows(x, self.kv_group_size)
+                    if self._kvq:
+                        lv, sc, ze = kv8_quantize_rows(x, self.kv_group_size, self.kv_bits)
                         for suffix, val in (("_cache", lv), ("_scale", sc), ("_zero", ze)):
                             blk[name + suffix][at] = val
                     else:
                         blk[name + "_cache"][at] = x
                 cv = self.cache_view(blk)
-                kc, vc = self._kv8_read(cv, self.cache_len) if self.kv_bits == 8 else (cv["k_cache"], cv["v_cache"])
-            elif self.kv_bits == 8:  # the rotated rows quantised into the cache; attention over the dequantised cache
+                kc, vc = self._kv8_read(cv, self.cache_len) if self._kvq else (cv["k_cache"], cv["v_cache"])
+            elif self._kvq:  # the rotated rows quantised into the cache; attention over the dequantised cache
                 self._kv8_write(blk, k.view(B, hkv, 1, hd), v.view(B, hkv, 1, hd), self.pos)
                 kc, vc = self._kv8_read(blk, self.cache_len)
             else:
@@ -708,16 +730,16 @@ class DecodeModel:
             self.hist.scatter_(1, self.pos.view(-1, 1), self.tok.view(-1, 1).to(torch.int32))
 
     def _kv8_write(self, blk, k, v, idx):
-        """kv_bits 8 on framework ops: rows k, v [batch, n_kv, n, 128] quantised into cache positions idx [n]."""
+        """kv_bits 8 / 4 on framework ops: rows k, v [batch, n_kv, n, 128] quantised into cache positions idx [n]."""
         for name, x in (("k", k), ("v", v)):
-            lv, sc, ze = kv8_quantize_rows(x, self.kv_group_size)
+            lv, sc, ze = kv8_quantize_rows(x, self.kv_group_size, self.kv_bits)
             blk[name + "_cache"].index_copy_(2, idx, lv)
             blk[name + "_scale"].index_copy_(2, idx, sc)
             blk[name + "_zero"].index_copy_(2, idx, ze)
 
     def _kv8_read(self, blk, end):
-        """kv_bits 8 on framework ops: the dequantised K and V cache rows [0, end)."""
-        return tuple(kv8_dequantize(blk[n + "_cache"][:, :, :end], blk[n + "_scale"][:, :, :end], blk[n + "_zero"][:, :, :end]) for n in ("k", "v"))
+        """kv_bits 8 / 4 on framework ops: the dequantised K and V cache rows [0, end)."""
+        return tuple(kv8_dequantize(blk[n + "_cache"][:, :, :end], blk[n + "_scale"][:, :, :end], blk[n + "_zero"][:, :, :end], self.kv_bits) for n in ("k", "v"))
 
     def _sample_ref(self, logits):
         """do_sample on framework ops (fused=False): sample_tokens on the full-vocabulary rows (under tensor parallelism every rank
@@ -1157,10 +1179,12 @@ class DecodeModel:
         code = DTYPE_CODE[self.dtype]
         B, n = ids.shape
         M = B * n
+        import ctypes
         if varlen is not None:
-            import ctypes
             B = self.batch
             vp0, vnt = (ctypes.c_int * B)(*varlen[0]), (ctypes.c_int * B)(*varlen[1])
+        elif self.kv_bits == 4:  # the lock-step chunk as slots for the 4-bit staging refill
+            vp0, vnt = (ctypes.c_int * B)(*[p0] * B), (ctypes.c_int * B)(*[n] * B)
         e = lambda w: torch.empty(M, w, device=self.device, dtype=self.dtype)
         h = self.embed.index_select(0, ids.reshape(-1))  # [M, hidden], row b * n + t
         x, q, k, v, qr, a, o = e(s.hidden), e(hq * hd), e(hkv * hd), e(hkv * hd), e(hq * hd), e(hq * hd), e(s.hidden)
@@ -1168,7 +1192,8 @@ class DecodeModel:
         gate, up, act, down = e(inter), e(inter), e(inter), e(s.hidden)
         norm = lambda d, w: check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(d), ptr(w), ptr(x), M, s.hidden, s.rms_eps, code, st))
         delta = None
-        kv8 = self.kv_bits == 8
+        kv8 = self._kvq  # 8 or 4 bits: the staging pair, as below
+        kvq = f"kv{self.kv_bits}"
         paged = self.kv_pages is not None
         if paged:
             pt, npg = ptr(self.page_table), self.kv_pages
@@ -1183,28 +1208,32 @@ class DecodeModel:
                 # staging rows [0, p0) dequantised from the 8-bit cache, rows [p0, p0 + n) written by the rows kernel; the attention
                 # kernel is the one of the fp16 cache, reading the staging pair
                 kst, vst = self._kv8_stage
-                for bi in range(0 if paged else B):
+                for bi in range(0 if paged or self.kv_bits == 4 else B):
                     sp0 = p0 if varlen is None else (varlen[0][bi] if varlen[1][bi] else 0)  # slots outside the chunk: nothing
                     for hh in range(hkv):
                         for c, dst in (("k", kst), ("v", vst)):
                             if sp0 > 0:
                                 check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][bi, hh]), ptr(blk[c + "_scale"][bi, hh]), ptr(blk[c + "_zero"][bi, hh]),
                                                               ptr(dst[bi, hh]), sp0, hd, self.kv_group_size, 8, 1, code, st))
+                if self.kv_bits == 4 and not paged:  # every row is packed on its own: one launch refills the staging rows [0, pos0)
+                    check(lib.hqq_b200_glue_kv4_stage(ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
+                                                      ptr(blk["v_zero"]), ptr(kst), ptr(vst), vp0, vnt, hkv, self.cache_len, hd, self.kv_group_size, B,
+                                                      code, st))
                 if paged:  # one launch refills the staging rows [0, pos0) of the slots in the chunk, through the table
-                    check(lib.hqq_b200_glue_kv8_stage_paged(ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]),
+                    check(getattr(lib, f"hqq_b200_glue_{kvq}_stage_paged")(ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]),
                                                             ptr(blk["v_scale"]), ptr(blk["v_zero"]), pt, ptr(kst), ptr(vst), vp0, vnt, hkv, self.cache_len, hd,
                                                             self.kv_group_size, B, npg, code, st))
-                    check(lib.hqq_b200_glue_rope_append_rows_kv8_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_paged")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
                                                                        ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
                                                                        ptr(blk["v_zero"]), pt, ptr(kst), ptr(vst), ptr(qr), vp0, vnt, hq, hkv, self.cache_len,
                                                                        hd, self.kv_group_size, B, npg, code, st))
                 elif varlen is not None:
-                    check(lib.hqq_b200_glue_rope_append_rows_kv8_varlen(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
+                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_varlen")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
                                                                         ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
                                                                         ptr(blk["v_zero"]), ptr(kst), ptr(vst), ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd,
                                                                         self.kv_group_size, B, code, st))
                 else:
-                    check(lib.hqq_b200_glue_rope_append_rows_kv8(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]),
+                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]),
                                                                  ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(kst),
                                                                  ptr(vst), ptr(qr), p0, n, hq, hkv, self.cache_len, hd, self.kv_group_size, B, code, st))
                 kc, vc = kst, vst
@@ -1264,7 +1293,7 @@ class DecodeModel:
             q, k, v = self._multi(x, (blk["q"], blk["k"], blk["v"]))
             q = self._rope(q.view(B, n, hq, hd), cos, sin)
             k = self._rope(k.view(B, n, hkv, hd), cos, sin)
-            if self.kv_bits == 8:
+            if self._kvq:
                 self._kv8_write(cb, k.transpose(1, 2), v.view(B, n, hkv, hd).transpose(1, 2), torch.arange(p0, end, device=self.device))
                 kc, vc = self._kv8_read(cb, end)
             else:
@@ -1441,18 +1470,19 @@ class DecodeModel:
         ws = self._bufs["verify_ws"]
 
         def attn(blk, q, k, v, qr, a):
-            if self.kv_bits == 8:
+            if self._kvq:
                 c8 = [ptr(blk[n]) for n in ("k_cache", "k_scale", "k_zero", "v_cache", "v_scale", "v_zero")]
                 gs = self.kv_group_size
+                kvq = f"kv{self.kv_bits}"
                 if self.kv_pages is None:
-                    check(lib.hqq_b200_glue_rope_append_rows_kv8_devpos(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, ptr(qr), ptr(self.pos), T,
+                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_devpos")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, ptr(qr), ptr(self.pos), T,
                                                                         hq, hkv, L, hd, gs, B, code, st))
-                    check(lib.hqq_b200_glue_attn_verify_split_kv8(ptr(qr), *c8, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B, code, st))
+                    check(getattr(lib, f"hqq_b200_glue_attn_verify_split_{kvq}")(ptr(qr), *c8, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B, code, st))
                     return
                 pt = ptr(self.page_table)
-                check(lib.hqq_b200_glue_rope_append_rows_kv8_devpos_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, pt, ptr(qr),
+                check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_devpos_paged")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, pt, ptr(qr),
                                                                           ptr(self.pos), T, hq, hkv, L, hd, gs, B, self.kv_pages, code, st))
-                check(lib.hqq_b200_glue_attn_verify_split_kv8_paged(ptr(qr), *c8, pt, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B,
+                check(getattr(lib, f"hqq_b200_glue_attn_verify_split_{kvq}_paged")(ptr(qr), *c8, pt, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B,
                                                                     self.kv_pages, code, st))
                 return
             if self.kv_pages is None:
@@ -1503,13 +1533,13 @@ class DecodeModel:
             q = self._rope(q.view(B, T, hq, hd), cos, sin)
             k = self._rope(k.view(B, T, hkv, hd), cos, sin)
             for name, x in (("k", k[bi, ti]), ("v", v.view(B, T, hkv, hd)[bi, ti])):
-                if self.kv_bits == 8:
-                    for suffix, val in zip(("_cache", "_scale", "_zero"), kv8_quantize_rows(x, self.kv_group_size)):
+                if self._kvq:
+                    for suffix, val in zip(("_cache", "_scale", "_zero"), kv8_quantize_rows(x, self.kv_group_size, self.kv_bits)):
                         blk[name + suffix][at] = val
                 else:
                     blk[name + "_cache"][at] = x
             cv = self.cache_view(blk)
-            kc, vc = self._kv8_read(cv, L) if self.kv_bits == 8 else (cv["k_cache"], cv["v_cache"])
+            kc, vc = self._kv8_read(cv, L) if self._kvq else (cv["k_cache"], cv["v_cache"])
             a = F.scaled_dot_product_attention(q.transpose(1, 2), kc, vc, attn_mask=mask, enable_gqa=True)
             o = blk["o"](a.transpose(1, 2).reshape(B * T, hq * hd))
             if self.tp > 1:

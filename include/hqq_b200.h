@@ -461,6 +461,75 @@ int hqq_b200_glue_attn_verify_split_kv8_paged(const void* q_rot, const void* k_q
                                               const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
                                               int cache_len, int head_dim, int group_size, int T, int batch, int n_pages, int dtype,
                                               void* stream);
+
+/* ---- 4-bit HQQ KV cache.
+ * A cache row of one kv head is HQQ's Quantizer.quantize(row[1, 128], nbits=4, group_size=gs, axis=1, optimize=False,
+ * round_zero=False) in fp32: inverse scale s = 15 / (max - min) (1 where |max - min| <= 1e-4, at most 2e4), zero z = -min * s,
+ * levels round(x * s + z) clamped to [0, 15] with the product and the sum rounded separately; stored meta scale = 1 / s and zero,
+ * both cast to T.  The levels are packed as the reference's 4bit_u8 packing of that row: 64 bytes, byte d = q[d] << 4 | q[d + 64].
+ * group_size is 32 or 64 (a one-group row has no 4bit_u8 packing).  Levels uint8 [batch, n_kv_heads, cache_len, 64] (pages
+ * [n_pages + 1, n_kv_heads, 64, 64]), meta [.., 128 / group_size] T.  The attended row is T(T(q - z) * s), what
+ * Quantizer.dequantize gives.  Each entry point below is its kv8 twin with the same arguments, grid, split count, merge order,
+ * workspace (the decode and verify forms use the existing workspace-size functions), RoPE rounding and preconditions, on this
+ * format: the decode kernel quantises and packs the fresh k / v row and attends to its dequantisation, split 0 writing it to the
+ * cache; the rows kernels write the rows the decode kernel writes and (not _devpos) stage their dequantisation. */
+int hqq_b200_glue_rope_attn_decode_split_kv4(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                             void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                             const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
+                                             int head_dim, int group_size, int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_attn_decode_split_kv4_seqpos(const void* q, const void* k, const void* v, const void* cos_table,
+                                                    const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
+                                                    void* v_zero, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                    int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int dtype,
+                                                    void* stream);
+int hqq_b200_glue_rope_attn_decode_split_kv4_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                   const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
+                                                   void* v_zero, const int* table, const int64_t* pos, void* out, void* workspace,
+                                                   int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int batch,
+                                                   int n_pages, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_kv4(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                       void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage,
+                                       void* v_stage, void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len,
+                                       int head_dim, int group_size, int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_kv4_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                              void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                              void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                              int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int dtype,
+                                              void* stream);
+int hqq_b200_glue_rope_append_rows_kv4_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                             void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                             const int* table, void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok,
+                                             int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int batch,
+                                             int n_pages, int dtype, void* stream);
+/* Staging rows [0, pos0[b]) of every slot with n_tok[b] > 0 (host pos0 / n_tok, as the _varlen appends take them), dequantised from
+ * the 4-bit cache: the contiguous caches (hqq_b200_dequantize cannot serve them: it unpacks slabs spanning all rows, while here
+ * every row is packed on its own), or the page pools through the table.  Staging [batch, n_kv_heads, cache_len, 128] T. */
+int hqq_b200_glue_kv4_stage(const void* k_q, const void* k_scale, const void* k_zero, const void* v_q, const void* v_scale,
+                            const void* v_zero, void* k_stage, void* v_stage, const int* pos0, const int* n_tok, int n_kv_heads,
+                            int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream);
+int hqq_b200_glue_kv4_stage_paged(const void* k_q, const void* k_scale, const void* k_zero, const void* v_q, const void* v_scale,
+                                  const void* v_zero, const int* table, void* k_stage, void* v_stage, const int* pos0, const int* n_tok,
+                                  int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
+                                  void* stream);
+int hqq_b200_glue_rope_append_rows_kv4_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                              void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
+                                              void* q_out, const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len,
+                                              int head_dim, int group_size, int batch, int dtype, void* stream);
+int hqq_b200_glue_rope_append_rows_kv4_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                    const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q,
+                                                    void* v_scale, void* v_zero, const int* table, void* q_out, const int64_t* pos, int T,
+                                                    int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int batch,
+                                                    int n_pages, int dtype, void* stream);
+int hqq_b200_glue_attn_verify_split_kv4(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero, const void* v_q,
+                                        const void* v_scale, const void* v_zero, const int64_t* pos, void* out, void* workspace,
+                                        int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int T, int batch,
+                                        int dtype, void* stream);
+int hqq_b200_glue_attn_verify_split_kv4_paged(const void* q_rot, const void* k_q, const void* k_scale, const void* k_zero,
+                                              const void* v_q, const void* v_scale, const void* v_zero, const int* table,
+                                              const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
+                                              int cache_len, int head_dim, int group_size, int T, int batch, int n_pages, int dtype,
+                                              void* stream);
+
 /* Prompt-lookup drafts: slot b knows L = pos[b] + 1 tokens, hist[b][0 .. pos - 1] (int32 [batch, cache_len]) and tok[b] at pos.
  * Take the longest g in {3, 2, 1} for which some j with j + g <= L - 1 has hist[j .. j+g-1] == the last g tokens, the largest such
  * j, and write drafts[b][i] = token j + g + i while j + g + i < L, else -1 (int64 [batch, K]); no match: every draft -1. */

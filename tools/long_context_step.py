@@ -5,11 +5,11 @@ caches filled with random rows so no prompt has to be decoded.  For each positio
     bytes = 2 n_kv (pos + 1) 128 * 2 (K and V rows read) + q / k / v / out, against the 3.35 TB/s data sheet,
   - at pos 8191 also the one-CTA-per-head kernel on cache_len 8192 caches, the same way,
   - the GPU name, power limit and median SM clock over the run (read-only nvidia-smi queries).
-With --kv-bits 16,8 one model per cache kind is built in the same process and the kinds alternate at every position; for the 8-bit
-cache (HQQ 8-bit rows, groups of --kv-group-size) the attention bytes are levels plus scale and zero.  kv_cache_bytes() of each
+With --kv-bits 16,8,4 one model per cache kind is built in the same process and the kinds alternate at every position; for the 8- and
+4-bit caches (HQQ rows, groups of --kv-group-size) the attention bytes are levels plus scale and zero.  kv_cache_bytes() of each
 model is printed first.
 
-    python tools/long_context_step.py [--steps 50] [--positions 1024,8191,...] [--kv-bits 16,8]"""
+    python tools/long_context_step.py [--steps 50] [--positions 1024,8191,...] [--kv-bits 16,8,4] [--kv-group-size 64]"""
 import argparse
 import json
 import os
@@ -82,9 +82,9 @@ def main():
             for n in ("k", "v"):
                 c = blk[n + "_cache"]
                 for i in range(0, c.shape[2], 16384):
-                    rows = torch.randn(c[:, :, i:i + 16384].shape, generator=g, device=dev, dtype=torch.float32).mul_(0.5).half()
-                    if kb == 8:
-                        lv, sc, ze = harness.kv8_quantize_rows(rows, args.kv_group_size)
+                    rows = torch.randn(c[:, :, i:i + 16384].shape[:-1] + (hd,), generator=g, device=dev, dtype=torch.float32).mul_(0.5).half()
+                    if kb != 16:
+                        lv, sc, ze = harness.kv8_quantize_rows(rows, args.kv_group_size, kb)
                         c[:, :, i:i + 16384].copy_(lv)
                         blk[n + "_scale"][:, :, i:i + 16384].copy_(sc)
                         blk[n + "_zero"][:, :, i:i + 16384].copy_(ze)
@@ -94,7 +94,7 @@ def main():
         for t in (model._bufs["q"], model._bufs["k"], model._bufs["v"]):
             t.copy_(torch.randn(t.shape, generator=g, device=dev))
         models[kb] = model
-        print(json.dumps({"kv_bits": kb, "kv_group_size": args.kv_group_size if kb == 8 else None, "kv_cache_bytes": model.kv_cache_bytes(), **info}),
+        print(json.dumps({"kv_bits": kb, "kv_group_size": args.kv_group_size if kb != 16 else None, "kv_cache_bytes": model.kv_cache_bytes(), **info}),
               flush=True)
     code = DTYPE_CODE[torch.float16]
     small = None
@@ -124,7 +124,7 @@ def main():
                 for blk in model.blocks:
                     model._attn_split(lib, blk, hq, hkv, code, stream_ptr(dev))
             ms = time_graph(dev, split) / len(model.blocks)
-            row = hd * 2 if kb == 16 else hd + 4 * (hd // args.kv_group_size)  # bytes of one cached row of one kv head
+            row = hd * 2 if kb == 16 else hd * kb // 8 + 4 * (hd // args.kv_group_size)  # bytes of one cached row of one kv head
             nbytes = 2 * hkv * (pos + 1) * row + (2 * hq + 2 * hkv) * hd * 2
             line = {"pos": pos, "kv_bits": kb, "cache_len": args.cache_len, "step_ms": round(step_ms, 4), "tok_s": round(1e3 / step_ms, 2),
                     "steps_timed": args.steps, "attn_kernel": model.attn_kernel, "attn_us_per_launch": round(ms * 1e3, 2),

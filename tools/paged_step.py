@@ -7,7 +7,7 @@ alternately.  For each --kv-bits it prints JSON lines with
   - "fork": the same for 32 slots forked from one 4096-token prefix (one prefill, 31 forks);
   - the GPU name, power limit and median SM clock over the run (read-only nvidia-smi queries).
 
-    python tools/paged_step.py [--kv-bits 16,8] [--steps 20] [--reps 3]"""
+    python tools/paged_step.py [--kv-bits 16,8,4] [--kv-group-size 64] [--steps 20] [--reps 3]"""
 import argparse
 import json
 import os
@@ -78,7 +78,8 @@ def measure(m, dev, pos, steps, fork_from=None):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--kv-bits", default="16,8")
+    ap.add_argument("--kv-bits", default="16,8", help="any of 16, 8 and 4")
+    ap.add_argument("--kv-group-size", type=int, default=64)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--reps", type=int, default=3)
     args = ap.parse_args()
@@ -99,7 +100,7 @@ def main():
         models = {}
         for name, kw in (("contiguous", {}), ("paged", {"kv_pages": n_pages})):
             m = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=L, fused=True, batch=B, kv_bits=kb,
-                                    ragged=True, **kw)
+                                    kv_group_size=args.kv_group_size, ragged=True, **kw)
             m.capture(warmup=2)
             models[name] = m
         res = {name: {"positions": [], "fork": [], "prefill": []} for name in models}

@@ -7,13 +7,15 @@ prompt length it prints one JSON line with
     T, 128], k / v expanded to 32 heads; the same positions attended, so the same FLOPs),
   - the GPU name, power limit and median SM clock over the run (read-only nvidia-smi queries).
 A last line times 8192 one-token decode steps from position 0 (the captured step), the other way to take in an 8192-token prompt.
-With --kv-bits 16,8 one model per cache kind is built in the same process and the kinds alternate at every prompt length; for the
-8-bit cache the attention launches read the staging pair, and the staging dequantisation (rows [0, pos0) of every layer and chunk,
-hqq_b200_dequantize) is timed the same way and reported as its share of the prefill.  kv_cache_bytes() of each model is printed, and
-at the end the relative L2 of the two kinds' last-position logits after one --logits-prompt-token prompt, in fp16 and in bf16.
+With --kv-bits 16,8,4 one model per cache kind is built in the same process and the kinds alternate at every prompt length; for the
+8- and 4-bit caches (groups of --kv-group-size) the attention launches read the staging pair, and the staging dequantisation (rows
+[0, pos0) of every layer and chunk: hqq_b200_dequantize for 8 bits, hqq_b200_glue_kv4_stage for 4) is timed the same way and reported
+as its share of the prefill.  kv_cache_bytes() of each model is printed, and at the end the relative L2 of each quantised kind's
+last-position logits against the 16-bit cache's after one --logits-prompt-token prompt, in fp16 and in bf16.
 
-    python tools/prefill_step.py [--lengths 512,2048,...] [--chunk 4096] [--sdpa-max 131072] [--kv-bits 16,8]"""
+    python tools/prefill_step.py [--lengths 512,2048,...] [--chunk 4096] [--sdpa-max 131072] [--kv-bits 16,8,4] [--kv-group-size 64]"""
 import argparse
+import ctypes
 import json
 import os
 import sys
@@ -50,6 +52,7 @@ def main():
     ap.add_argument("--sdpa-max", type=int, default=131072, help="longest prompt the SDPA comparison runs on")
     ap.add_argument("--decode-steps", type=int, default=8192)
     ap.add_argument("--kv-bits", default="16")
+    ap.add_argument("--kv-group-size", type=int, default=64)
     ap.add_argument("--logits-prompt", type=int, default=4096, help="with two cache kinds: their last-position logits after a prompt this long")
     args = ap.parse_args()
     dev = torch.device("cuda", 0)
@@ -58,7 +61,8 @@ def main():
     shape = harness.LLAMA31_8B
     models = {}
     for kb in [int(x) for x in args.kv_bits.split(",")]:
-        models[kb] = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=args.cache_len, fused=5, kv_bits=kb)
+        models[kb] = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=torch.float16, device=dev, cache_len=args.cache_len, fused=5, kv_bits=kb,
+                                         kv_group_size=args.kv_group_size)
         models[kb].capture(warmup=2)
         print(json.dumps({"kv_bits": kb, "kv_cache_bytes": models[kb].kv_cache_bytes(), **info}), flush=True)
     model = models[min(models)]
@@ -79,7 +83,7 @@ def main():
             qr = torch.randn(min(T, args.chunk), hq * hd, generator=g, device=dev).half()
             out = torch.empty_like(qr)
             chunks = [(c0, min(args.chunk, T - c0)) for c0 in range(0, T, args.chunk)]
-            kc, vc = m._kv8_stage if kb == 8 else (None, None)
+            kc, vc = m._kv8_stage if kb != 16 else (None, None)
 
             def attention():
                 for c0, n in chunks:
@@ -93,12 +97,17 @@ def main():
                     "prompt_tok_s": round(T / total_ms * 1e3, 1), "attn_ms": round(attn_ms, 2), "rest_ms": round(total_ms - attn_ms, 2),
                     "attn_share": round(attn_ms / total_ms, 3), "attn_tflops": round(flops / attn_ms / 1e9, 1),
                     "attn_frac_of_989": round(flops / attn_ms / 1e9 / PEAK_TFLOPS, 3)}
-            if kb == 8:  # the staging dequantisation of rows [0, c0) the prefill ran before each chunk's attention
+            if kb != 16:  # the staging dequantisation of rows [0, c0) the prefill ran before each chunk's attention
                 def staging():
                     for c0, n in chunks:
                         if c0 == 0:
                             continue
                         for blk in m.blocks:
+                            if kb == 4:
+                                check(lib.hqq_b200_glue_kv4_stage(*[ptr(blk[c]) for c in ("k_cache", "k_scale", "k_zero", "v_cache", "v_scale", "v_zero")],
+                                                                  ptr(kc), ptr(vc), (ctypes.c_int * 1)(c0), (ctypes.c_int * 1)(n), hkv, args.cache_len, hd,
+                                                                  m.kv_group_size, 1, code, stream_ptr(dev)))
+                                continue
                             for h in range(hkv):
                                 for c, dst in (("k", kc), ("v", vc)):
                                     check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][0, h]), ptr(blk[c + "_scale"][0, h]), ptr(blk[c + "_zero"][0, h]),
@@ -130,21 +139,24 @@ def main():
     clocks = sampler.stop()
     print(json.dumps({"clocks": clocks, **info}), flush=True)
     if args.logits_prompt and len(models) > 1:
-        # last-position logits of the 8-bit cache against the fp16 / bf16 cache after the same prompt, same weights (seed)
+        # last-position logits of each quantised cache against the fp16 / bf16 cache after the same prompt, same weights (seed)
         del models, model
         torch.cuda.empty_cache()
         prompt = torch.randint(0, shape.vocab, (1, args.logits_prompt), generator=g, device=dev)
         for dt in (torch.float16, torch.bfloat16):
             logits = {}
-            for kb in (16, 8):
-                m = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=dt, device=dev, cache_len=args.logits_prompt, fused=5, kv_bits=kb)
+            kinds = sorted({16} | {int(x) for x in args.kv_bits.split(",")}, reverse=True)
+            for kb in kinds:
+                m = harness.DecodeModel(shape, nbits=4, group_size=64, dtype=dt, device=dev, cache_len=args.logits_prompt, fused=5, kv_bits=kb,
+                                        kv_group_size=args.kv_group_size)
                 m.prefill(prompt, chunk=args.chunk)
                 logits[kb] = m.last_logits.float().clone()
                 del m
                 torch.cuda.empty_cache()
-            rel = float((logits[8] - logits[16]).norm() / logits[16].norm())
-            print(json.dumps({"logits_prompt": args.logits_prompt, "dtype": str(dt).split(".")[-1], "kv8_vs_kv16_logits_rel_l2": rel,
-                              "same_argmax": bool(torch.equal(logits[8].argmax(-1), logits[16].argmax(-1))), **info}), flush=True)
+            for kb in kinds[1:]:
+                rel = float((logits[kb] - logits[16]).norm() / logits[16].norm())
+                print(json.dumps({"logits_prompt": args.logits_prompt, "dtype": str(dt).split(".")[-1], f"kv{kb}_vs_kv16_logits_rel_l2": rel,
+                                  "same_argmax": bool(torch.equal(logits[kb].argmax(-1), logits[16].argmax(-1))), **info}), flush=True)
 
 
 if __name__ == "__main__":
