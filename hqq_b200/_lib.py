@@ -107,6 +107,8 @@ SIGNATURES = {
     "hqq_b200_glue_argmax_key": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_argmax_tp": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "hqq_b200_glue_sample": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_void_p, c_void_p, c_int, c_void_p]),
+    "hqq_b200_glue_sample_pos": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_int, c_float, ctypes.c_uint64, c_int, c_void_p, c_void_p, c_void_p,
+                                         c_int, c_void_p]),
     "hqq_b200_launch_count": (c_int64, []),
     "hqq_b200_launch_count_reset": (None, []),
     "hqq_b200_reload_env": (None, []),

@@ -2125,10 +2125,28 @@ __device__ __forceinline__ unsigned long long warp_bin_sum(const unsigned long l
   return s;
 }
 
-template <typename T>
+// A row's Philox counter words: word 1 in w1, words 2 and 3 returned as one 64-bit value (word 0 is i / 4).  StepKeys (hqq_b200_glue_sample):
+// (row, *counter).  PosKeys (hqq_b200_glue_sample_pos): row r is slot r / T at position pos[slot] + r % T, giving (slot, position,
+// 0x80000000 | seq[slot] & 0x7FFFFFFF).
+struct StepKeys { const unsigned long long* counter; };
+struct PosKeys { const long long* pos; const long long* seq; int T; };
+
+__device__ __forceinline__ unsigned long long sample_counter(StepKeys k, uint32_t row, uint32_t& w1) {
+  w1 = row;
+  return __ldg(k.counter);
+}
+
+__device__ __forceinline__ unsigned long long sample_counter(PosKeys k, uint32_t row, uint32_t& w1) {
+  const uint32_t slot = row / (uint32_t)k.T;
+  const uint32_t p = (uint32_t)(__ldg(k.pos + slot) + (long long)(row - slot * (uint32_t)k.T));
+  w1 = slot;
+  return (unsigned long long)(0x80000000u | ((uint32_t)__ldg(k.seq + slot) & 0x7FFFFFFFu)) << 32 | p;
+}
+
+template <typename T, typename Keys>
 __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __restrict__ logits, int n, long long ld, float temperature, int top_k,
-                                                                float top_p, uint32_t seed_lo, uint32_t seed_hi,
-                                                                const unsigned long long* __restrict__ counter, long long* __restrict__ out) {
+                                                                float top_p, uint32_t seed_lo, uint32_t seed_hi, Keys keys,
+                                                                long long* __restrict__ out) {
   __shared__ unsigned cnt_hi[256], cnt_lo[256];
   __shared__ unsigned long long mass_hi[256], mass_lo[256], best_lo[256], red[32];
   __shared__ unsigned max_key;
@@ -2142,7 +2160,8 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __re
   if (tid == 0) { max_key = 0; sel_bin = 0; sel_above = 0; }
   pdl_launch_dependents();
   pdl_wait();
-  const unsigned long long ctr = *counter;
+  uint32_t word1;
+  const unsigned long long ctr = sample_counter(keys, row, word1);  // counter words 2, 3
   __syncthreads();
   auto each = [&](auto&& f) {
     for (int i = tid * 8; i < n; i += kSampleThreads * 8) {
@@ -2250,7 +2269,7 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __re
     if (__fadd_rn(lt, kGumbelMax) < best_r) return;
     if ((long long)(i >> 2) != pq) {
       pq = i >> 2;
-      ph[0] = (uint32_t)pq; ph[1] = row; ph[2] = (uint32_t)ctr; ph[3] = (uint32_t)(ctr >> 32);
+      ph[0] = (uint32_t)pq; ph[1] = word1; ph[2] = (uint32_t)ctr; ph[3] = (uint32_t)(ctr >> 32);
       philox4x32_10(ph, seed_lo, seed_hi);
     }
     const int wi = i & 3;
@@ -3223,10 +3242,9 @@ extern "C" int hqq_b200_glue_spec_accept(const int64_t* targets, const int64_t* 
                     batch, K, cache_len);
 }
 
-extern "C" int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
-                                    const uint64_t* counter, int64_t* out, int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_sample";
-  HQQ_REQUIRE(logits && counter && out, HQQ_E_INVALID, "%s: null pointer", name);
+template <typename Keys>
+static int sample_launch(const char* name, const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
+                         Keys keys, int64_t* out, int dtype, void* stream) {
   HQQ_REQUIRE(dtype == HQQ_F16 || dtype == HQQ_BF16, HQQ_E_INVALID, "%s: dtype must be f16/bf16", name);
   HQQ_REQUIRE(temperature > 0.0f && temperature <= 3.40282347e38f, HQQ_E_INVALID, "%s: temperature must be finite and > 0 (got %g)", name, (double)temperature);
   HQQ_REQUIRE(top_k >= 0, HQQ_E_INVALID, "%s: top_k must be >= 0 (got %d)", name, top_k);
@@ -3238,10 +3256,27 @@ extern "C" int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows,
   cudaStream_t st = (cudaStream_t)stream;
   auto go = [&](auto t) {
     using E = decltype(t);
-    return launch_pdl("sample", sample_kernel<E>, dim3((unsigned)rows), dim3(kSampleThreads), 0, st, (const E*)logits, n, (long long)ld, temperature, top_k,
-                      top_p, (uint32_t)seed, (uint32_t)(seed >> 32), (const unsigned long long*)counter, (long long*)out);
+    return launch_pdl("sample", sample_kernel<E, Keys>, dim3((unsigned)rows), dim3(kSampleThreads), 0, st, (const E*)logits, n, (long long)ld, temperature,
+                      top_k, top_p, (uint32_t)seed, (uint32_t)(seed >> 32), keys, (long long*)out);
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
+                                    const uint64_t* counter, int64_t* out, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_sample";
+  HQQ_REQUIRE(logits && counter && out, HQQ_E_INVALID, "%s: null pointer", name);
+  return sample_launch(name, logits, n, ld, rows, temperature, top_k, top_p, seed, StepKeys{(const unsigned long long*)counter}, out, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_sample_pos(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
+                                        int rows_per_slot, const int64_t* pos, const int64_t* seq, int64_t* out, int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_sample_pos";
+  HQQ_REQUIRE(logits && pos && seq && out, HQQ_E_INVALID, "%s: null pointer", name);
+  HQQ_REQUIRE(rows_per_slot >= 1 && rows_per_slot <= 8 && rows % rows_per_slot == 0, HQQ_E_INVALID,
+              "%s: needs 1 <= rows_per_slot <= 8 dividing rows (rows_per_slot=%d rows=%d)", name, rows_per_slot, rows);
+  return sample_launch(name, logits, n, ld, rows, temperature, top_k, top_p, seed, PosKeys{(const long long*)pos, (const long long*)seq, rows_per_slot},
+                       out, dtype, stream);
 }
 
 #ifndef HQQ_EMU

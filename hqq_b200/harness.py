@@ -134,18 +134,29 @@ def _mulhilo32(a: torch.Tensor, m: int):
     return (p1 >> 16) + (s >> 32), s & _U32
 
 
+def position_counter(pos: torch.Tensor, seq: torch.Tensor) -> torch.Tensor:
+    """Counter words 2 and 3 of hqq_b200_glue_sample_pos for rows at positions pos of sequences seq (int64 [rows] each): int64
+    [rows, 2] = (pos & 0xFFFFFFFF, 0x80000000 | (seq & 0x7FFFFFFF)), for philox_uniforms / sample_tokens with the row's slot as b."""
+    return torch.stack((pos.to(torch.int64) & _U32, (seq.to(torch.int64) & 0x7FFFFFFF) | 0x80000000), dim=-1)
+
+
 def philox_uniforms(n: int, rows: int, seed: int, counter, device=None) -> torch.Tensor:
     """The race's uniforms of hqq_b200_glue_sample on framework ops: u [rows, n] in float64, u[b, i] = ((x >> 9) + 0.5) * 2^-23 with x
     word i % 4 of Philox4x32-10 under key (seed & 0xFFFFFFFF, seed >> 32) and counter (i / 4, b, ctr & 0xFFFFFFFF, ctr >> 32).
-    counter: a python int or an int64 tensor of one element (read on the device, so a captured graph sees it advance)."""
+    counter: a python int or an int64 tensor of one element (read on the device, so a captured graph sees it advance); or an int64
+    tensor [rows, 2] of per-row counter words 2 and 3 (position_counter: hqq_b200_glue_sample_pos's keys, row b being slot b)."""
     if not torch.is_tensor(counter):
         counter = torch.tensor([int(counter)], dtype=torch.int64, device=device)
     device = counter.device
-    ctr = counter.reshape(1, 1).to(torch.int64)
     nq = -(-n // 4)
     c0 = torch.arange(nq, dtype=torch.int64, device=device).view(1, nq).expand(rows, nq)
     c1 = torch.arange(rows, dtype=torch.int64, device=device).view(rows, 1).expand(rows, nq)
-    c2, c3 = (ctr & _U32).expand(rows, nq), ((ctr >> 32) & _U32).expand(rows, nq)
+    if counter.dim() == 2:
+        w = counter.to(torch.int64) & _U32
+        c2, c3 = w[:, :1].expand(rows, nq), w[:, 1:].expand(rows, nq)
+    else:
+        ctr = counter.reshape(1, 1).to(torch.int64)
+        c2, c3 = (ctr & _U32).expand(rows, nq), ((ctr >> 32) & _U32).expand(rows, nq)
     k0, k1 = int(seed) & _U32, (int(seed) >> 32) & _U32
     for r in range(10):
         if r:
@@ -159,7 +170,8 @@ def philox_uniforms(n: int, rows: int, seed: int, counter, device=None) -> torch
 
 def sample_tokens(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, seed: int, counter) -> torch.Tensor:
     """hqq_b200_glue_sample restated on framework ops in float64 (the definition is in include/hqq_b200.h): logits [rows, n] in
-    fp16 / bf16, row b sampled with Philox counter (., b, counter); returns int64 [rows].  temperature and top_p are taken at fp32
+    fp16 / bf16, row b sampled with Philox counter (., b, counter), counter as philox_uniforms takes it (per-row words 2 and 3
+    restate hqq_b200_glue_sample_pos); returns int64 [rows].  temperature and top_p are taken at fp32
     precision, as the kernel receives them.  Top-k compares the 16-bit values as stored.  The reference generator's
     torch.where(logits < pivot, -inf, logits) on fp16(logits / T) can merge neighbouring values by that rounding; here they stay
     apart, so its keep set can be larger than ours at the pivot."""
@@ -386,7 +398,8 @@ class DecodeModel:
                  device="cuda", cache_len: int = 256, tp: int = 1, rank: int = 0, seed: int = 0, process_group=None,
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
                  kv_bits: int = 16, kv_group_size: int | None = None, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
-                 top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None, spec_k: int | None = None):
+                 top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None, spec_k: int | None = None,
+                 sample_keys: str = "step"):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
         # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
         # top-k, top-p, then a Gumbel race on Philox numbers keyed by sample_seed and countered by _sample_ctr -- instead of the argmax.
@@ -401,6 +414,15 @@ class DecodeModel:
         if not (isinstance(sample_seed, int) and 0 <= sample_seed < 2 ** 64):
             raise ValueError(f"sample_seed must be an int in [0, 2^64) (got {sample_seed!r})")
         self.do_sample, self.temperature, self.top_k, self.top_p, self.sample_seed = bool(do_sample), float(temperature), int(top_k), float(top_p), int(sample_seed)
+        # sample_keys "position" (do_sample): the token drawn from the row at position p of slot b takes the Philox numbers keyed by
+        # (b, p, seq[b]) (hqq_b200_glue_sample_pos), seq the slot's sequence number.  A sequence's token at a position then draws the
+        # same numbers in decode(), prefill() and decode_spec(), and does not depend on when other slots were refilled; this is what
+        # lets sampling and speculative decoding combine.  "step" (the default): the counter _sample_ctr, + 1 per sampling call.
+        if sample_keys not in ("step", "position"):
+            raise ValueError(f"sample_keys must be 'step' or 'position' (got {sample_keys!r})")
+        if sample_keys == "position" and not self.do_sample:
+            raise ValueError("sample_keys='position' needs do_sample=True")
+        self.position_keys = sample_keys == "position"
         # kv_bits 8: every layer's K and V cache in HQQ's 8-bit format (kv8_quantize_rows), groups of kv_group_size along the head dim;
         # kv_bits 4: HQQ's 4-bit format, each row's levels packed by 4bit_u8 (kv8_quantize_rows(..., bits=4)), groups of 32 or 64.
         # kv_group_size defaults to 64 for the 8-bit cache; the 4-bit cache takes it explicitly: at 4 bits the group size is the
@@ -441,14 +463,15 @@ class DecodeModel:
             if not self.ragged:
                 raise ValueError("kv_pages needs ragged=True")
             self.pages = PageAllocator(kv_pages, self.batch, cache_len)
-        # spec_k K (ragged, greedy): decode_spec() verifies the window [tok, d1 .. dK] of every slot in one captured pass and emits
-        # the accepted drafts plus one target (include/hqq_b200.h states the rule); the drafts come from prompt lookup over the
-        # device token history `hist` [batch, cache_len] or from the caller.
+        # spec_k K (ragged): decode_spec() verifies the window [tok, d1 .. dK] of every slot in one captured pass and emits the
+        # accepted drafts plus one target (include/hqq_b200.h states the rule); the drafts come from prompt lookup over the device
+        # token history `hist` [batch, cache_len] or from the caller.  The targets are the rows' greedy picks, or with do_sample and
+        # position keys their sampled tokens: for one-token drafts, accepting while draft == target is exact speculative sampling.
         self.spec_k = spec_k
         if spec_k is not None:
             if not self.ragged:
                 raise ValueError("spec_k needs ragged=True")
-            if do_sample:
+            if do_sample and not self.position_keys:
                 raise ValueError("spec_k verifies greedy targets: it cannot be combined with do_sample")
             if not (isinstance(spec_k, int) and 1 <= spec_k <= 7):
                 raise ValueError(f"spec_k must be an int in [1, 7] (got {spec_k!r})")
@@ -527,6 +550,8 @@ class DecodeModel:
         self._slot_idx = torch.arange(self.batch, device=self.device)
         self.next_tok = torch.zeros(self.batch, dtype=torch.long, device=self.device)
         self._sample_ctr = torch.zeros(1, dtype=torch.long, device=self.device)  # Philox counter: + 1 per sampled token
+        # position keys: slot b's sequence number, + 1 when a prefill starts the slot at position 0, copied by fork()
+        self.seq = torch.zeros(self.batch, dtype=torch.long, device=self.device) if self.position_keys else None
         if kv_pages is not None:
             self.page_table = torch.full((self.batch, cache_len // KV_PAGE), kv_pages, dtype=torch.int32, device=self.device)
         if spec_k is not None:  # hist[b][p] = the token fed at position p; the verify step's static I/O
@@ -585,7 +610,7 @@ class DecodeModel:
 
     def fork(self, src: int, dst: int):
         """kv_pages: slot dst continues slot src -- dst is released, then shares src's full pages below pos[src] (stored once) and
-        gets a copy of the partial page in every layer; pos and tok are copied.  Neither slot ever writes a shared page."""
+        gets a copy of the partial page in every layer; pos and tok (and with position keys seq) are copied.  Neither slot ever writes a shared page."""
         self._paged_only("fork")
         src, dst = int(src), int(dst)
         if not (0 <= src < self.batch and 0 <= dst < self.batch):
@@ -593,6 +618,8 @@ class DecodeModel:
         self._apply_pages(self.pages.fork(src, dst))
         self.pos[dst].copy_(self.pos[src])
         self.tok[dst].copy_(self.tok[src])
+        if self.seq is not None:
+            self.seq[dst].copy_(self.seq[src])
         if self.spec_k is not None:
             self.hist[dst].copy_(self.hist[src])
 
@@ -711,7 +738,7 @@ class DecodeModel:
         h = F.rms_norm(h, (s.hidden,), self.final_norm, s.rms_eps)
         logits = torch.matmul(h, self.lm_head.t())
         if self.do_sample:
-            self.next_tok.copy_(self._sample_ref(logits))
+            self.next_tok.copy_(self._sample_ref(logits, self.pos.expand(B)))
             self._sample_ctr.add_(1)
         elif self.tp > 1:  # vocabulary shards: the global maximum, then the lowest global index that attains it (two small all-reduces)
             val, idx = torch.max(logits.float(), dim=-1)
@@ -741,14 +768,15 @@ class DecodeModel:
         """kv_bits 8 / 4 on framework ops: the dequantised K and V cache rows [0, end)."""
         return tuple(kv8_dequantize(blk[n + "_cache"][:, :, :end], blk[n + "_scale"][:, :, :end], blk[n + "_zero"][:, :, :end], self.kv_bits) for n in ("k", "v"))
 
-    def _sample_ref(self, logits):
+    def _sample_ref(self, logits, pos=None):
         """do_sample on framework ops (fused=False): sample_tokens on the full-vocabulary rows (under tensor parallelism every rank
-        gathers the shards and draws the same tokens)."""
+        gathers the shards and draws the same tokens).  Row b is slot b; with position keys pos [rows] holds the rows' positions."""
         if self.tp > 1:
             g = torch.empty(self.tp * logits.shape[0], logits.shape[1], dtype=logits.dtype, device=logits.device)
             torch.distributed.all_gather_into_tensor(g, logits.contiguous(), group=self.pg)
             logits = g.view(self.tp, -1, self.vocab_shard).transpose(0, 1).reshape(-1, self.shape.vocab)
-        return sample_tokens(logits, self.temperature, self.top_k, self.top_p, self.sample_seed, self._sample_ctr)
+        ctr = position_counter(pos, self.seq) if self.position_keys else self._sample_ctr
+        return sample_tokens(logits, self.temperature, self.top_k, self.top_p, self.sample_seed, ctr)
 
     def _sample_buffers(self, rows):
         """What _sample_rows needs for `rows` sequences: the all-gather target under tensor parallelism, and padded rows where the
@@ -779,11 +807,25 @@ class DecodeModel:
         rows[:, :n].view(B, self.tp, self.vocab_shard).copy_(src)
         return rows
 
-    def _sample(self, lib, rows, out, code, st):
-        """One launch of hqq_b200_glue_sample over rows [B, >= vocab]: out[b] = the token of row b at the current _sample_ctr."""
+    def _sample(self, lib, rows, out, code, st, pos=None, T=1):
+        """One launch of hqq_b200_glue_sample over rows [B, >= vocab]: out[b] = the token of row b at the current _sample_ctr.  With
+        position keys hqq_b200_glue_sample_pos instead: row r is slot r / T at position pos[r / T] + r % T (pos: device int64)."""
         from ._lib import check, ptr
+        if self.position_keys:
+            check(lib.hqq_b200_glue_sample_pos(ptr(rows), self.shape.vocab, rows.stride(0), rows.shape[0], self.temperature, self.top_k, self.top_p,
+                                               self.sample_seed, T, ptr(pos), ptr(self.seq), ptr(out), code, st))
+            return
         check(lib.hqq_b200_glue_sample(ptr(rows), self.shape.vocab, rows.stride(0), rows.shape[0], self.temperature, self.top_k, self.top_p,
                                        self.sample_seed, ptr(self._sample_ctr), ptr(out), code, st))
+
+    def _step_pos(self):
+        """Position keys in a captured step: the rows' positions, one per slot (a lock-step model's single position copied to every
+        slot inside the step)."""
+        if self.pos.numel() == self.batch:
+            return self.pos
+        p = self._bufs["sample_pos"]
+        p.copy_(self.pos.expand(self.batch))
+        return p
 
     def _head(self, lib, x, code, st):
         """Final projection + greedy pick inside the captured step: fp16 lm_head through the library GEMV (it is not an HQQ
@@ -795,7 +837,7 @@ class DecodeModel:
         b = self._bufs
         torch.matmul(x, self.lm_head.t(), out=b["logits"])
         if self.do_sample:
-            self._sample(lib, self._sample_rows(b["logits"], b), self.next_tok, code, st)
+            self._sample(lib, self._sample_rows(b["logits"], b), self.next_tok, code, st, pos=self._step_pos() if self.position_keys else None)
             return
         if self.batch > 1:  # a row per sequence: framework ops
             self.next_tok.copy_(self._greedy(b["logits"]))
@@ -970,7 +1012,8 @@ class DecodeModel:
         The prompt runs in chunks of at most `chunk` tokens (batch * chunk <= 65535, the row limit of the rows kernels); each
         chunk goes through every block, writing its rotated k and v into the caches.  Only the last position of each sequence
         goes through the final norm, the lm_head and the argmax (with do_sample: the sampling kernel at the current sample counter,
-        which then advances by one); self.last_logits [batch, vocab / tp] keeps those logits (this rank's vocabulary shard).  Afterwards self.pos = (start + T) mod cache_len -- the steps' own wrap, so a prompt that fills
+        which then advances by one; with position keys at the last prompt position, after a prefill from position 0 has added one
+        to every slot's sequence number seq); self.last_logits [batch, vocab / tp] keeps those logits (this rank's vocabulary shard).  Afterwards self.pos = (start + T) mod cache_len -- the steps' own wrap, so a prompt that fills
         the cache leaves the next step at position 0 as a step at the last position does -- and self.tok [batch] holds the greedy
         (do_sample: the sampled) next token, which is returned: a captured decode step continues from there.
 
@@ -1071,7 +1114,9 @@ class DecodeModel:
                     score["out"][:, c0:c0 + n] = lp[:, :min(n, T - 1 - c0)]
                 if c0 + n == T:
                     h_last, d_last = h.view(B, n, s.hidden)[:, -1].contiguous(), delta.view(B, n, s.hidden)[:, -1].contiguous()
-            tok = self._prefill_head(h_last, d_last)
+            if self.position_keys and start == 0:  # every slot starts a new sequence
+                self.seq.add_(1)
+            tok = self._prefill_head(h_last, d_last, key_pos=[start + T - 1] * B)
         self.tok.copy_(tok)
         self.pos.fill_((start + T) % self.cache_len)
         return self.tok.clone()
@@ -1083,7 +1128,8 @@ class DecodeModel:
         has tokens left (at most 65535 rows in all) and runs them packed in slot order through every block: the linears at
         M = sum of the slots' rows, the _varlen RoPE / append and attention kernels.  With kv_bits 8 the staging rows [0, pos0) are
         dequantised for the slots in the chunk only.  Each slot's last position goes through the final norm, the lm_head and the
-        pick (with do_sample: Philox row index = the slot, the counter advancing by one per call).  Afterwards pos[b] =
+        pick (with do_sample: Philox row index = the slot, the counter advancing by one per call; with position keys the slots
+        whose prompt starts at position 0 first add one to their seq).  Afterwards pos[b] =
         (start_b + T_b) mod cache_len and tok[b] holds the next token for every prefilled slot; tok is returned and last_logits holds
         the prefilled slots' rows in slot order.  Refilling one slot -- continuous batching -- is a prefill with None for every other
         slot: rows past the slot's new position are never read, so its old cache needs no clearing.
@@ -1162,7 +1208,11 @@ class DecodeModel:
                             done[b] += n_tok[b]
                             if done[b] == toks[b].numel():
                                 last[b] = (h[r - 1], delta[r - 1])
-            tok = self._prefill_head(torch.stack([last[b][0] for b in slots]), torch.stack([last[b][1] for b in slots]), slots=slots)
+            if self.position_keys and any(starts[b] == 0 for b in slots):  # those slots start new sequences
+                new = torch.tensor([b for b in slots if starts[b] == 0], device=self.device)
+                self.seq.index_add_(0, new, torch.ones_like(new))
+            key_pos = [starts[b] + int(toks[b].numel()) - 1 if toks[b] is not None else 0 for b in range(B)]
+            tok = self._prefill_head(torch.stack([last[b][0] for b in slots]), torch.stack([last[b][1] for b in slots]), slots=slots, key_pos=key_pos)
         idx = torch.tensor(slots, device=self.device)
         self.tok.index_copy_(0, idx, tok)
         self.pos.index_copy_(0, idx, torch.tensor([(starts[b] + int(toks[b].numel())) % L for b in slots], device=self.device))
@@ -1317,10 +1367,12 @@ class DecodeModel:
                 torch.distributed.all_reduce(delta, group=self.pg)
         return h, delta
 
-    def _prefill_head(self, h, delta, slots=None):
+    def _prefill_head(self, h, delta, slots=None, key_pos=None):
         """Final norm, lm_head and greedy pick for the last position of each sequence: h, delta [batch, hidden].  slots (ragged): h,
-        delta hold the rows of those slots; with do_sample row b is drawn with Philox row index b, its slot."""
+        delta hold the rows of those slots; with do_sample row b is drawn with Philox row index b, its slot.  key_pos: host list of
+        every slot's last prompt position, the position keys' p (slots outside a ragged subset: any value, their draws discarded)."""
         s, B = self.shape, h.shape[0]
+        kp = torch.tensor(key_pos, dtype=torch.long, device=self.device) if self.position_keys else None
 
         def full(lg):  # do_sample on a ragged subset: the rows at their slots in a [batch, vocab / tp] block (the others discarded)
             if slots is None:
@@ -1335,7 +1387,7 @@ class DecodeModel:
             logits = torch.matmul(x, self.lm_head.t())
             self.last_logits = logits
             if self.do_sample:
-                tok = pick(self._sample_ref(full(logits)))
+                tok = pick(self._sample_ref(full(logits), kp))
                 self._sample_ctr.add_(1)
                 return tok
             if self.tp == 1:
@@ -1356,7 +1408,7 @@ class DecodeModel:
         if self.do_sample:
             rows = full(self.last_logits)
             tok = torch.empty(rows.shape[0], dtype=torch.long, device=self.device)
-            self._sample(lib, self._sample_rows(rows, self._sample_buffers(rows.shape[0])), tok, code, st)
+            self._sample(lib, self._sample_rows(rows, self._sample_buffers(rows.shape[0])), tok, code, st, pos=kp)
             self._sample_ctr.add_(1)
             return pick(tok)
         # the argmax kernel reads 16-byte vectors: every row starts on a 16-byte boundary whatever the vocabulary shard's length
@@ -1380,6 +1432,8 @@ class DecodeModel:
                       "key": torch.zeros(1, dtype=torch.long, device=dev)}
         if self.do_sample:
             self._bufs.update(self._sample_buffers(self.batch))
+            if self.position_keys and self.pos.numel() != self.batch:
+                self._bufs["sample_pos"] = torch.zeros(self.batch, dtype=torch.long, device=dev)
         if self.attn_kernel != "single":  # partials + tickets, zeroed once: every launch leaves the tickets at zero
             from ._lib import load
             with torch.cuda.device(dev):
@@ -1414,6 +1468,8 @@ class DecodeModel:
         self.tok.fill_(token)
         self.pos.zero_()
         self._sample_ctr.zero_()
+        if self.seq is not None:
+            self.seq.zero_()
         if self.kv_pages is not None:  # every page free, every entry the sink, every slot active at position 0
             self.pages.reset()
             self.page_table.fill_(self.kv_pages)
@@ -1458,7 +1514,8 @@ class DecodeModel:
     def verify_fused(self):
         """One speculative verify step on the package's kernels: the window [tok, d1 .. dK] of every slot runs the prefill block walk
         (_prefill_chunk_fused) at M = batch (K + 1) rows, with the device-position append and the verify attention as its attention
-        step; every row goes through the final norm and the lm_head, the targets are the rows' greedy picks, and one
+        step; every row goes through the final norm and the lm_head, the targets are the rows' greedy picks (do_sample: one
+        hqq_b200_glue_sample_pos launch over all rows, after one all-gather under tensor parallelism), and one
         hqq_b200_glue_spec_accept launch emits the accepted tokens and advances pos, tok, next_tok and hist on the device."""
         from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
         lib, s = load(), self.shape
@@ -1503,15 +1560,18 @@ class DecodeModel:
         check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(delta), ptr(self.final_norm), ptr(x), B * T, s.hidden, s.rms_eps, code, st))
         logits = self._bufs["verify_logits"]
         torch.matmul(x, self.lm_head.t(), out=logits)
-        self._spec_targets.copy_(self._greedy(logits))
+        if self.do_sample:  # position keys: row b T + t is drawn at position pos[b] + t
+            self._sample(lib, self._sample_rows(logits, self._verify_sample_bufs), self._spec_targets, code, st, pos=self.pos, T=T)
+        else:
+            self._spec_targets.copy_(self._greedy(logits))
         check(lib.hqq_b200_glue_spec_accept(ptr(self._spec_targets), ptr(self._spec_drafts), ptr(self.pos), ptr(self.tok), ptr(self.next_tok),
                                             ptr(self.hist), ptr(self._spec_tokens), ptr(self._spec_n_new), L, K, B, st))
 
     def verify(self):
         """The same verify step on framework ops (fused=False), the reference: per-row RoPE, the window's valid rows (t < n[b]) written
         into the caches (through the page table when paged; kv_bits 8: quantised by kv8_quantize_rows, attention over the
-        dequantised cache), SDPA with the per-slot causal masks key <= pos[b] + t, the head, and
-        the accept rule restated with tensor ops."""
+        dequantised cache), SDPA with the per-slot causal masks key <= pos[b] + t, the head, the targets (do_sample: sample_tokens
+        with the position keys of each row), and the accept rule restated with tensor ops."""
         s, B, K, L = self.shape, self.batch, self.spec_k, self.cache_len
         T = K + 1
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
@@ -1554,7 +1614,10 @@ class DecodeModel:
         h = F.rms_norm(h, (s.hidden,), self.final_norm, s.rms_eps)
         logits = torch.matmul(h, self.lm_head.t())
         self.spec_logits = logits.view(B, T, -1)
-        tg = self._greedy(logits).view(B, T)
+        if self.do_sample:  # position keys: row t of slot b at position pos[b] + t
+            tg = torch.stack([self._sample_ref(self.spec_logits[:, t], self.pos + t) for t in range(T)], dim=1)
+        else:
+            tg = self._greedy(logits).view(B, T)
         d = self._spec_drafts
         ok = (d == tg[:, :K]) & (torch.arange(1, T, device=dev).view(1, K) < n.view(B, 1))
         a = torch.cumprod(ok.long(), dim=1).sum(dim=1)  # accepted drafts
@@ -1589,6 +1652,8 @@ class DecodeModel:
                 nbytes = load().hqq_b200_glue_attn_verify_split_workspace_bytes(s.n_heads // tp, s.n_kv_heads // tp, s.head_dim, T, self.batch)
             self._bufs["verify_ws"] = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
             self._bufs["verify_logits"] = torch.zeros(self.batch * T, self.vocab_shard, dtype=self.dtype, device=self.device)
+            if self.do_sample:
+                self._verify_sample_bufs = self._sample_buffers(self.batch * T)
         self.spec_logits = self._bufs["verify_logits"].view(self.batch, self.spec_k + 1, -1)
         saved = [t.clone() for t in (self.pos, self.tok, self.next_tok, self.hist, self._spec_drafts)]
         self._spec_drafts.fill_(-1)

@@ -568,6 +568,17 @@ int hqq_b200_glue_argmax_tp(const void* logits, int n, int64_t index_offset, voi
  * by one per sampled token).  No workspace, no atomics outside shared memory.  Needs rows <= 65535. */
 int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
                          const uint64_t* counter, int64_t* out, int dtype, void* stream);
+/* Position keys: the same kept set and race, with the random numbers of each token keyed by the slot, the sequence and the
+ * position of the row whose logits are sampled, so that a sequence's token at a given position draws the same numbers whichever
+ * step (one-token decode, prefill, speculative verify) samples it and whatever the other slots do.  Row r of `rows` is slot
+ * b = r / T at position p = pos[b] + r % T (T = rows_per_slot in [1, 8], dividing rows; pos and seq device int64 [rows / T]);
+ * its race uses counter (i / 4, b, p & 0xFFFFFFFF, 0x80000000 | (seq[b] & 0x7FFFFFFF)) under the same key.  The high bit of
+ * the last word keeps these counters apart from every counter of hqq_b200_glue_sample below 2^63.  The token is a function of
+ * (row bits, n, temperature, top_k, top_p, seed, b, p, seq[b]) alone: not of the grid, the row's index in the launch or the
+ * other slots.  The decode harness's seq[b] is a per-slot sequence number: zeroed by a reset, + 1 when a prefill starts the
+ * slot at position 0, copied by a fork.  pos and seq are read, never written. */
+int hqq_b200_glue_sample_pos(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
+                             int rows_per_slot, const int64_t* pos, const int64_t* seq, int64_t* out, int dtype, void* stream);
 
 /* Number of kernels launched by this library on the calling thread since the last reset
  * (used by bench.py for its gpu_launches claim).                                        */
