@@ -313,11 +313,11 @@ __global__ void __launch_bounds__(kAttnThreads) rope_attn_decode_kernel(const T*
 //
 // Each CTA handles all G = n_q / n_kv query heads of its group, so every K/V row crosses HBM once, not G times.  Both products
 // run on mma.sync m16n8k16 with the (at most 8) heads as the n = 8 dimension:
-//   scores^T [16 positions x 8 heads] = K tile [16 x 128] . Q^T       (K from shared memory through ldmatrix, Q^T in registers)
-//   O^T      [128 dims x 8 heads]    += V^T [128 x 16] . P^T           (V^T through ldmatrix.trans, P^T from the score fragments)
-// Each of the 8 warps streams the 16-position tiles w, w+8, ... of its CTA's chunk through a private 3-stage cp.async ring
-// (16 KB per warp: K then V, 16-byte chunks XOR-swizzled by row so ldmatrix is conflict-free) and keeps an online softmax in
-// fp32; P is rounded to T for the MMA and the row sum adds the rounded values.  The warps meet in shared memory in warp order,
+//   scores^T [16 positions x 8 heads] = K tile [16 x 128] . Q^T       (K from shared memory, Q^T in registers)
+//   O^T      [128 dims x 8 heads]    += V^T [128 x 16] . P^T           (V^T from shared memory, P^T from the score fragments)
+// Each of the 8 warps streams the 16-position tiles w, w+8, ... of its CTA's chunk through a private cp.async ring (its stages and
+// their layout depend on the cache format: 16-bit, or HQQ 8- or 4-bit levels dequantised into the MMA fragments) and keeps an online
+// softmax in fp32; P is rounded to T for the MMA and the row sum adds the rounded values.  The warps meet in shared memory in warp order,
 // the CTA publishes its partial (m, l, o[G][128]) to the workspace, and the last CTA of a (sequence, kv head) -- found with a
 // fence and a ticket -- combines the S partials in split order, writes out with one rounding to T and resets the ticket.
 //
@@ -335,9 +335,7 @@ constexpr int kHd = 128;
 constexpr int kTileBytes = kSplitTile * kHd * 2;                          // one K or V tile, 4 KB
 constexpr int kStageBytes = 2 * kTileBytes;
 constexpr int kRingBytes = kSplitWarps * kSplitStages * kStageBytes;      // 192 KB
-constexpr int kSmemBytes = kRingBytes + (kSplitMaxGroup + 2) * kHd * 2 + 16;  // + rotated q [8][128], fresh k, v + the last-CTA flag
 constexpr int kPartFloats = kHd + 2;                                      // per head: m, l, o[128]
-static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kRingBytes, "the warp partials reuse the ring");
 
 template <typename T> __device__ __forceinline__ uint32_t bits16(T v) { return (uint32_t)*reinterpret_cast<const unsigned short*>(&v); }
 
@@ -400,214 +398,95 @@ __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], 
 #endif
 }
 
+// x*cos + rotate_half(x)*sin at dim d of the head row x, with the cos / sin rows of its position: each product and the sum rounded
+// to T, as rope_attn_decode_kernel rounds them (a cache row written by any kernel is bit for bit the row a decode step writes)
 template <typename T>
-__device__ __forceinline__ void split_merge(const float* wp, float* __restrict__ part, unsigned* __restrict__ tickets, T* __restrict__ out, int* last,
-                                           int S, int split, int G, int tid);
-
-// grid = (S, n_kv, batch), block = 256.  q / out [batch, n_q * 128], k / v [batch, n_kv * 128], caches [batch, n_kv, L, 128].
-// part: [batch, n_kv, S, G, 2 + 128] floats (m, l, o per head), tickets: [batch, n_kv] uint32, zero between launches.
-// SEQPOS: sequence b at its own position pos_p[b]; its chunk, staged rows, RoPE row and written row follow it (S stays fixed).
-// PAGED (SEQPOS only): caches are page pools [pages, n_kv, 64, 128]; a tile's rows are found with one read of the table row.
-template <typename T, bool SEQPOS = false, bool PAGED = false>
-__global__ void __launch_bounds__(kSplitThreads, 1)
-    rope_attn_decode_split_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
-                                  const T* __restrict__ sin_t, T* __restrict__ k_cache, T* __restrict__ v_cache, const long long* __restrict__ pos_p,
-                                  T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
-                                  float scale_log2, const PageArg<PAGED> pg) {
-  extern __shared__ __align__(16) char smem[];
-  constexpr int NW = kSplitWarps, ST = kSplitStages;
-  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
-  const int G = n_q / n_kv;
-  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
-  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
-  const int* tab = nullptr;
-  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
-  {
-    const long long kv = (long long)b * n_kv + kvh;
-    if constexpr (!PAGED) { k_cache += kv * L * kHd; v_cache += kv * L * kHd; }
-    k_in += kv * kHd; v_in += kv * kHd;
-    q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
-    part += kv * S * G * kPartFloats;
-    tickets += kv;
-  }
-  char* ring = smem + warp * ST * kStageBytes;
-  T* qs = reinterpret_cast<T*>(smem + kRingBytes);  // rotated q [8][128]
-  T* kf = qs + kSplitMaxGroup * kHd;                // rotated k and v of position pos
-  T* vf = kf + kHd;
-  int* last = reinterpret_cast<int*>(vf + kHd);
-
-  // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
-  const int pos = (int)pos_p[SEQPOS ? b : 0], n_pos = pos + 1;
-  const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
-  const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
-  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
-  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;  // tiles warp, warp + NW, ... of the chunk
-  pdl_launch_dependents();
-
-  // Stage local tile i into its ring slot: rows < pos from the cache (cp.async), row pos from the rotated k / v of this step once
-  // `fresh` (the cache row is written by another CTA of this launch), rows past pos zero (finite: their probability is 0).
-  auto issue = [&](int i, bool fresh) {
-    if (i < my_tiles) {
-      const int t0 = c0 + (warp + i * NW) * kSplitTile;
-      char* st = ring + (i % ST) * kStageBytes;
-      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
-      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
-#pragma unroll 4
-      for (int j = lane; j < 2 * kSplitTile * 16; j += 32) {
-        const int isv = j >> 8, r = (j >> 4) & 15, c = j & 15, p = t0 + r;
-        char* dst = st + isv * kTileBytes + swz(r, c);
-        if (p < pos) {
-          split_cp16(dst, (isv ? v_cache : k_cache) + (rt + p) * kHd + c * 8);
-        } else if (p > pos || fresh) {
-          uint4 val;
-          val.x = val.y = val.z = val.w = 0u;
-          if (p == pos) val = *reinterpret_cast<const uint4*>((isv ? vf : kf) + c * 8);
-          *reinterpret_cast<uint4*>(dst) = val;
-        }
-      }
-    }
-    split_commit();  // always (possibly empty): every iteration waits on the same group count
-  };
-  // cache rows < pos were written by earlier launches: the first ST - 1 tiles stream in under the previous kernel's tail
-#pragma unroll
-  for (int i = 0; i < ST - 1; ++i) issue(i, false);
-  pdl_wait();
-
-  // RoPE exactly as rope_attn_decode_kernel: x*cos + rotate_half(x)*sin, each product and the sum rounded to T
-  for (int i = tid; i < (G + 1) * kHd; i += kSplitThreads) {
-    const int h = i >> 7, d = i & (kHd - 1), half = kHd / 2;
-    const float c = to_f32<T>(cos_t[(long long)pos * kHd + d]), s = to_f32<T>(sin_t[(long long)pos * kHd + d]);
-    const T* x = h < G ? q_in + h * kHd : k_in;
-    const float xv = to_f32<T>(x[d]);
-    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
-    const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
-    if (h < G) {
-      qs[h * kHd + d] = r;
-    } else {
-      kf[d] = r;
-      vf[d] = v_in[d];
-      if (split == 0) {  // one writer per (sequence, kv head); no CTA of this launch reads cache row pos
-        long long pr = pos;
-        if constexpr (PAGED) pr = page_row(tab, n_kv, kvh, pos);
-        k_cache[pr * kHd + d] = r;
-        v_cache[pr * kHd + d] = v_in[d];
-      }
-    }
-  }
-  __syncthreads();
-  if (pos >= c0 && pos < c1) {  // row pos in a tile staged before the wait: its owner fills it in now
-    const int ti = (pos - c0) / kSplitTile, i = ti / NW;
-    if (ti % NW == warp && i < ST - 1) {
-      const int r = pos - (c0 + ti * kSplitTile), c = lane & 15;
-      *reinterpret_cast<uint4*>(ring + (i % ST) * kStageBytes + (lane >> 4) * kTileBytes + swz(r, c)) =
-          *reinterpret_cast<const uint4*>((lane >> 4 ? vf : kf) + c * 8);
-    }
-  }
-  // Q^T fragments (B operand of the score MMA, n = head g): dims 16 kk + 2 qd + {0, 1} and + 8
-  uint32_t qb[8][2];
-#pragma unroll
-  for (int kk = 0; kk < 8; ++kk) {
-    const T* qr = qs + g * kHd + kk * 16 + 2 * qd;
-    qb[kk][0] = g < G ? *reinterpret_cast<const uint32_t*>(qr) : 0u;
-    qb[kk][1] = g < G ? *reinterpret_cast<const uint32_t*>(qr + 8) : 0u;
-  }
-
-  // lane (g, qd) holds the running max / sum of heads 2 qd, 2 qd + 1 and O^T rows 16 mt + g (+ 8) of those heads
-  float o[8][4];
-#pragma unroll
-  for (int mt = 0; mt < 8; ++mt) o[mt][0] = o[mt][1] = o[mt][2] = o[mt][3] = 0.f;
-  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  const int kr = (lane & 7) + ((lane >> 3) & 1) * 8, kc = lane >> 4;       // ldmatrix row / chunk, K (a0..a3: rows +8, then k +8)
-  const int vr = (lane & 7) + ((lane >> 4) & 1) * 8, vc = (lane >> 3) & 1;  // V^T (a0..a3: dims +8, then positions +8)
-  for (int i = 0; i < my_tiles; ++i) {
-    __syncwarp();  // every lane is done with the slot the next issue overwrites
-    issue(i + ST - 1, true);
-    split_wait<ST - 1>();
-    __syncwarp();  // this tile's copies and plain stores of every lane are visible to the warp
-    const char* kt = ring + (i % ST) * kStageBytes;
-    const char* vt = kt + kTileBytes;
-    float s[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t a[4];
-      ldsm4<false>(a, kt + swz(kr, 2 * kk + kc));
-      mma16816<T>(s, a, qb[kk][0], qb[kk][1]);
-    }
-    const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
-    const float x0 = p0 < c1 ? s[0] * scale_log2 : -INFINITY, x1 = p0 < c1 ? s[1] * scale_log2 : -INFINITY;
-    const float x2 = p0 + 8 < c1 ? s[2] * scale_log2 : -INFINITY, x3 = p0 + 8 < c1 ? s[3] * scale_log2 : -INFINITY;
-    float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
-#pragma unroll
-    for (int off = 4; off < 32; off <<= 1) {
-      t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
-      t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
-    }
-    const float n0 = fmaxf(m0, t0), n1 = fmaxf(m1, t1);  // finite: every tile holds position c0 + 16 j < c1
-    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
-    m0 = n0; m1 = n1;
-    const T p00 = from_f32<T>(exp2f(x0 - n0)), p01 = from_f32<T>(exp2f(x1 - n1));
-    const T p10 = from_f32<T>(exp2f(x2 - n0)), p11 = from_f32<T>(exp2f(x3 - n1));
-    l0 = l0 * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
-    l1 = l1 * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
-#pragma unroll
-    for (int mt = 0; mt < 8; ++mt) { o[mt][0] *= a0; o[mt][1] *= a1; o[mt][2] *= a0; o[mt][3] *= a1; }
-    // P^T fragment (k = position, n = head g): positions 2 qd, 2 qd + 1 (+ 8) sit in lanes (2 qd, g / 2) and (2 qd + 1, g / 2)
-    const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
-    const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
-    const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
-    const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
-    const uint32_t b0 = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
-    const uint32_t b1 = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
-#pragma unroll
-    for (int mt = 0; mt < 8; ++mt) {
-      uint32_t a[4];
-      ldsm4<true>(a, vt + swz(vr, 2 * mt + vc));
-      mma16816<T>(o[mt], a, b0, b1);
-    }
-  }
-  split_wait<0>();
-#pragma unroll
-  for (int off = 4; off < 32; off <<= 1) {
-    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
-  }
-  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][8][m, l, o[128]]
-  float* wp = reinterpret_cast<float*>(smem);
-  {
-    float* w0 = wp + (warp * kSplitMaxGroup + 2 * qd) * kPartFloats;
-    float* w1 = w0 + kPartFloats;
-    if (g == 0) { w0[0] = m0; w0[1] = l0; w1[0] = m1; w1[1] = l1; }
-#pragma unroll
-    for (int mt = 0; mt < 8; ++mt) {
-      w0[2 + 16 * mt + g] = o[mt][0]; w1[2 + 16 * mt + g] = o[mt][1];
-      w0[2 + 16 * mt + g + 8] = o[mt][2]; w1[2 + 16 * mt + g + 8] = o[mt][3];
-    }
-  }
-  __syncthreads();
-  split_merge<T>(wp, part, tickets, out, last, S, split, G, tid);
+__device__ __forceinline__ T rope_rounded(const T* x, int d, const T* cos_row, const T* sin_row) {
+  constexpr int half = kHd / 2;
+  const float c = to_f32<T>(cos_row[d]), s = to_f32<T>(sin_row[d]);
+  const float xv = to_f32<T>(x[d]);
+  const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
+  return from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
 }
 
-// The end of both split kernels, once the warp partials wp [NW][8][m, l, o[128]] are in shared memory: this CTA's partial to the
-// workspace, the ticket, and in the last CTA of the (sequence, kv head) the merge of all S partials into out.
-template <typename T>
-__device__ __forceinline__ void split_merge(const float* wp, float* __restrict__ part, unsigned* __restrict__ tickets, T* __restrict__ out, int* last,
-                                           int S, int split, int G, int tid) {
+// One 16-position tile of the online softmax of the split kernels for lane (g, qd): columns 2 qd, 2 qd + 1 (heads, or the verify
+// kernel's (t, h) columns), scores s of positions p0 and p0 + 8, column u seeing the positions below lim_u.  P is rounded to T for the
+// MMA and l adds the rounded values.  b0, b1: the P^T fragment of the V^T . P^T MMA (k = position, n = column g): positions 2 qd,
+// 2 qd + 1 (+ 8) sit in lanes (2 qd, g / 2) and (2 qd + 1, g / 2).  GUARD: a tile may lie wholly past a column's last key, so a column
+// with no key yet keeps m = -inf, l = 0, o = 0; without it every tile holds a key of every column and the running max is finite.
+template <typename T, bool GUARD>
+__device__ __forceinline__ void softmax_tile(const float (&s)[4], float scale_log2, int p0, int lim0, int lim1, float (&m)[2], float (&l)[2],
+                                             float (&o)[8][4], int g, int qd, uint32_t& b0, uint32_t& b1) {
+  const float x0 = p0 < lim0 ? s[0] * scale_log2 : -INFINITY, x1 = p0 < lim1 ? s[1] * scale_log2 : -INFINITY;
+  const float x2 = p0 + 8 < lim0 ? s[2] * scale_log2 : -INFINITY, x3 = p0 + 8 < lim1 ? s[3] * scale_log2 : -INFINITY;
+  float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
+#pragma unroll
+  for (int off = 4; off < 32; off <<= 1) {
+    t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
+    t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
+  }
+  const float n0 = fmaxf(m[0], t0), n1 = fmaxf(m[1], t1);
+  float r0 = n0, r1 = n1;
+  if constexpr (GUARD) {
+    r0 = n0 == -INFINITY ? 0.f : n0;
+    r1 = n1 == -INFINITY ? 0.f : n1;
+  }
+  const float a0 = exp2f(m[0] - r0), a1 = exp2f(m[1] - r1);
+  m[0] = n0; m[1] = n1;
+  const T p00 = from_f32<T>(exp2f(x0 - r0)), p01 = from_f32<T>(exp2f(x1 - r1));
+  const T p10 = from_f32<T>(exp2f(x2 - r0)), p11 = from_f32<T>(exp2f(x3 - r1));
+  l[0] = l[0] * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
+  l[1] = l[1] * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
+#pragma unroll
+  for (int mt = 0; mt < 8; ++mt) { o[mt][0] *= a0; o[mt][1] *= a1; o[mt][2] *= a0; o[mt][3] *= a1; }
+  const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
+  const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
+  const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
+  const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
+  b0 = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
+  b1 = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
+}
+
+// Lane (g, qd)'s share of its warp's partials of columns 2 qd, 2 qd + 1, w0 pointing at the first one's [m, l, o[128]]: l summed over
+// the lanes of a column, O^T row g (+ 8) of step mt being dim Dims::odim(mt, g, 0 (1)).  Every lane must call it.
+template <class Dims>
+__device__ __forceinline__ void put_partial(float* w0, const float (&m)[2], float (&l)[2], const float (&o)[8][4], int g) {
+#pragma unroll
+  for (int off = 4; off < 32; off <<= 1) {
+    l[0] += __shfl_xor_sync(0xffffffffu, l[0], off);
+    l[1] += __shfl_xor_sync(0xffffffffu, l[1], off);
+  }
+  float* w1 = w0 + kPartFloats;
+  if (g == 0) { w0[0] = m[0]; w0[1] = l[0]; w1[0] = m[1]; w1[1] = l[1]; }
+#pragma unroll
+  for (int mt = 0; mt < 8; ++mt) {
+    w0[2 + Dims::odim(mt, g, 0)] = o[mt][0]; w1[2 + Dims::odim(mt, g, 0)] = o[mt][1];
+    w0[2 + Dims::odim(mt, g, 1)] = o[mt][2]; w1[2 + Dims::odim(mt, g, 1)] = o[mt][3];
+  }
+}
+
+// The end of the split kernels, once the warp partials wp [NW][WC][m, l, o[128]] are in shared memory: this CTA's partial of its nc
+// columns to the workspace part [S][PC][m, l, o[128]], the ticket, and in the last CTA of the group the merge of all S partials into
+// row out_row(c) of column c.
+template <typename T, int WC, typename OutRow>
+__device__ __forceinline__ void split_merge(const float* wp, float* __restrict__ part, unsigned* __restrict__ tickets, int* last, int S, int split,
+                                           int PC, int nc, int tid, OutRow out_row) {
   constexpr int NW = kSplitWarps;
-  // this CTA's partial, warps in order (an empty chunk publishes m = -inf, l = 0, o = 0)
-  for (int i = tid; i < G * kHd; i += kSplitThreads) {
-    const int h = i >> 7, d = i & (kHd - 1);
+  // this CTA's partial, warps in order (an empty chunk, or a column with no key in it, publishes m = -inf, l = 0, o = 0)
+  for (int i = tid; i < nc * kHd; i += kSplitThreads) {
+    const int c = i >> 7, d = i & (kHd - 1);
     float M = -INFINITY;
-    for (int w = 0; w < NW; ++w) M = fmaxf(M, wp[(w * kSplitMaxGroup + h) * kPartFloats]);
+    for (int w = 0; w < NW; ++w) M = fmaxf(M, wp[(w * WC + c) * kPartFloats]);
     float lsum = 0.f, osum = 0.f;
     if (M != -INFINITY) {
       for (int w = 0; w < NW; ++w) {
-        const float* e = wp + (w * kSplitMaxGroup + h) * kPartFloats;
+        const float* e = wp + (w * WC + c) * kPartFloats;
         const float f = exp2f(e[0] - M);
         lsum += f * e[1];
         osum += f * e[2 + d];
       }
     }
-    float* dst = part + ((long long)split * G + h) * kPartFloats;
+    float* dst = part + ((long long)split * PC + c) * kPartFloats;
     if (d == 0) { dst[0] = M; dst[1] = lsum; }
     dst[2 + d] = osum;
   }
@@ -617,19 +496,19 @@ __device__ __forceinline__ void split_merge(const float* wp, float* __restrict__
   __syncthreads();
   if (!*last) return;
   __threadfence();
-  // last CTA of the group: all S partials, split order, one rounding to T
-  for (int i = tid; i < G * kHd; i += kSplitThreads) {
-    const int h = i >> 7, d = i & (kHd - 1);
+  // last CTA of the group: all S partials, split order, one rounding to T.  Split 0 holds key 0, which every column sees: M is finite
+  for (int i = tid; i < nc * kHd; i += kSplitThreads) {
+    const int c = i >> 7, d = i & (kHd - 1);
     float M = -INFINITY;
-    for (int sp = 0; sp < S; ++sp) M = fmaxf(M, __ldcg(part + ((long long)sp * G + h) * kPartFloats));  // split 0 is never empty
+    for (int sp = 0; sp < S; ++sp) M = fmaxf(M, __ldcg(part + ((long long)sp * PC + c) * kPartFloats));
     float lsum = 0.f, osum = 0.f;
     for (int sp = 0; sp < S; ++sp) {
-      const float* e = part + ((long long)sp * G + h) * kPartFloats;
+      const float* e = part + ((long long)sp * PC + c) * kPartFloats;
       const float f = exp2f(__ldcg(e) - M);
       lsum += f * __ldcg(e + 1);
       osum += f * __ldcg(e + 2 + d);
     }
-    out[h * kHd + d] = from_f32<T>(osum / lsum);
+    out_row(c)[d] = from_f32<T>(osum / lsum);
   }
   if (tid == 0) *tickets = 0u;  // ready for the next launch (graph replay needs no memset)
 }
@@ -685,284 +564,6 @@ __device__ __forceinline__ uint32_t kv8_deq2(uint32_t w, typename Pair<T>::type 
   return *reinterpret_cast<const uint32_t*>(&r);
 }
 
-// Split-KV decode attention over an 8-bit cache: rope_attn_decode_split_kernel's grid, chunks, ticket, merge and RoPE.  Each warp
-// streams levels and meta of its 16-position tiles through a 4-stage cp.async ring (4352 bytes a stage: K and V levels [16][128],
-// 16-byte chunks XOR-swizzled by row, then k scale | k zero | v scale | v zero [16][128 / gs]) and dequantises straight into the MMA
-// fragments.  The head dim is permuted, the same way for both operands of a product (so the products are unchanged): lane
-// (g, qd) takes K dims 32 qd .. 32 qd + 31 of positions g, g + 8 (k slot 2 qd + {0, 1, 8, 9} of step kk is dim 32 qd + 4 kk + {0..3})
-// and V dims 16 g .. 16 g + 15 of positions 2 qd + {0, 1, 8, 9} (O^T row g / g + 8 of step mt is dim 16 g + 2 mt / + 1): two
-// 16-byte loads a row, one group each.  Row pos is this launch's quantisation of the fresh k / v in every CTA that holds it; split
-// 0 writes it to the cache.
-constexpr int kKv8Stages = 4;
-constexpr int kKv8LvlBytes = kSplitTile * kHd;                                    // one K or V level tile, 2 KB
-constexpr int kKv8MetaBytes = kSplitTile * 2 * 2;                                 // one meta array of a tile: [16][<= 2] T
-constexpr int kKv8StageBytes = 2 * kKv8LvlBytes + 4 * kKv8MetaBytes;
-constexpr int kKv8RingBytes = kSplitWarps * kKv8Stages * kKv8StageBytes;           // 136 KB
-// + rotated q [8][128] T, fresh k, v [128] T, their levels [2][128] and meta [4][2] T, the last-CTA flag
-constexpr int kKv8SmemBytes = kKv8RingBytes + (kSplitMaxGroup + 2) * kHd * 2 + 2 * kHd + 16 + 16;
-static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kKv8RingBytes, "the warp partials reuse the ring");
-
-__device__ __forceinline__ int swz8(int r, int c) { return r * kHd + ((c ^ (r & 7)) << 4); }  // 16-byte chunk c of level row r
-
-// grid = (S, n_kv, batch), block = 256.  q / out, k / v as rope_attn_decode_split_kernel; levels [batch, n_kv, L, 128] uint8, meta
-// [batch, n_kv, L, 128 / gs] T; part / tickets as there.  SEQPOS and PAGED as there (paged levels [pages, n_kv, 64, 128], meta
-// [pages, n_kv, 64, 128 / gs]).
-template <typename T, bool SEQPOS = false, bool PAGED = false>
-__global__ void __launch_bounds__(kSplitThreads, 1)
-    rope_attn_decode_split_kv8_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
-                                      const T* __restrict__ sin_t, uint8_t* __restrict__ k_q, T* __restrict__ k_s, T* __restrict__ k_z,
-                                      uint8_t* __restrict__ v_q, T* __restrict__ v_s, T* __restrict__ v_z, const long long* __restrict__ pos_p,
-                                      T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
-                                      int gs, float scale_log2, const PageArg<PAGED> pg) {
-  extern __shared__ __align__(16) char smem[];
-  constexpr int NW = kSplitWarps, ST = kKv8Stages;
-  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
-  const int G = n_q / n_kv, ng = kHd / gs;
-  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
-  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
-  const int* tab = nullptr;
-  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
-  {
-    const long long kv = (long long)b * n_kv + kvh;
-    if constexpr (!PAGED) {
-      k_q += kv * L * kHd; v_q += kv * L * kHd;
-      k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
-    }
-    k_in += kv * kHd; v_in += kv * kHd;
-    q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
-    part += kv * S * G * kPartFloats;
-    tickets += kv;
-  }
-  char* ring = smem + warp * ST * kKv8StageBytes;
-  T* qs = reinterpret_cast<T*>(smem + kKv8RingBytes);  // rotated q [8][128]
-  T* kf = qs + kSplitMaxGroup * kHd;                   // rotated k and v of position pos
-  T* vf = kf + kHd;
-  uint8_t* fq = reinterpret_cast<uint8_t*>(vf + kHd);  // their levels: k [128], v [128]
-  T* fm = reinterpret_cast<T*>(fq + 2 * kHd);          // their meta: k scale, k zero, v scale, v zero [2] each
-  int* last = reinterpret_cast<int*>(fm + 8);
-
-  // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
-  const int pos = (int)pos_p[SEQPOS ? b : 0], n_pos = pos + 1;
-  const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
-  const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
-  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
-  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;
-  pdl_launch_dependents();
-
-  // Stage local tile i as rope_attn_decode_split_kernel does: rows < pos from the cache, row pos from this launch's quantisation
-  // once `fresh`, rows past pos zero (levels and meta: they dequantise to 0).  A meta chunk of 16 bytes spans 8 / ng rows; one that
-  // reaches row pos (or sits on a misaligned address) is staged row by row.
-  auto issue = [&](int i, bool fresh) {
-    if (i < my_tiles) {
-      const int t0 = c0 + (warp + i * NW) * kSplitTile;
-      char* st = ring + (i % ST) * kKv8StageBytes;
-      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
-      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
-#pragma unroll 4
-      for (int j = lane; j < 2 * kSplitTile * 8; j += 32) {
-        const int isv = j >> 7, r = (j >> 3) & 15, c = j & 7, p = t0 + r;
-        char* dst = st + isv * kKv8LvlBytes + swz8(r, c);
-        if (p < pos) {
-          split_cp16(dst, (isv ? v_q : k_q) + (rt + p) * kHd + c * 16);
-        } else if (p > pos || fresh) {
-          uint4 val;
-          val.x = val.y = val.z = val.w = 0u;
-          if (p == pos) val = *reinterpret_cast<const uint4*>(fq + isv * kHd + c * 16);
-          *reinterpret_cast<uint4*>(dst) = val;
-        }
-      }
-      if (lane < 8 * ng) {  // 4 arrays x 2 ng chunks
-        const int a = lane / (2 * ng), j = lane % (2 * ng), rows = 8 / ng, r0 = j * rows;
-        const T* src = (a == 0 ? k_s : a == 1 ? k_z : a == 2 ? v_s : v_z) + (rt + (t0 + r0)) * ng;
-        char* dst = st + 2 * kKv8LvlBytes + a * kKv8MetaBytes + j * 16;
-        if (t0 + r0 + rows <= pos && ((uintptr_t)src & 15) == 0) {
-          split_cp16(dst, src);
-        } else {
-          for (int e = 0; e < 8; ++e) {
-            const int p = t0 + r0 + e / ng;
-            if (p < pos) reinterpret_cast<T*>(dst)[e] = src[e];
-            else if (p > pos) reinterpret_cast<T*>(dst)[e] = from_f32<T>(0.f);
-            else if (fresh) reinterpret_cast<T*>(dst)[e] = fm[2 * a + e % ng];
-          }
-        }
-      }
-    }
-    split_commit();  // always (possibly empty): every iteration waits on the same group count
-  };
-#pragma unroll
-  for (int i = 0; i < ST - 1; ++i) issue(i, false);
-  pdl_wait();
-
-  // RoPE exactly as rope_attn_decode_kernel: x*cos + rotate_half(x)*sin, each product and the sum rounded to T
-  for (int i = tid; i < (G + 1) * kHd; i += kSplitThreads) {
-    const int h = i >> 7, d = i & (kHd - 1), half = kHd / 2;
-    const float c = to_f32<T>(cos_t[(long long)pos * kHd + d]), s = to_f32<T>(sin_t[(long long)pos * kHd + d]);
-    const T* x = h < G ? q_in + h * kHd : k_in;
-    const float xv = to_f32<T>(x[d]);
-    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
-    const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
-    if (h < G) {
-      qs[h * kHd + d] = r;
-    } else {
-      kf[d] = r;
-      vf[d] = v_in[d];
-    }
-  }
-  __syncthreads();
-  if (warp < 2) {  // warp 0 quantises the rotated k row, warp 1 the v row; split 0 writes them to the cache
-    const T* src = warp ? vf : kf;
-    float x[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) x[j] = to_f32<T>(src[4 * lane + j]);
-    T sc, ze;
-    const uint32_t q = kv8_quant4<T>(x, gs, sc, ze);
-    *reinterpret_cast<uint32_t*>(fq + warp * kHd + 4 * lane) = q;
-    const int grp = 4 * lane / gs;
-    if ((4 * lane) % gs == 0) { fm[4 * warp + grp] = sc; fm[4 * warp + 2 + grp] = ze; }
-    if (split == 0) {
-      long long pr = pos;
-      if constexpr (PAGED) pr = page_row(tab, n_kv, kvh, pos);
-      *reinterpret_cast<uint32_t*>((warp ? v_q : k_q) + pr * kHd + 4 * lane) = q;
-      if ((4 * lane) % gs == 0) {
-        (warp ? v_s : k_s)[pr * ng + grp] = sc;
-        (warp ? v_z : k_z)[pr * ng + grp] = ze;
-      }
-    }
-  }
-  __syncthreads();
-  if (pos >= c0 && pos < c1) {  // row pos in a tile staged before the wait: its owner fills it in now
-    const int ti = (pos - c0) / kSplitTile, i = ti / NW;
-    if (ti % NW == warp && i < ST - 1) {
-      const int r = pos - (c0 + ti * kSplitTile);
-      char* st = ring + (i % ST) * kKv8StageBytes;
-      if (lane < 16) {
-        const int isv = lane >> 3, c = lane & 7;
-        *reinterpret_cast<uint4*>(st + isv * kKv8LvlBytes + swz8(r, c)) = *reinterpret_cast<const uint4*>(fq + isv * kHd + c * 16);
-      } else if (lane < 16 + 4 * ng) {
-        const int a = (lane - 16) / ng, e = (lane - 16) % ng;
-        reinterpret_cast<T*>(st + 2 * kKv8LvlBytes + a * kKv8MetaBytes)[r * ng + e] = fm[2 * a + e];
-      }
-    }
-  }
-  // Q^T fragments in the permuted dims: k slots 2 qd + {0, 1} / + {8, 9} of step kk are dims 32 qd + 4 kk + {0, 1} / + {2, 3}
-  uint32_t qb[8][2];
-#pragma unroll
-  for (int kk = 0; kk < 8; ++kk) {
-    const T* qr = qs + g * kHd + 32 * qd + 4 * kk;
-    qb[kk][0] = g < G ? *reinterpret_cast<const uint32_t*>(qr) : 0u;
-    qb[kk][1] = g < G ? *reinterpret_cast<const uint32_t*>(qr + 2) : 0u;
-  }
-
-  float o[8][4];
-#pragma unroll
-  for (int mt = 0; mt < 8; ++mt) o[mt][0] = o[mt][1] = o[mt][2] = o[mt][3] = 0.f;
-  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  const int gk = 32 * qd / gs, gv = 16 * g / gs;  // the group of the lane's K dims and of its V dims
-  for (int i = 0; i < my_tiles; ++i) {
-    __syncwarp();  // every lane is done with the slot the next issue overwrites
-    issue(i + ST - 1, true);
-    split_wait<ST - 1>();
-    __syncwarp();  // this tile's copies and plain stores of every lane are visible to the warp
-    const char* st = ring + (i % ST) * kKv8StageBytes;
-    const T* ms = reinterpret_cast<const T*>(st + 2 * kKv8LvlBytes);
-    constexpr int MA = kKv8MetaBytes / 2;  // T elements per meta array
-    float s[4] = {0.f, 0.f, 0.f, 0.f};
-    {
-      const uint4 ka0 = *reinterpret_cast<const uint4*>(st + swz8(g, 2 * qd)), ka1 = *reinterpret_cast<const uint4*>(st + swz8(g, 2 * qd + 1));
-      const uint4 kb0 = *reinterpret_cast<const uint4*>(st + swz8(g + 8, 2 * qd)), kb1 = *reinterpret_cast<const uint4*>(st + swz8(g + 8, 2 * qd + 1));
-      typename Pair<T>::type sa, sb, za, zb;  // rows g and g + 8, both halves alike
-      sa.x = sa.y = ms[g * ng + gk]; sb.x = sb.y = ms[(g + 8) * ng + gk];
-      za.x = za.y = ms[MA + g * ng + gk]; zb.x = zb.y = ms[MA + (g + 8) * ng + gk];
-      const uint32_t wa[8] = {ka0.x, ka0.y, ka0.z, ka0.w, ka1.x, ka1.y, ka1.z, ka1.w};
-      const uint32_t wb[8] = {kb0.x, kb0.y, kb0.z, kb0.w, kb1.x, kb1.y, kb1.z, kb1.w};
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        uint32_t a[4];
-        a[0] = kv8_deq2<T, 0>(wa[kk], za, sa);
-        a[2] = kv8_deq2<T, 1>(wa[kk], za, sa);
-        a[1] = kv8_deq2<T, 0>(wb[kk], zb, sb);
-        a[3] = kv8_deq2<T, 1>(wb[kk], zb, sb);
-        mma16816<T>(s, a, qb[kk][0], qb[kk][1]);
-      }
-    }
-    const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
-    const float x0 = p0 < c1 ? s[0] * scale_log2 : -INFINITY, x1 = p0 < c1 ? s[1] * scale_log2 : -INFINITY;
-    const float x2 = p0 + 8 < c1 ? s[2] * scale_log2 : -INFINITY, x3 = p0 + 8 < c1 ? s[3] * scale_log2 : -INFINITY;
-    float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
-#pragma unroll
-    for (int off = 4; off < 32; off <<= 1) {
-      t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
-      t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
-    }
-    const float n0 = fmaxf(m0, t0), n1 = fmaxf(m1, t1);  // finite: every tile holds position c0 + 16 j < c1
-    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
-    m0 = n0; m1 = n1;
-    const T p00 = from_f32<T>(exp2f(x0 - n0)), p01 = from_f32<T>(exp2f(x1 - n1));
-    const T p10 = from_f32<T>(exp2f(x2 - n0)), p11 = from_f32<T>(exp2f(x3 - n1));
-    l0 = l0 * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
-    l1 = l1 * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
-#pragma unroll
-    for (int mt = 0; mt < 8; ++mt) { o[mt][0] *= a0; o[mt][1] *= a1; o[mt][2] *= a0; o[mt][3] *= a1; }
-    // P^T fragment (k = position, n = head g), as in rope_attn_decode_split_kernel
-    const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
-    const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
-    const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
-    const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
-    const uint32_t b0 = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
-    const uint32_t b1 = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
-    {
-      // V^T: positions r = 2 qd + {0, 1, 8, 9}, dims 16 g .. 16 g + 15 (one 16-byte chunk each)
-      const char* vt = st + kKv8LvlBytes;
-      const int r0 = 2 * qd;
-      const uint4 v0 = *reinterpret_cast<const uint4*>(vt + swz8(r0, g)), v1 = *reinterpret_cast<const uint4*>(vt + swz8(r0 + 1, g));
-      const uint4 v8 = *reinterpret_cast<const uint4*>(vt + swz8(r0 + 8, g)), v9 = *reinterpret_cast<const uint4*>(vt + swz8(r0 + 9, g));
-      const T* vs = ms + 2 * MA;
-      const T* vz = ms + 3 * MA;
-      typename Pair<T>::type s01, s89, z01, z89;  // positions r0, r0 + 1 and r0 + 8, r0 + 9
-      s01.x = vs[r0 * ng + gv]; s01.y = vs[(r0 + 1) * ng + gv];
-      s89.x = vs[(r0 + 8) * ng + gv]; s89.y = vs[(r0 + 9) * ng + gv];
-      z01.x = vz[r0 * ng + gv]; z01.y = vz[(r0 + 1) * ng + gv];
-      z89.x = vz[(r0 + 8) * ng + gv]; z89.y = vz[(r0 + 9) * ng + gv];
-      const uint32_t w0[4] = {v0.x, v0.y, v0.z, v0.w}, w1[4] = {v1.x, v1.y, v1.z, v1.w};
-      const uint32_t w8[4] = {v8.x, v8.y, v8.z, v8.w}, w9[4] = {v9.x, v9.y, v9.z, v9.w};
-#pragma unroll
-      for (int wi = 0; wi < 4; ++wi) {
-        // dims 16 g + 4 wi .. + 3 are bytes 0..3 of word wi; interleave the two positions of each pair: [p.b, p'.b, p.b+1, p'.b+1]
-        const uint32_t lo01 = prmt(w0[wi], w1[wi], 0x5140u), hi01 = prmt(w0[wi], w1[wi], 0x7362u);
-        const uint32_t lo89 = prmt(w8[wi], w9[wi], 0x5140u), hi89 = prmt(w8[wi], w9[wi], 0x7362u);
-        uint32_t a[4];
-        // step mt = 2 wi: dims 16 g + 4 wi (+ 1); step 2 wi + 1: dims 16 g + 4 wi + 2 (+ 3)
-        a[0] = kv8_deq2<T, 0>(lo01, z01, s01); a[1] = kv8_deq2<T, 1>(lo01, z01, s01);
-        a[2] = kv8_deq2<T, 0>(lo89, z89, s89); a[3] = kv8_deq2<T, 1>(lo89, z89, s89);
-        mma16816<T>(o[2 * wi], a, b0, b1);
-        a[0] = kv8_deq2<T, 0>(hi01, z01, s01); a[1] = kv8_deq2<T, 1>(hi01, z01, s01);
-        a[2] = kv8_deq2<T, 0>(hi89, z89, s89); a[3] = kv8_deq2<T, 1>(hi89, z89, s89);
-        mma16816<T>(o[2 * wi + 1], a, b0, b1);
-      }
-    }
-  }
-  split_wait<0>();
-#pragma unroll
-  for (int off = 4; off < 32; off <<= 1) {
-    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
-  }
-  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][8][m, l, o[128]]
-  float* wp = reinterpret_cast<float*>(smem);
-  {
-    float* w0 = wp + (warp * kSplitMaxGroup + 2 * qd) * kPartFloats;
-    float* w1 = w0 + kPartFloats;
-    if (g == 0) { w0[0] = m0; w0[1] = l0; w1[0] = m1; w1[1] = l1; }
-#pragma unroll
-    for (int mt = 0; mt < 8; ++mt) {  // O^T rows g, g + 8 of step mt are dims 16 g + 2 mt, 16 g + 2 mt + 1
-      w0[2 + 16 * g + 2 * mt] = o[mt][0]; w1[2 + 16 * g + 2 * mt] = o[mt][1];
-      w0[2 + 16 * g + 2 * mt + 1] = o[mt][2]; w1[2 + 16 * g + 2 * mt + 1] = o[mt][3];
-    }
-  }
-  __syncthreads();
-  split_merge<T>(wp, part, tickets, out, last, S, split, G, tid);
-}
-
 // 4-bit HQQ KV cache (DESIGN.md 3.5).  A cache row of one kv head is Quantizer.quantize(row, nbits=4, group_size=gs, axis=1,
 // optimize=False) with gs 32 or 64, packed as the reference's 4bit_u8 packing of that row: 64 bytes, byte d = q[d] << 4 | q[d + 64];
 // meta [128 / gs] T.  The attended row is T(T(q - z) * s), what oracle.dequantize gives.  16-byte chunk c of a row holds dims
@@ -987,192 +588,204 @@ __device__ __forceinline__ uint32_t kv4_deq2(uint32_t t, typename Pair<T>::type 
   return *reinterpret_cast<const uint32_t*>(&r);
 }
 
-// Split-KV decode attention over a 4-bit cache: rope_attn_decode_split_kv8_kernel's grid, chunks, ticket, merge, RoPE and
-// pre-wait staging, with a 6-stage ring of 2560-byte stages (K and V levels [16][64], 16-byte chunks swizzled so that the 16 rows
-// of a tile fill 8 lines of 128 bytes with line l = r / 2 holding chunk (4 (r & 1) + c) ^ 2 (l & 3) -- conflict-free for the K reads
-// (16 bytes a lane) and the V reads (8 bytes a lane) below -- then k scale | k zero | v scale | v zero [16][<= 4]).  The head dim is
-// permuted the same way for both operands of a product: lane (g, qd) takes K chunk qd of positions g, g + 8 (k slot
-// 2 qd + {0, 1, 8, 9} of step kk is dim 16 qd + 4 kk + {0..3} for kk < 4, the high nibbles, and 64 + 16 qd + 4 (kk - 4) + {0..3}
-// for kk >= 4, the low nibbles), and V bytes 8 g .. 8 g + 7 of positions 2 qd + {0, 1, 8, 9} (O^T row g of step mt is dim 8 g + mt,
-// the high nibble of byte 8 g + mt; row g + 8 is dim 64 + 8 g + mt, its low nibble).  Each lane's K half-row and V half-row span
-// two groups, one per nibble.  Row pos is this launch's quantisation of the fresh k / v in every CTA that holds it; split 0 writes
-// it to the cache.
-constexpr int kKv4Stages = 6;
-constexpr int kKv4LvlBytes = kSplitTile * kHd / 2;                                // one K or V level tile, 1 KB
-constexpr int kKv4MetaBytes = kSplitTile * 4 * 2;                                 // one meta array of a tile: [16][<= 4] T
-constexpr int kKv4StageBytes = 2 * kKv4LvlBytes + 4 * kKv4MetaBytes;
-constexpr int kKv4RingBytes = kSplitWarps * kKv4Stages * kKv4StageBytes;           // 120 KB
-// + rotated q [8][128] T, fresh k, v [128] T, their packed levels [2][64] and meta [4][4] T, the last-CTA flag
-constexpr int kKv4SmemBytes = kKv4RingBytes + (kSplitMaxGroup + 2) * kHd * 2 + kHd + 32 + 16;
-static_assert(kSplitWarps * kSplitMaxGroup * kPartFloats * 4 <= kKv4RingBytes, "the warp partials reuse the ring");
-
-__device__ __forceinline__ int swz4(int r, int c) { return (r >> 1) * 128 + (((((r & 1) << 2) | c) ^ (((r >> 1) & 3) << 1)) << 4); }
-
-// grid = (S, n_kv, batch), block = 256.  As rope_attn_decode_split_kv8_kernel, with packed levels [batch, n_kv, L, 64] uint8 and meta
-// [batch, n_kv, L, 128 / gs] T (paged: [pages, n_kv, 64, 64] and [pages, n_kv, 64, 128 / gs]), gs 32 or 64.
-template <typename T, bool SEQPOS = false, bool PAGED = false>
-__global__ void __launch_bounds__(kSplitThreads, 1)
-    rope_attn_decode_split_kv4_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
-                                      const T* __restrict__ sin_t, uint8_t* __restrict__ k_q, T* __restrict__ k_s, T* __restrict__ k_z,
-                                      uint8_t* __restrict__ v_q, T* __restrict__ v_s, T* __restrict__ v_z, const long long* __restrict__ pos_p,
-                                      T* __restrict__ out, float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L,
-                                      int gs, float scale_log2, const PageArg<PAGED> pg) {
-  extern __shared__ __align__(16) char smem[];
-  constexpr int NW = kSplitWarps, ST = kKv4Stages, LB = kHd / 2;
-  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
-  const int G = n_q / n_kv, ng = kHd / gs;
-  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
-  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
-  const int* tab = nullptr;
-  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
-  {
-    const long long kv = (long long)b * n_kv + kvh;
-    if constexpr (!PAGED) {
-      k_q += kv * L * LB; v_q += kv * L * LB;
-      k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
-    }
-    k_in += kv * kHd; v_in += kv * kHd;
-    q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
-    part += kv * S * G * kPartFloats;
-    tickets += kv;
+// The warp row quantiser of the quantised caches: the 128-element row x (lane l: elements 4 l .. 4 l + 3) quantised by kv8_quant4 to
+// BITS bits, its levels stored at lq (BITS 4: packed by kv4_pack, 64 bytes written by lanes 0..15) and each group's scale and zero at
+// s[group], z[group].  Returns the lane's four levels (one per byte) and, in sc / ze, their group's meta.  Every lane must call it.
+template <typename T, int BITS>
+__device__ __forceinline__ uint32_t kv_quant_row(const float (&x)[4], int gs, uint8_t* lq, T* s, T* z, T& sc, T& ze) {
+  const int lane = (int)threadIdx.x & 31;
+  const uint32_t lv = kv8_quant4<T, (1 << BITS) - 1>(x, gs, sc, ze);
+  if constexpr (BITS == 8) {
+    *reinterpret_cast<uint32_t*>(lq + 4 * lane) = lv;
+  } else {
+    const uint32_t pk = kv4_pack(lv);
+    if (lane < 16) *reinterpret_cast<uint32_t*>(lq + 4 * lane) = pk;
   }
-  char* ring = smem + warp * ST * kKv4StageBytes;
-  T* qs = reinterpret_cast<T*>(smem + kKv4RingBytes);  // rotated q [8][128]
-  T* kf = qs + kSplitMaxGroup * kHd;                   // rotated k and v of position pos
-  T* vf = kf + kHd;
-  uint8_t* fq = reinterpret_cast<uint8_t*>(vf + kHd);  // their packed levels: k [64], v [64]
-  T* fm = reinterpret_cast<T*>(fq + 2 * LB);           // their meta: k scale, k zero, v scale, v zero [4] each
-  int* last = reinterpret_cast<int*>(fm + 16);
+  if ((4 * lane) % gs == 0) {
+    s[4 * lane / gs] = sc;
+    z[4 * lane / gs] = ze;
+  }
+  return lv;
+}
 
-  // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
-  const int pos = (int)pos_p[SEQPOS ? b : 0], n_pos = pos + 1;
-  const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
-  const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
-  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
-  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;
-  pdl_launch_dependents();
+// The cache formats of rope_attn_decode_split_kernel.  A format holds the cache pointers -- level arrays k and v with rows of kRowBytes
+// bytes, copied in 16-byte chunks -- and supplies what differs between formats:
+//   - the stage layout: each warp's ring has kStages stages of kStageBytes, the K then the V levels of a 16-position tile (kLvlBytes
+//     each, chunk c of row r at slot(r, c)), then the format's meta (4 arrays of kMetaBytes); the smem a CTA needs (kSmemBytes);
+//   - the per-(sequence, kv head) advance of the pointers (contiguous caches);
+//   - the staging of a tile's meta rows and the row-pos patch of that meta in a tile staged before the wait;
+//   - the fresh row pos: the kFreshBytes after the rotated k, v hold it in cache format (none: the rotated rows are that), and split 0
+//     writes it to the cache;
+//   - the head-dim permutation, the same for both operands of a product (so the products are unchanged): the Q^T fragment dims
+//     (k slots 2 qd + {0, 1} of step kk are dims qdim(kk, qd) + {0, 1}, slots 2 qd + {8, 9} kQPair dims further) and the O^T -> dim
+//     map odim(mt, g, hi) (O^T row g + 8 hi of step mt);
+//   - the score MMA loop (K . Q^T) and the V^T . P^T loop over one staged tile.
+//
+// 16-bit cache: [16][128] T tiles of 16-byte chunks XOR-swizzled by row, read through ldmatrix (conflict-free) in 3 stages of 8 KB.
+template <typename T>
+struct KvF16 {
+  static constexpr int kStages = kSplitStages, kRowBytes = 2 * kHd, kFreshBytes = 0;
+  static constexpr int kLvlBytes = kTileBytes, kStageBytes = 2 * kLvlBytes;
+  static constexpr int kRingBytes = kSplitWarps * kStages * kStageBytes;  // 192 KB
+  static constexpr int kSmemBytes = kRingBytes + (kSplitMaxGroup + 2) * kHd * 2 + kFreshBytes + 16;  // + q [8][128], k, v, the fresh row, the flag
+  static constexpr int kQPair = 8;
+  T* k;
+  T* v;
 
-  // Stage local tile i as the 8-bit kernel does: rows < pos from the cache, row pos from this launch's quantisation once `fresh`,
-  // rows past pos zero (levels and meta: they dequantise to 0).  A meta chunk of 16 bytes spans 8 / ng rows; one that reaches row pos
-  // (or sits on a misaligned address) is staged row by row.
-  auto issue = [&](int i, bool fresh) {
-    if (i < my_tiles) {
-      const int t0 = c0 + (warp + i * NW) * kSplitTile;
-      char* st = ring + (i % ST) * kKv4StageBytes;
-      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
-      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
+  __device__ static int slot(int r, int c) { return swz(r, c); }
+  __device__ static int qdim(int kk, int qd) { return 16 * kk + 2 * qd; }
+  __device__ static int odim(int mt, int g, int hi) { return 16 * mt + g + 8 * hi; }
+  __device__ void advance(long long kv, int L) { k += kv * L * kHd; v += kv * L * kHd; }
+  __device__ void stage_meta(char*, long long, int, int, int, bool, const char*) const {}
+  __device__ void patch_meta(char*, int, int, const char*) const {}
+  // kf: the rotated k row, then v.  Split 0 writes them to the cache row pr (no CTA of this launch reads it).
+  __device__ void fresh(const T* kf, char*, bool write, long long pr, int tid) const {
+    if (write && tid < kHd) {
+      k[pr * kHd + tid] = kf[tid];
+      v[pr * kHd + tid] = kf[kHd + tid];
+    }
+  }
+  __device__ void scores(float (&s)[4], const char* st, const uint32_t (&qb)[8][2], int lane) const {
+    const int kr = (lane & 7) + ((lane >> 3) & 1) * 8, kc = lane >> 4;  // ldmatrix row / chunk, K (a0..a3: rows +8, then k +8)
 #pragma unroll
-      for (int j = lane; j < 2 * kSplitTile * 4; j += 32) {
-        const int isv = j >> 6, r = (j >> 2) & 15, c = j & 3, p = t0 + r;
-        char* dst = st + isv * kKv4LvlBytes + swz4(r, c);
-        if (p < pos) {
-          split_cp16(dst, (isv ? v_q : k_q) + (rt + p) * LB + c * 16);
-        } else if (p > pos || fresh) {
-          uint4 val;
-          val.x = val.y = val.z = val.w = 0u;
-          if (p == pos) val = *reinterpret_cast<const uint4*>(fq + isv * LB + c * 16);
-          *reinterpret_cast<uint4*>(dst) = val;
-        }
-      }
-      if (lane < 8 * ng) {  // 4 arrays x 2 ng chunks
-        const int a = lane / (2 * ng), j = lane % (2 * ng), rows = 8 / ng, r0 = j * rows;
-        const T* src = (a == 0 ? k_s : a == 1 ? k_z : a == 2 ? v_s : v_z) + (rt + (t0 + r0)) * ng;
-        char* dst = st + 2 * kKv4LvlBytes + a * kKv4MetaBytes + j * 16;
-        if (t0 + r0 + rows <= pos && ((uintptr_t)src & 15) == 0) {
-          split_cp16(dst, src);
-        } else {
-          for (int e = 0; e < 8; ++e) {
-            const int p = t0 + r0 + e / ng;
-            if (p < pos) reinterpret_cast<T*>(dst)[e] = src[e];
-            else if (p > pos) reinterpret_cast<T*>(dst)[e] = from_f32<T>(0.f);
-            else if (fresh) reinterpret_cast<T*>(dst)[e] = fm[4 * a + e % ng];
-          }
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t a[4];
+      ldsm4<false>(a, st + swz(kr, 2 * kk + kc));
+      mma16816<T>(s, a, qb[kk][0], qb[kk][1]);
+    }
+  }
+  __device__ void pv(float (&o)[8][4], const char* st, uint32_t b0, uint32_t b1, int lane) const {
+    const int vr = (lane & 7) + ((lane >> 4) & 1) * 8, vc = (lane >> 3) & 1;  // V^T (a0..a3: dims +8, then positions +8)
+    const char* vt = st + kLvlBytes;
+#pragma unroll
+    for (int mt = 0; mt < 8; ++mt) {
+      uint32_t a[4];
+      ldsm4<true>(a, vt + swz(vr, 2 * mt + vc));
+      mma16816<T>(o[mt], a, b0, b1);
+    }
+  }
+};
+
+// HQQ cache of BITS 8 (gs 64 or 128) or 4 (gs 32 or 64): levels [.., L, 128 BITS / 8] uint8, meta k_s, k_z, v_s, v_z [.., L, 128 / gs]
+// T, dequantised straight into the MMA fragments.  The meta of a stage is k scale | k zero | v scale | v zero [16][kNg], kNg the most
+// groups a row has; the fresh row is its levels [2][kRowBytes] and meta [4][kNg].  A meta chunk of 16 bytes spans 8 / ng rows.
+//   8 bits: 4 stages of 4352 bytes, level rows of 8 chunks XOR-swizzled by row.  Lane (g, qd) takes K dims 32 qd .. 32 qd + 31 of
+//     positions g, g + 8 (k slot 2 qd + {0, 1, 8, 9} of step kk is dim 32 qd + 4 kk + {0..3}) and V dims 16 g .. 16 g + 15 of positions
+//     2 qd + {0, 1, 8, 9} (O^T row g / g + 8 of step mt is dim 16 g + 2 mt / + 1): two 16-byte loads a row, one group each.
+//   4 bits: 6 stages of 2560 bytes, the 16 level rows of a tile filling 8 lines of 128 bytes, line l = r / 2 holding chunk
+//     (4 (r & 1) + c) ^ 2 (l & 3) -- conflict-free for the K reads (16 bytes a lane) and the V reads (8 bytes a lane).  Lane (g, qd)
+//     takes K chunk qd of positions g, g + 8 (k slot 2 qd + {0, 1, 8, 9} of step kk is dim 16 qd + 4 kk + {0..3} for kk < 4, the high
+//     nibbles, and 64 + 16 qd + 4 (kk - 4) + {0..3} for kk >= 4, the low nibbles), and V bytes 8 g .. 8 g + 7 of positions
+//     2 qd + {0, 1, 8, 9} (O^T row g of step mt is dim 8 g + mt, the high nibble of byte 8 g + mt; row g + 8 is dim 64 + 8 g + mt, its
+//     low nibble).  Each lane's K half-row and V half-row span two groups, one per nibble.
+template <typename T, int BITS>
+struct KvHqq {
+  static_assert(BITS == 8 || BITS == 4, "8- or 4-bit levels");
+  static constexpr int kNg = BITS == 8 ? 2 : 4;
+  static constexpr int kStages = BITS == 8 ? 4 : 6, kRowBytes = kHd * BITS / 8, kMetaBytes = kSplitTile * kNg * 2;
+  static constexpr int kFreshBytes = 2 * kRowBytes + 4 * kNg * 2;
+  static constexpr int kLvlBytes = kSplitTile * kRowBytes, kStageBytes = 2 * kLvlBytes + 4 * kMetaBytes;
+  static constexpr int kRingBytes = kSplitWarps * kStages * kStageBytes;  // 136 KB (8 bits), 120 KB (4 bits)
+  static constexpr int kSmemBytes = kRingBytes + (kSplitMaxGroup + 2) * kHd * 2 + kFreshBytes + 16;
+  static constexpr int kQPair = 2;
+  uint8_t* k;
+  T* k_s;
+  T* k_z;
+  uint8_t* v;
+  T* v_s;
+  T* v_z;
+  int gs;
+  int ng;  // 128 / gs groups a row
+
+  // group of dim d: d / gs without a division by the run-time gs, which the compiler will not hoist out of the tile loop
+  __device__ int grp(int d) const { return d * ng / kHd; }
+
+  __device__ static int slot(int r, int c) {
+    if constexpr (BITS == 8) return r * kHd + ((c ^ (r & 7)) << 4);
+    else return (r >> 1) * 128 + (((((r & 1) << 2) | c) ^ (((r >> 1) & 3) << 1)) << 4);
+  }
+  __device__ static int qdim(int kk, int qd) {
+    if constexpr (BITS == 8) return 32 * qd + 4 * kk;
+    else return kk < 4 ? 16 * qd + 4 * kk : 64 + 16 * qd + 4 * (kk - 4);
+  }
+  __device__ static int odim(int mt, int g, int hi) {
+    if constexpr (BITS == 8) return 16 * g + 2 * mt + hi;
+    else return 8 * g + mt + 64 * hi;
+  }
+  __device__ void advance(long long kv, int L) {
+    k += kv * L * kRowBytes; v += kv * L * kRowBytes;
+    k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
+  }
+  // Meta rows < pos from the cache, row pos from the fresh meta fx once `fresh`, rows past pos zero (they dequantise to 0).  A chunk
+  // that reaches row pos (or sits on a misaligned address) is staged row by row.
+  __device__ void stage_meta(char* st, long long rt, int t0, int pos, int lane, bool fresh, const char* fx) const {
+    if (lane < 8 * ng) {  // 4 arrays x 2 ng chunks
+      const T* fm = reinterpret_cast<const T*>(fx + 2 * kRowBytes);
+      const int a = lane / (2 * ng), j = lane % (2 * ng), rows = 8 / ng, r0 = j * rows;
+      const T* src = (a == 0 ? k_s : a == 1 ? k_z : a == 2 ? v_s : v_z) + (rt + (t0 + r0)) * ng;
+      char* dst = st + 2 * kLvlBytes + a * kMetaBytes + j * 16;
+      if (t0 + r0 + rows <= pos && ((uintptr_t)src & 15) == 0) {
+        split_cp16(dst, src);
+      } else {
+        for (int e = 0; e < 8; ++e) {
+          const int p = t0 + r0 + e / ng;
+          if (p < pos) reinterpret_cast<T*>(dst)[e] = src[e];
+          else if (p > pos) reinterpret_cast<T*>(dst)[e] = from_f32<T>(0.f);
+          else if (fresh) reinterpret_cast<T*>(dst)[e] = fm[kNg * a + e % ng];
         }
       }
     }
-    split_commit();  // always (possibly empty): every iteration waits on the same group count
-  };
+  }
+  __device__ void patch_meta(char* st, int r, int lane, const char* fx) const {
+    if (lane >= 16 && lane < 16 + 4 * ng) {
+      const T* fm = reinterpret_cast<const T*>(fx + 2 * kRowBytes);
+      const int a = (lane - 16) / ng, e = (lane - 16) % ng;
+      reinterpret_cast<T*>(st + 2 * kLvlBytes + a * kMetaBytes)[r * ng + e] = fm[kNg * a + e];
+    }
+  }
+  // Warp 0 quantises the rotated k row kf, warp 1 the v row after it, into the fresh row fx.  In split 0 warps 2 and 3 quantise the same
+  // rows into cache row pr: the same bits, from warps that would otherwise wait at the barrier.  Ends with a barrier.
+  __device__ void fresh(const T* kf, char* fx, bool write, long long pr, int tid) const {
+    const int warp = tid >> 5, lane = tid & 31, isv = warp & 1;
+    if (warp < 2 || (write && warp < 4)) {
+      float x[4];
 #pragma unroll
-  for (int i = 0; i < ST - 1; ++i) issue(i, false);
-  pdl_wait();
-
-  // RoPE exactly as rope_attn_decode_kernel: x*cos + rotate_half(x)*sin, each product and the sum rounded to T
-  for (int i = tid; i < (G + 1) * kHd; i += kSplitThreads) {
-    const int h = i >> 7, d = i & (kHd - 1), half = kHd / 2;
-    const float c = to_f32<T>(cos_t[(long long)pos * kHd + d]), s = to_f32<T>(sin_t[(long long)pos * kHd + d]);
-    const T* x = h < G ? q_in + h * kHd : k_in;
-    const float xv = to_f32<T>(x[d]);
-    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
-    const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
-    if (h < G) {
-      qs[h * kHd + d] = r;
+      for (int j = 0; j < 4; ++j) x[j] = to_f32<T>(kf[isv * kHd + 4 * lane + j]);
+      T* fm = reinterpret_cast<T*>(fx + 2 * kRowBytes);
+      const bool own = warp < 2;
+      uint8_t* lq = own ? reinterpret_cast<uint8_t*>(fx) + isv * kRowBytes : (isv ? v : k) + pr * kRowBytes;
+      T* ls = own ? fm + 2 * isv * kNg : (isv ? v_s : k_s) + pr * ng;
+      T* lz = own ? fm + (2 * isv + 1) * kNg : (isv ? v_z : k_z) + pr * ng;
+      T sc, ze;
+      kv_quant_row<T, BITS>(x, gs, lq, ls, lz, sc, ze);
+    }
+    __syncthreads();
+  }
+  __device__ void scores(float (&s)[4], const char* st, const uint32_t (&qb)[8][2], int lane) const {
+    const int g = lane >> 2, qd = lane & 3;
+    const T* ms = reinterpret_cast<const T*>(st + 2 * kLvlBytes);
+    constexpr int MA = kMetaBytes / 2;  // T elements per meta array
+    if constexpr (BITS == 8) {
+      const int gk = grp(32 * qd);  // the group of the lane's K dims
+      const uint4 ka0 = *reinterpret_cast<const uint4*>(st + slot(g, 2 * qd)), ka1 = *reinterpret_cast<const uint4*>(st + slot(g, 2 * qd + 1));
+      const uint4 kb0 = *reinterpret_cast<const uint4*>(st + slot(g + 8, 2 * qd)), kb1 = *reinterpret_cast<const uint4*>(st + slot(g + 8, 2 * qd + 1));
+      typename Pair<T>::type sa, sb, za, zb;  // rows g and g + 8, both halves alike
+      sa.x = sa.y = ms[g * ng + gk]; sb.x = sb.y = ms[(g + 8) * ng + gk];
+      za.x = za.y = ms[MA + g * ng + gk]; zb.x = zb.y = ms[MA + (g + 8) * ng + gk];
+      const uint32_t wa[8] = {ka0.x, ka0.y, ka0.z, ka0.w, ka1.x, ka1.y, ka1.z, ka1.w};
+      const uint32_t wb[8] = {kb0.x, kb0.y, kb0.z, kb0.w, kb1.x, kb1.y, kb1.z, kb1.w};
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        uint32_t a[4];
+        a[0] = kv8_deq2<T, 0>(wa[kk], za, sa);
+        a[2] = kv8_deq2<T, 1>(wa[kk], za, sa);
+        a[1] = kv8_deq2<T, 0>(wb[kk], zb, sb);
+        a[3] = kv8_deq2<T, 1>(wb[kk], zb, sb);
+        mma16816<T>(s, a, qb[kk][0], qb[kk][1]);
+      }
     } else {
-      kf[d] = r;
-      vf[d] = v_in[d];
-    }
-  }
-  __syncthreads();
-  if (warp < 2) {  // warp 0 quantises the rotated k row, warp 1 the v row; split 0 writes them to the cache
-    const T* src = warp ? vf : kf;
-    float x[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) x[j] = to_f32<T>(src[4 * lane + j]);
-    T sc, ze;
-    const uint32_t q = kv4_pack(kv8_quant4<T, 15>(x, gs, sc, ze));
-    if (lane < 16) *reinterpret_cast<uint32_t*>(fq + warp * LB + 4 * lane) = q;
-    const int grp = 4 * lane / gs;
-    if ((4 * lane) % gs == 0) { fm[8 * warp + grp] = sc; fm[8 * warp + 4 + grp] = ze; }
-    if (split == 0) {
-      long long pr = pos;
-      if constexpr (PAGED) pr = page_row(tab, n_kv, kvh, pos);
-      if (lane < 16) *reinterpret_cast<uint32_t*>((warp ? v_q : k_q) + pr * LB + 4 * lane) = q;
-      if ((4 * lane) % gs == 0) {
-        (warp ? v_s : k_s)[pr * ng + grp] = sc;
-        (warp ? v_z : k_z)[pr * ng + grp] = ze;
-      }
-    }
-  }
-  __syncthreads();
-  if (pos >= c0 && pos < c1) {  // row pos in a tile staged before the wait: its owner fills it in now
-    const int ti = (pos - c0) / kSplitTile, i = ti / NW;
-    if (ti % NW == warp && i < ST - 1) {
-      const int r = pos - (c0 + ti * kSplitTile);
-      char* st = ring + (i % ST) * kKv4StageBytes;
-      if (lane < 8) {
-        const int isv = lane >> 2, c = lane & 3;
-        *reinterpret_cast<uint4*>(st + isv * kKv4LvlBytes + swz4(r, c)) = *reinterpret_cast<const uint4*>(fq + isv * LB + c * 16);
-      } else if (lane >= 16 && lane < 16 + 4 * ng) {
-        const int a = (lane - 16) / ng, e = (lane - 16) % ng;
-        reinterpret_cast<T*>(st + 2 * kKv4LvlBytes + a * kKv4MetaBytes)[r * ng + e] = fm[4 * a + e];
-      }
-    }
-  }
-  // Q^T fragments in the permuted dims: k slots 2 qd + {0, 1} / + {8, 9} of step kk are dims dk + {0, 1} / + {2, 3}
-  uint32_t qb[8][2];
-#pragma unroll
-  for (int kk = 0; kk < 8; ++kk) {
-    const T* qr = qs + g * kHd + (kk < 4 ? 16 * qd + 4 * kk : 64 + 16 * qd + 4 * (kk - 4));
-    qb[kk][0] = g < G ? *reinterpret_cast<const uint32_t*>(qr) : 0u;
-    qb[kk][1] = g < G ? *reinterpret_cast<const uint32_t*>(qr + 2) : 0u;
-  }
-
-  float o[8][4];
-#pragma unroll
-  for (int mt = 0; mt < 8; ++mt) o[mt][0] = o[mt][1] = o[mt][2] = o[mt][3] = 0.f;
-  float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  const int gkh = 16 * qd / gs, gkl = (64 + 16 * qd) / gs;  // the groups of the lane's K dims (high, low nibbles)
-  const int gvh = 8 * g / gs, gvl = (64 + 8 * g) / gs;      // and of its V dims
-  for (int i = 0; i < my_tiles; ++i) {
-    __syncwarp();  // every lane is done with the slot the next issue overwrites
-    issue(i + ST - 1, true);
-    split_wait<ST - 1>();
-    __syncwarp();  // this tile's copies and plain stores of every lane are visible to the warp
-    const char* st = ring + (i % ST) * kKv4StageBytes;
-    const T* ms = reinterpret_cast<const T*>(st + 2 * kKv4LvlBytes);
-    constexpr int MA = kKv4MetaBytes / 2;  // T elements per meta array
-    float s[4] = {0.f, 0.f, 0.f, 0.f};
-    {
-      const uint4 ka = *reinterpret_cast<const uint4*>(st + swz4(g, qd)), kb = *reinterpret_cast<const uint4*>(st + swz4(g + 8, qd));
+      const int gkh = grp(16 * qd), gkl = grp(64 + 16 * qd);  // the groups of the lane's K dims (high, low nibbles)
+      const uint4 ka = *reinterpret_cast<const uint4*>(st + slot(g, qd)), kb = *reinterpret_cast<const uint4*>(st + slot(g + 8, qd));
       typename Pair<T>::type sah, sal, sbh, sbl, zah, zal, zbh, zbl;  // rows g (a) and g + 8 (b), high and low nibbles
       sah.x = sah.y = ms[g * ng + gkh]; sal.x = sal.y = ms[g * ng + gkl];
       sbh.x = sbh.y = ms[(g + 8) * ng + gkh]; sbl.x = sbl.y = ms[(g + 8) * ng + gkl];
@@ -1193,39 +806,44 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
         mma16816<T>(s, a, qb[w + 4][0], qb[w + 4][1]);
       }
     }
-    const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
-    const float x0 = p0 < c1 ? s[0] * scale_log2 : -INFINITY, x1 = p0 < c1 ? s[1] * scale_log2 : -INFINITY;
-    const float x2 = p0 + 8 < c1 ? s[2] * scale_log2 : -INFINITY, x3 = p0 + 8 < c1 ? s[3] * scale_log2 : -INFINITY;
-    float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
+  }
+  __device__ void pv(float (&o)[8][4], const char* st, uint32_t b0, uint32_t b1, int lane) const {
+    const int g = lane >> 2, qd = lane & 3, r0 = 2 * qd;
+    const T* vs = reinterpret_cast<const T*>(st + 2 * kLvlBytes + 2 * kMetaBytes);
+    const T* vz = reinterpret_cast<const T*>(st + 2 * kLvlBytes + 3 * kMetaBytes);
+    const char* vt = st + kLvlBytes;
+    if constexpr (BITS == 8) {
+      // V^T: positions r = 2 qd + {0, 1, 8, 9}, dims 16 g .. 16 g + 15 (one 16-byte chunk each)
+      const int gv = grp(16 * g);  // the group of the lane's V dims
+      const uint4 v0 = *reinterpret_cast<const uint4*>(vt + slot(r0, g)), v1 = *reinterpret_cast<const uint4*>(vt + slot(r0 + 1, g));
+      const uint4 v8 = *reinterpret_cast<const uint4*>(vt + slot(r0 + 8, g)), v9 = *reinterpret_cast<const uint4*>(vt + slot(r0 + 9, g));
+      typename Pair<T>::type s01, s89, z01, z89;  // positions r0, r0 + 1 and r0 + 8, r0 + 9
+      s01.x = vs[r0 * ng + gv]; s01.y = vs[(r0 + 1) * ng + gv];
+      s89.x = vs[(r0 + 8) * ng + gv]; s89.y = vs[(r0 + 9) * ng + gv];
+      z01.x = vz[r0 * ng + gv]; z01.y = vz[(r0 + 1) * ng + gv];
+      z89.x = vz[(r0 + 8) * ng + gv]; z89.y = vz[(r0 + 9) * ng + gv];
+      const uint32_t w0[4] = {v0.x, v0.y, v0.z, v0.w}, w1[4] = {v1.x, v1.y, v1.z, v1.w};
+      const uint32_t w8[4] = {v8.x, v8.y, v8.z, v8.w}, w9[4] = {v9.x, v9.y, v9.z, v9.w};
 #pragma unroll
-    for (int off = 4; off < 32; off <<= 1) {
-      t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
-      t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
-    }
-    const float n0 = fmaxf(m0, t0), n1 = fmaxf(m1, t1);  // finite: every tile holds position c0 + 16 j < c1
-    const float a0 = exp2f(m0 - n0), a1 = exp2f(m1 - n1);
-    m0 = n0; m1 = n1;
-    const T p00 = from_f32<T>(exp2f(x0 - n0)), p01 = from_f32<T>(exp2f(x1 - n1));
-    const T p10 = from_f32<T>(exp2f(x2 - n0)), p11 = from_f32<T>(exp2f(x3 - n1));
-    l0 = l0 * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
-    l1 = l1 * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
-#pragma unroll
-    for (int mt = 0; mt < 8; ++mt) { o[mt][0] *= a0; o[mt][1] *= a1; o[mt][2] *= a0; o[mt][3] *= a1; }
-    // P^T fragment (k = position, n = head g), as in rope_attn_decode_split_kernel
-    const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
-    const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
-    const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
-    const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
-    const uint32_t b0 = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
-    const uint32_t b1 = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
-    {
+      for (int wi = 0; wi < 4; ++wi) {
+        // dims 16 g + 4 wi .. + 3 are bytes 0..3 of word wi; interleave the two positions of each pair: [p.b, p'.b, p.b+1, p'.b+1]
+        const uint32_t lo01 = prmt(w0[wi], w1[wi], 0x5140u), hi01 = prmt(w0[wi], w1[wi], 0x7362u);
+        const uint32_t lo89 = prmt(w8[wi], w9[wi], 0x5140u), hi89 = prmt(w8[wi], w9[wi], 0x7362u);
+        uint32_t a[4];
+        // step mt = 2 wi: dims 16 g + 4 wi (+ 1); step 2 wi + 1: dims 16 g + 4 wi + 2 (+ 3)
+        a[0] = kv8_deq2<T, 0>(lo01, z01, s01); a[1] = kv8_deq2<T, 1>(lo01, z01, s01);
+        a[2] = kv8_deq2<T, 0>(lo89, z89, s89); a[3] = kv8_deq2<T, 1>(lo89, z89, s89);
+        mma16816<T>(o[2 * wi], a, b0, b1);
+        a[0] = kv8_deq2<T, 0>(hi01, z01, s01); a[1] = kv8_deq2<T, 1>(hi01, z01, s01);
+        a[2] = kv8_deq2<T, 0>(hi89, z89, s89); a[3] = kv8_deq2<T, 1>(hi89, z89, s89);
+        mma16816<T>(o[2 * wi + 1], a, b0, b1);
+      }
+    } else {
       // V^T: positions r = 2 qd + {0, 1, 8, 9}, bytes 8 g .. 8 g + 7 (half of chunk g / 2)
-      const char* vt = st + kKv4LvlBytes;
-      const int r0 = 2 * qd, cb = 8 * (g & 1);
-      const uint2 v0 = *reinterpret_cast<const uint2*>(vt + swz4(r0, g >> 1) + cb), v1 = *reinterpret_cast<const uint2*>(vt + swz4(r0 + 1, g >> 1) + cb);
-      const uint2 v8 = *reinterpret_cast<const uint2*>(vt + swz4(r0 + 8, g >> 1) + cb), v9 = *reinterpret_cast<const uint2*>(vt + swz4(r0 + 9, g >> 1) + cb);
-      const T* vs = ms + 2 * MA;
-      const T* vz = ms + 3 * MA;
+      const int gvh = grp(8 * g), gvl = grp(64 + 8 * g);  // the groups of the lane's V dims (high, low nibbles)
+      const int cb = 8 * (g & 1);
+      const uint2 v0 = *reinterpret_cast<const uint2*>(vt + slot(r0, g >> 1) + cb), v1 = *reinterpret_cast<const uint2*>(vt + slot(r0 + 1, g >> 1) + cb);
+      const uint2 v8 = *reinterpret_cast<const uint2*>(vt + slot(r0 + 8, g >> 1) + cb), v9 = *reinterpret_cast<const uint2*>(vt + slot(r0 + 9, g >> 1) + cb);
       typename Pair<T>::type s01h, s01l, s89h, s89l, z01h, z01l, z89h, z89l;  // positions r0, r0 + 1 / r0 + 8, r0 + 9; high / low nibbles
       s01h.x = vs[r0 * ng + gvh]; s01h.y = vs[(r0 + 1) * ng + gvh]; s01l.x = vs[r0 * ng + gvl]; s01l.y = vs[(r0 + 1) * ng + gvl];
       s89h.x = vs[(r0 + 8) * ng + gvh]; s89h.y = vs[(r0 + 9) * ng + gvh]; s89l.x = vs[(r0 + 8) * ng + gvl]; s89l.y = vs[(r0 + 9) * ng + gvl];
@@ -1244,26 +862,141 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
       }
     }
   }
-  split_wait<0>();
-#pragma unroll
-  for (int off = 4; off < 32; off <<= 1) {
-    l0 += __shfl_xor_sync(0xffffffffu, l0, off);
-    l1 += __shfl_xor_sync(0xffffffffu, l1, off);
-  }
-  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][8][m, l, o[128]]
-  float* wp = reinterpret_cast<float*>(smem);
+};
+
+// grid = (S, n_kv, batch), block = 256.  q / out [batch, n_q * 128], k / v [batch, n_kv * 128], the cache arrays of cc [batch, n_kv, L, .].
+// part: [batch, n_kv, S, G, 2 + 128] floats (m, l, o per head), tickets: [batch, n_kv] uint32, zero between launches.
+// SEQPOS: sequence b at its own position pos_p[b]; its chunk, staged rows, RoPE row and written row follow it (S stays fixed).
+// PAGED (SEQPOS only): the cache arrays are page pools [pages, n_kv, 64, .]; a tile's rows are found with one read of the table row.
+template <typename T, class Cache, bool SEQPOS = false, bool PAGED = false>
+__global__ void __launch_bounds__(kSplitThreads, 1)
+    rope_attn_decode_split_kernel(const T* __restrict__ q_in, const T* __restrict__ k_in, const T* __restrict__ v_in, const T* __restrict__ cos_t,
+                                  const T* __restrict__ sin_t, Cache cc, const long long* __restrict__ pos_p, T* __restrict__ out,
+                                  float* __restrict__ part, unsigned* __restrict__ tickets, int n_q, int n_kv, int L, float scale_log2,
+                                  const PageArg<PAGED> pg) {
+  extern __shared__ __align__(16) char smem[];
+  constexpr int NW = kSplitWarps, ST = Cache::kStages, CH = Cache::kRowBytes / 16;  // CH: 16-byte chunks a level row
+  static_assert(NW * kSplitMaxGroup * kPartFloats * 4 <= Cache::kRingBytes, "the warp partials reuse the ring");
+  static_assert(SEQPOS || !PAGED, "a paged cache needs per-sequence positions");
+  const int S = (int)gridDim.x, split = (int)blockIdx.x, kvh = (int)blockIdx.y, b = (int)blockIdx.z;
+  const int G = n_q / n_kv;
+  const int tid = (int)threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, qd = lane & 3;
+  const int* tab = nullptr;
+  if constexpr (PAGED) tab = pg.table + (long long)b * (L / kPage);
   {
-    float* w0 = wp + (warp * kSplitMaxGroup + 2 * qd) * kPartFloats;
-    float* w1 = w0 + kPartFloats;
-    if (g == 0) { w0[0] = m0; w0[1] = l0; w1[0] = m1; w1[1] = l1; }
+    const long long kv = (long long)b * n_kv + kvh;
+    if constexpr (!PAGED) cc.advance(kv, L);
+    k_in += kv * kHd; v_in += kv * kHd;
+    q_in += ((long long)b * n_q + (long long)kvh * G) * kHd; out += ((long long)b * n_q + (long long)kvh * G) * kHd;
+    part += kv * S * G * kPartFloats;
+    tickets += kv;
+  }
+  char* ring = smem + warp * ST * Cache::kStageBytes;
+  T* qs = reinterpret_cast<T*>(smem + Cache::kRingBytes);  // rotated q [8][128]
+  T* kf = qs + kSplitMaxGroup * kHd;                        // rotated k and v of position pos
+  T* vf = kf + kHd;
+  char* fx = reinterpret_cast<char*>(vf + kHd);  // the format's fresh row pos, if the rotated rows are not that
+  const char* fr = Cache::kFreshBytes ? fx : reinterpret_cast<const char*>(kf);  // fresh K levels, the V levels kRowBytes later
+  int* last = reinterpret_cast<int*>(fx + Cache::kFreshBytes);
+
+  // *pos was written by a completed launch (the step's final, non-programmatic kernel): it may be read before the wait
+  const int pos = (int)pos_p[SEQPOS ? b : 0], n_pos = pos + 1;
+  const int chunk = (((n_pos + S - 1) / S) + kSplitTile - 1) / kSplitTile * kSplitTile;
+  const int c0 = min(split * chunk, n_pos), c1 = min(c0 + chunk, n_pos);
+  const int n_tiles = (c1 - c0 + kSplitTile - 1) / kSplitTile;
+  const int my_tiles = warp < n_tiles ? (n_tiles - warp + NW - 1) / NW : 0;  // tiles warp, warp + NW, ... of the chunk
+  pdl_launch_dependents();
+
+  // Stage local tile i into its ring slot: rows < pos from the cache (cp.async), row pos from this launch's fresh row once `fresh`
+  // (the cache row is written by another CTA of this launch), rows past pos zero (finite: their probability is 0).
+  auto issue = [&](int i, bool fresh) {
+    if (i < my_tiles) {
+      const int t0 = c0 + (warp + i * NW) * kSplitTile;
+      char* st = ring + (i % ST) * Cache::kStageBytes;
+      long long rt = 0;  // cache row of position 0 of the tile's page, minus the page's first position
+      if constexpr (PAGED) rt = page_row(tab, n_kv, kvh, t0) - t0;
+#pragma unroll 4
+      for (int j = lane; j < 2 * kSplitTile * CH; j += 32) {
+        const int isv = j / (kSplitTile * CH), r = (j / CH) % kSplitTile, c = j % CH, p = t0 + r;
+        char* dst = st + isv * Cache::kLvlBytes + Cache::slot(r, c);
+        if (p < pos) {
+          split_cp16(dst, reinterpret_cast<const char*>(isv ? cc.v : cc.k) + (rt + p) * Cache::kRowBytes + c * 16);
+        } else if (p > pos || fresh) {
+          uint4 val;
+          val.x = val.y = val.z = val.w = 0u;
+          if (p == pos) val = *reinterpret_cast<const uint4*>(fr + isv * Cache::kRowBytes + c * 16);
+          *reinterpret_cast<uint4*>(dst) = val;
+        }
+      }
+      cc.stage_meta(st, rt, t0, pos, lane, fresh, fx);
+    }
+    split_commit();  // always (possibly empty): every iteration waits on the same group count
+  };
+  // cache rows < pos were written by earlier launches: the first ST - 1 tiles stream in under the previous kernel's tail
 #pragma unroll
-    for (int mt = 0; mt < 8; ++mt) {  // O^T rows g, g + 8 of step mt are dims 8 g + mt, 64 + 8 g + mt
-      w0[2 + 8 * g + mt] = o[mt][0]; w1[2 + 8 * g + mt] = o[mt][1];
-      w0[2 + 64 + 8 * g + mt] = o[mt][2]; w1[2 + 64 + 8 * g + mt] = o[mt][3];
+  for (int i = 0; i < ST - 1; ++i) issue(i, false);
+  pdl_wait();
+
+  for (int i = tid; i < (G + 1) * kHd; i += kSplitThreads) {
+    const int h = i >> 7, d = i & (kHd - 1);
+    const T r = rope_rounded<T>(h < G ? q_in + h * kHd : k_in, d, cos_t + (long long)pos * kHd, sin_t + (long long)pos * kHd);
+    if (h < G) {
+      qs[h * kHd + d] = r;
+    } else {
+      kf[d] = r;
+      vf[d] = v_in[d];
     }
   }
   __syncthreads();
-  split_merge<T>(wp, part, tickets, out, last, S, split, G, tid);
+  long long pr = pos;  // cache row of position pos: one writer per (sequence, kv head), split 0
+  if constexpr (PAGED) {
+    if (split == 0) pr = page_row(tab, n_kv, kvh, pos);
+  }
+  cc.fresh(kf, fx, split == 0, pr, tid);
+  if (pos >= c0 && pos < c1) {  // row pos in a tile staged before the wait: its owner fills it in now
+    const int ti = (pos - c0) / kSplitTile, i = ti / NW;
+    if (ti % NW == warp && i < ST - 1) {
+      const int r = pos - (c0 + ti * kSplitTile);
+      char* st = ring + (i % ST) * Cache::kStageBytes;
+      if (lane < 2 * CH) {
+        const int isv = lane / CH, c = lane % CH;
+        *reinterpret_cast<uint4*>(st + isv * Cache::kLvlBytes + Cache::slot(r, c)) = *reinterpret_cast<const uint4*>(fr + isv * Cache::kRowBytes + c * 16);
+      }
+      cc.patch_meta(st, r, lane, fx);
+    }
+  }
+  // Q^T fragments (B operand of the score MMA, n = head g) in the format's dims
+  uint32_t qb[8][2];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+    const T* qr = qs + g * kHd + Cache::qdim(kk, qd);
+    qb[kk][0] = g < G ? *reinterpret_cast<const uint32_t*>(qr) : 0u;
+    qb[kk][1] = g < G ? *reinterpret_cast<const uint32_t*>(qr + Cache::kQPair) : 0u;
+  }
+
+  // lane (g, qd) holds the running max / sum of heads 2 qd, 2 qd + 1 and O^T rows g (+ 8) of each step mt of those heads
+  float o[8][4];
+#pragma unroll
+  for (int mt = 0; mt < 8; ++mt) o[mt][0] = o[mt][1] = o[mt][2] = o[mt][3] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  for (int i = 0; i < my_tiles; ++i) {
+    __syncwarp();  // every lane is done with the slot the next issue overwrites
+    issue(i + ST - 1, true);
+    split_wait<ST - 1>();
+    __syncwarp();  // this tile's copies and plain stores of every lane are visible to the warp
+    const char* st = ring + (i % ST) * Cache::kStageBytes;
+    float s[4] = {0.f, 0.f, 0.f, 0.f};
+    cc.scores(s, st, qb, lane);
+    uint32_t b0, b1;  // every tile holds position c0 + 16 j < c1
+    softmax_tile<T, false>(s, scale_log2, c0 + (warp + i * NW) * kSplitTile + g, c1, c1, m, l, o, g, qd, b0, b1);
+    cc.pv(o, st, b0, b1, lane);
+  }
+  split_wait<0>();
+  __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][8][m, l, o[128]]
+  float* wp = reinterpret_cast<float*>(smem);
+  put_partial<Cache>(wp + (warp * kSplitMaxGroup + 2 * qd) * kPartFloats, m, l, o, g);
+  __syncthreads();
+  split_merge<T, kSplitMaxGroup>(wp, part, tickets, last, S, split, G, G, tid, [&](int h) { return out + h * kHd; });
 }
 
 int split_count(int n_kv, int cache_len) {
@@ -1448,32 +1181,7 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
     const int p0 = c0 + (warp + i * NW) * kSplitTile + g;
     uint32_t pb[NT][2];
 #pragma unroll
-    for (int j = 0; j < NT; ++j) {
-      const float x0 = p0 < lim[j][0] ? s[j][0] * scale_log2 : -INFINITY, x1 = p0 < lim[j][1] ? s[j][1] * scale_log2 : -INFINITY;
-      const float x2 = p0 + 8 < lim[j][0] ? s[j][2] * scale_log2 : -INFINITY, x3 = p0 + 8 < lim[j][1] ? s[j][3] * scale_log2 : -INFINITY;
-      float t0 = fmaxf(x0, x2), t1 = fmaxf(x1, x3);
-#pragma unroll
-      for (int off = 4; off < 32; off <<= 1) {
-        t0 = fmaxf(t0, __shfl_xor_sync(0xffffffffu, t0, off));
-        t1 = fmaxf(t1, __shfl_xor_sync(0xffffffffu, t1, off));
-      }
-      const float n0 = fmaxf(m[j][0], t0), n1 = fmaxf(m[j][1], t1);
-      const float r0 = n0 == -INFINITY ? 0.f : n0, r1 = n1 == -INFINITY ? 0.f : n1;  // no key of the column yet: everything stays 0
-      const float a0 = exp2f(m[j][0] - r0), a1 = exp2f(m[j][1] - r1);
-      m[j][0] = n0; m[j][1] = n1;
-      const T p00 = from_f32<T>(exp2f(x0 - r0)), p01 = from_f32<T>(exp2f(x1 - r1));
-      const T p10 = from_f32<T>(exp2f(x2 - r0)), p11 = from_f32<T>(exp2f(x3 - r1));
-      l[j][0] = l[j][0] * a0 + (to_f32<T>(p00) + to_f32<T>(p10));
-      l[j][1] = l[j][1] * a1 + (to_f32<T>(p01) + to_f32<T>(p11));
-#pragma unroll
-      for (int mt = 0; mt < 8; ++mt) { o[j][mt][0] *= a0; o[j][mt][1] *= a1; o[j][mt][2] *= a0; o[j][mt][3] *= a1; }
-      const uint32_t lo = bits16(p00) | (bits16(p01) << 16), hi = bits16(p10) | (bits16(p11) << 16);
-      const int src = 8 * qd + (g >> 1), sh = (g & 1) * 16;
-      const uint32_t lo0 = __shfl_sync(0xffffffffu, lo, src), lo1 = __shfl_sync(0xffffffffu, lo, src + 4);
-      const uint32_t hi0 = __shfl_sync(0xffffffffu, hi, src), hi1 = __shfl_sync(0xffffffffu, hi, src + 4);
-      pb[j][0] = ((lo0 >> sh) & 0xFFFFu) | (((lo1 >> sh) & 0xFFFFu) << 16);
-      pb[j][1] = ((hi0 >> sh) & 0xFFFFu) | (((hi1 >> sh) & 0xFFFFu) << 16);
-    }
+    for (int j = 0; j < NT; ++j) softmax_tile<T, true>(s[j], scale_log2, p0, lim[j][0], lim[j][1], m[j], l[j], o[j], g, qd, pb[j][0], pb[j][1]);
 #pragma unroll
     for (int mt = 0; mt < 8; ++mt) {
       uint32_t a[4];
@@ -1483,66 +1191,15 @@ __global__ void __launch_bounds__(kSplitThreads, 1)
     }
   }
   split_wait<0>();
-#pragma unroll
-  for (int j = 0; j < NT; ++j) {
-#pragma unroll
-    for (int off = 4; off < 32; off <<= 1) {
-      l[j][0] += __shfl_xor_sync(0xffffffffu, l[j][0], off);
-      l[j][1] += __shfl_xor_sync(0xffffffffu, l[j][1], off);
-    }
-  }
   __syncthreads();  // every warp is done with the ring: it now holds the warp partials [NW][NC][m, l, o[128]]
   float* wp = reinterpret_cast<float*>(smem);
 #pragma unroll
-  for (int j = 0; j < NT; ++j) {
-    float* w0 = wp + (warp * NC + 8 * j + 2 * qd) * kPartFloats;
-    float* w1 = w0 + kPartFloats;
-    if (g == 0) { w0[0] = m[j][0]; w0[1] = l[j][0]; w1[0] = m[j][1]; w1[1] = l[j][1]; }
-#pragma unroll
-    for (int mt = 0; mt < 8; ++mt) {
-      w0[2 + 16 * mt + g] = o[j][mt][0]; w1[2 + 16 * mt + g] = o[j][mt][1];
-      w0[2 + 16 * mt + g + 8] = o[j][mt][2]; w1[2 + 16 * mt + g + 8] = o[j][mt][3];
-    }
-  }
+  for (int j = 0; j < NT; ++j) put_partial<KvF16<T>>(wp + (warp * NC + 8 * j + 2 * qd) * kPartFloats, m[j], l[j], o[j], g);
   __syncthreads();
-  const int nc = min(NC, C - cg * NC);  // this CTA's real columns
-  for (int i = tid; i < nc * kHd; i += kSplitThreads) {
-    const int c = i >> 7, d = i & (kHd - 1);
-    float M = -INFINITY;
-    for (int w = 0; w < NW; ++w) M = fmaxf(M, wp[(w * NC + c) * kPartFloats]);
-    float lsum = 0.f, osum = 0.f;
-    if (M != -INFINITY) {
-      for (int w = 0; w < NW; ++w) {
-        const float* e = wp + (w * NC + c) * kPartFloats;
-        const float f = exp2f(e[0] - M);
-        lsum += f * e[1];
-        osum += f * e[2 + d];
-      }
-    }
-    float* dst = part + ((long long)split * NC + c) * kPartFloats;
-    if (d == 0) { dst[0] = M; dst[1] = lsum; }
-    dst[2 + d] = osum;
-  }
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) *last = atomicAdd(tickets, 1u) == (unsigned)(S - 1);
-  __syncthreads();
-  if (!*last) return;
-  __threadfence();
-  for (int i = tid; i < nc * kHd; i += kSplitThreads) {  // split 0 holds key 0, which every column sees: M is finite
-    const int c = i >> 7, d = i & (kHd - 1), col = cg * NC + c;
-    float M = -INFINITY;
-    for (int sp = 0; sp < S; ++sp) M = fmaxf(M, __ldcg(part + ((long long)sp * NC + c) * kPartFloats));
-    float lsum = 0.f, osum = 0.f;
-    for (int sp = 0; sp < S; ++sp) {
-      const float* e = part + ((long long)sp * NC + c) * kPartFloats;
-      const float f = exp2f(__ldcg(e) - M);
-      lsum += f * __ldcg(e + 1);
-      osum += f * __ldcg(e + 2 + d);
-    }
-    out[(((long long)b * TQ + col / G) * n_q + (long long)kvh * G + col % G) * kHd + d] = from_f32<T>(osum / lsum);
-  }
-  if (tid == 0) *tickets = 0u;
+  split_merge<T, NC>(wp, part, tickets, last, S, split, NC, min(NC, C - cg * NC), tid, [&](int c) {  // this CTA's real columns
+    const int col = cg * NC + c;
+    return out + (((long long)b * TQ + col / G) * n_q + (long long)kvh * G + col % G) * kHd;
+  });
 }
 
 // Prompt-lookup drafts (DESIGN.md 3.5).  Slot b knows n = pos[b] + 1 tokens: hist[b][0 .. pos - 1] and tok[b] at pos.  Take the
@@ -1692,15 +1349,10 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
   if constexpr (PAGED) c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
   pdl_launch_dependents();
   pdl_wait();
-  constexpr int half = kHd / 2;
   for (int i = (int)threadIdx.x; i < (n_q + 2 * n_kv) * kHd; i += (int)blockDim.x) {
     const int h = i >> 7, d = i & (kHd - 1);
-    if (h < n_q + n_kv) {  // x*cos + rotate_half(x)*sin, each product and the sum rounded to T (rope_attn_decode_kernel)
-      const float c = to_f32<T>(cos_t[(long long)p * kHd + d]), s = to_f32<T>(sin_t[(long long)p * kHd + d]);
-      const T* x = h < n_q ? q + h * kHd : k + (h - n_q) * kHd;
-      const float xv = to_f32<T>(x[d]);
-      const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
-      const T r = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
+    if (h < n_q + n_kv) {
+      const T r = rope_rounded<T>(h < n_q ? q + h * kHd : k + (h - n_q) * kHd, d, cos_t + (long long)p * kHd, sin_t + (long long)p * kHd);
       if (h < n_q) q_out[h * kHd + d] = r;
       else if constexpr (PAGED) k_cache[(c0 + (long long)(h - n_q) * kPage) * kHd + d] = r;
       else k_cache[((long long)(h - n_q) * L + p) * kHd + d] = r;
@@ -1712,13 +1364,13 @@ __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restri
   }
 }
 
-// Prefill into an 8-bit cache: rope_append_rows_kernel's RoPE, then every k and v row quantised as the kv8 decode kernel quantises
-// row pos (the same levels and meta bit for bit), and its dequantisation written to the staging caches at the same row.
+// Prefill into an 8-bit cache: rope_append_rows_kernel's RoPE, then every k and v row quantised by kv_quant_row, as the split decode
+// kernel quantises row pos (the same levels and meta bit for bit), and its dequantisation written to the staging caches at the same row.
 // grid = (T, batch), block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position (k and v of each kv head).
 // Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.  VARLEN as
 // rope_append_rows_kernel.  PAGED as there: levels and meta in the page pools, the staging pair stays [batch, n_kv, L, 128].
 // DEVPOS as rope_append_rows_kernel (positions from the device, rows past the cache end skipped); it writes no staging rows (k_st /
-// v_st unused): the verify attention dequantises the cache itself.  BITS 4: the 4-bit cache (rope_attn_decode_split_kv4_kernel's
+// v_st unused): the verify attention dequantises the cache itself.  BITS 4: the 4-bit cache (the split decode kernel's
 // quantisation and packing, levels [.., 64]).
 template <typename T, bool VARLEN = false, bool PAGED = false, bool DEVPOS = false, int BITS = 8>
 __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
@@ -1756,47 +1408,23 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
   if constexpr (PAGED) c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
   pdl_launch_dependents();
   pdl_wait();
-  constexpr int half = kHd / 2;
+  const T* cs = cos_t + (long long)p * kHd;
+  const T* sn = sin_t + (long long)p * kHd;
   for (int i = (int)threadIdx.x; i < n_q * kHd; i += (int)blockDim.x) {  // rope(q) as rope_append_rows_kernel
     const int h = i >> 7, d = i & (kHd - 1);
-    const float c = to_f32<T>(cos_t[(long long)p * kHd + d]), s = to_f32<T>(sin_t[(long long)p * kHd + d]);
-    const T* x = q + h * kHd;
-    const float xv = to_f32<T>(x[d]);
-    const float xr = (d < half) ? -to_f32<T>(x[d + half]) : to_f32<T>(x[d - half]);
-    q_out[h * kHd + d] = from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s)));
+    q_out[h * kHd + d] = rope_rounded<T>(q + h * kHd, d, cs, sn);
   }
   const int warp = (int)threadIdx.x >> 5, lane = (int)threadIdx.x & 31;
   for (int r = warp; r < 2 * n_kv; r += (int)blockDim.x >> 5) {
     const int kvh = r >> 1, isv = r & 1;
     float x[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int d = 4 * lane + j;
-      if (isv) {
-        x[j] = to_f32<T>(v[kvh * kHd + d]);
-      } else {
-        const float c = to_f32<T>(cos_t[(long long)p * kHd + d]), s = to_f32<T>(sin_t[(long long)p * kHd + d]);
-        const T* xk = k + kvh * kHd;
-        const float xv = to_f32<T>(xk[d]);
-        const float xr = (d < half) ? -to_f32<T>(xk[d + half]) : to_f32<T>(xk[d - half]);
-        x[j] = to_f32<T>(from_f32<T>(to_f32<T>(from_f32<T>(xv * c)) + to_f32<T>(from_f32<T>(xr * s))));
-      }
-    }
-    T sc, ze;
-    const uint32_t lv = kv8_quant4<T, (1 << BITS) - 1>(x, gs, sc, ze);
+    for (int j = 0; j < 4; ++j) x[j] = to_f32<T>(isv ? v[kvh * kHd + 4 * lane + j] : rope_rounded<T>(k + kvh * kHd, 4 * lane + j, cs, sn));
     const long long row = (long long)kvh * L + p;
     long long crow = row;
     if constexpr (PAGED) crow = c0 + (long long)kvh * kPage;
-    if constexpr (BITS == 8) {
-      *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + crow * kHd + 4 * lane) = lv;
-    } else {
-      const uint32_t pk = kv4_pack(lv);
-      if (lane < 16) *reinterpret_cast<uint32_t*>((isv ? v_q : k_q) + crow * LB + 4 * lane) = pk;
-    }
-    if ((4 * lane) % gs == 0) {
-      (isv ? v_s : k_s)[crow * ng + 4 * lane / gs] = sc;
-      (isv ? v_z : k_z)[crow * ng + 4 * lane / gs] = ze;
-    }
+    T sc, ze;
+    const uint32_t lv = kv_quant_row<T, BITS>(x, gs, (isv ? v_q : k_q) + crow * LB, (isv ? v_s : k_s) + crow * ng, (isv ? v_z : k_z) + crow * ng, sc, ze);
     typename Pair<T>::type s2, z2;
     s2.x = s2.y = sc;
     z2.x = z2.y = ze;
@@ -2527,74 +2155,6 @@ extern "C" size_t hqq_b200_glue_rope_attn_decode_split_workspace_bytes(int n_q_h
   return groups * s_max * (size_t)(n_q_heads / n_kv_heads) * (size_t)(head_dim + 2) * sizeof(float) + groups * sizeof(unsigned);
 }
 
-template <typename T, bool SEQPOS, bool PAGED>
-static int launch_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache, void* v_cache,
-                               const int64_t* pos, void* out, float* part, unsigned* tickets, int n_q_heads, int n_kv_heads, int cache_len,
-                               float scale_log2, dim3 grid, cudaStream_t st, PageArg<PAGED> pg) {
-  if (int rc = reserve_smem<rope_attn_decode_split_kernel<T, SEQPOS, PAGED>>(kSmemBytes)) return rc;
-  return launch_pdl("rope_attn_decode_split", rope_attn_decode_split_kernel<T, SEQPOS, PAGED>, grid, dim3(kSplitThreads), kSmemBytes, st, (const T*)q,
-                    (const T*)k, (const T*)v, (const T*)cos_table, (const T*)sin_table, (T*)k_cache, (T*)v_cache, (const long long*)pos, (T*)out,
-                    part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2, pg);
-}
-
-// table == nullptr: contiguous caches; else page pools (seqpos only)
-static int rope_attn_decode_split(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
-                                  const void* sin_table, void* k_cache, void* v_cache, const int* table, const int64_t* pos, void* out, void* workspace,
-                                  int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && pos && out && workspace, HQQ_E_INVALID, "%s: null pointer", name);
-  HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
-  HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0, HQQ_E_INVALID, "%s: workspace must be 4-byte aligned", name);
-  HQQ_REQUIRE(head_dim == kHd && n_kv_heads > 0 && n_kv_heads <= 65535 && n_q_heads % n_kv_heads == 0 && n_q_heads / n_kv_heads >= 1 &&
-                  n_q_heads / n_kv_heads <= kSplitMaxGroup && cache_len > 0 && cache_len <= kSplitMaxLen,
-              HQQ_E_UNSUPPORTED, "%s: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072", name);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int S = split_count(n_kv_heads, cache_len);
-  const int G = n_q_heads / n_kv_heads;
-  const size_t part_bytes = (size_t)batch * n_kv_heads * max(1, sm_count() / n_kv_heads) * G * kPartFloats * sizeof(float);
-  float* part = (float*)workspace;
-  unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
-  const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
-  const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
-  auto go = [&](auto f, auto pg) {
-    return f(q, k, v, cos_table, sin_table, k_cache, v_cache, pos, out, part, tickets, n_q_heads, n_kv_heads, cache_len, scale_log2, grid, st, pg);
-  };
-  const PageTable pt{table};
-  if (dtype == HQQ_F16) {
-    if (table) return go(launch_decode_split<__half, true, true>, pt);
-    return seqpos ? go(launch_decode_split<__half, true, false>, NoPages()) : go(launch_decode_split<__half, false, false>, NoPages());
-  }
-  if (dtype == HQQ_BF16) {
-    if (table) return go(launch_decode_split<__nv_bfloat16, true, true>, pt);
-    return seqpos ? go(launch_decode_split<__nv_bfloat16, true, false>, NoPages()) : go(launch_decode_split<__nv_bfloat16, false, false>, NoPages());
-  }
-  set_error("%s: dtype must be f16/bf16", name);
-  return HQQ_E_INVALID;
-}
-
-extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                    void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
-                                                    int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split", false, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, pos, out,
-                                workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
-}
-
-extern "C" int hqq_b200_glue_rope_attn_decode_split_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                           void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
-                                                           int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_seqpos", true, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, pos, out,
-                                workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
-}
-
-extern "C" int hqq_b200_glue_rope_attn_decode_split_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                          void* k_pool, void* v_pool, const int* table, const int64_t* pos, void* out, void* workspace,
-                                                          int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
-                                                          void* stream) {
-  const char* name = "hqq_b200_glue_rope_attn_decode_split_paged";
-  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  return rope_attn_decode_split(name, true, q, k, v, cos_table, sin_table, k_pool, v_pool, table, pos, out, workspace, n_q_heads, n_kv_heads, cache_len,
-                                head_dim, batch, dtype, stream);
-}
-
 // The group sizes of a quantised cache: 64 or 128 for 8 bits, 32 or 64 for 4 bits (a 4-bit row of one group has no 4bit_u8 packing)
 static int kv_group_args(const char* name, int bits, int group_size) {
   if (bits == 8) {
@@ -2605,20 +2165,30 @@ static int kv_group_args(const char* name, int bits, int group_size) {
   return HQQ_OK;
 }
 
-// table == nullptr: contiguous caches; else page pools (seqpos only).  bits 8 or 4.
-static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
-                                      const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
-                                      const int* table, const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
-                                      int group_size, int batch, int dtype, void* stream, int bits = 8) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && pos && out && workspace, HQQ_E_INVALID,
-              "%s: null pointer", name);
+// bits 16: k_cache / v_cache are the 16-bit caches (meta, gs unused); bits 8 or 4: they are the HQQ level caches, meta = {k_scale,
+// k_zero, v_scale, v_zero} and gs their group size.  table == nullptr: contiguous caches; else page pools (seqpos only).
+static int rope_attn_decode_split(const char* name, int bits, bool seqpos, const void* q, const void* k, const void* v, const void* cos_table,
+                                  const void* sin_table, void* k_cache, void* v_cache, void* const* meta, int gs, const int* table, const int64_t* pos,
+                                  void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int dtype,
+                                  void* stream) {
+  const bool quant = bits != 16;
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && (!quant || (meta[0] && meta[1] && meta[2] && meta[3])) && pos && out &&
+                  workspace,
+              HQQ_E_INVALID, "%s: null pointer", name);
   HQQ_REQUIRE(batch > 0 && batch <= 65535, HQQ_E_INVALID, "%s: batch %d", name, batch);
-  HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0 && ((uintptr_t)k_q & 15) == 0 && ((uintptr_t)v_q & 15) == 0, HQQ_E_INVALID,
-              "%s: workspace must be 4-byte and the level caches 16-byte aligned", name);
+  if (quant) {
+    HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0 && ((uintptr_t)k_cache & 15) == 0 && ((uintptr_t)v_cache & 15) == 0, HQQ_E_INVALID,
+                "%s: workspace must be 4-byte and the level caches 16-byte aligned", name);
+  } else {
+    HQQ_REQUIRE(((uintptr_t)workspace & 3) == 0, HQQ_E_INVALID, "%s: workspace must be 4-byte aligned", name);
+  }
   HQQ_REQUIRE(head_dim == kHd && n_kv_heads > 0 && n_kv_heads <= 65535 && n_q_heads % n_kv_heads == 0 && n_q_heads / n_kv_heads >= 1 &&
                   n_q_heads / n_kv_heads <= kSplitMaxGroup && cache_len > 0 && cache_len <= kSplitMaxLen,
-              HQQ_E_UNSUPPORTED, "%s: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072, group_size 64 or 128", name);
-  if (int rc = kv_group_args(name, bits, group_size)) return rc;
+              HQQ_E_UNSUPPORTED, "%s: needs head_dim 128, n_q_heads / n_kv_heads <= 8, cache_len <= 131072%s", name,
+              quant ? ", group_size 64 or 128" : "");
+  if (quant) {
+    if (int rc = kv_group_args(name, bits, gs)) return rc;
+  }
   cudaStream_t st = (cudaStream_t)stream;
   const int S = split_count(n_kv_heads, cache_len);
   const int G = n_q_heads / n_kv_heads;
@@ -2627,22 +2197,23 @@ static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void*
   unsigned* tickets = (unsigned*)((char*)workspace + part_bytes);
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)head_dim);
   const dim3 grid((unsigned)S, (unsigned)n_kv_heads, (unsigned)batch);
-  auto go = [&](auto tag, auto sp, auto pg) {
+  auto launch = [&](auto tag, auto sp, auto pg, auto cache) {
     using E = decltype(tag);
+    using C = decltype(cache);
     constexpr bool SP = decltype(sp)::value;
     constexpr bool PG = std::is_same<decltype(pg), PageTable>::value;
-    if (bits == 4) {
-      if (int rc = reserve_smem<rope_attn_decode_split_kv4_kernel<E, SP, PG>>(kKv4SmemBytes)) return rc;
-      return launch_pdl("rope_attn_decode_split_kv4", rope_attn_decode_split_kv4_kernel<E, SP, PG>, grid, dim3(kSplitThreads), kKv4SmemBytes, st,
-                        (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
-                        (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, group_size,
-                        scale_log2, pg);
-    }
-    if (int rc = reserve_smem<rope_attn_decode_split_kv8_kernel<E, SP, PG>>(kKv8SmemBytes)) return rc;
-    return launch_pdl("rope_attn_decode_split_kv8", rope_attn_decode_split_kv8_kernel<E, SP, PG>, grid, dim3(kSplitThreads), kKv8SmemBytes, st,
-                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero,
-                      (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len, group_size,
+    if (int rc = reserve_smem<rope_attn_decode_split_kernel<E, C, SP, PG>>(C::kSmemBytes)) return rc;
+    return launch_pdl(bits == 16 ? "rope_attn_decode_split" : bits == 8 ? "rope_attn_decode_split_kv8" : "rope_attn_decode_split_kv4",
+                      rope_attn_decode_split_kernel<E, C, SP, PG>, grid, dim3(kSplitThreads), C::kSmemBytes, st, (const E*)q, (const E*)k, (const E*)v,
+                      (const E*)cos_table, (const E*)sin_table, cache, (const long long*)pos, (E*)out, part, tickets, n_q_heads, n_kv_heads, cache_len,
                       scale_log2, pg);
+  };
+  auto go = [&](auto tag, auto sp, auto pg) {
+    using E = decltype(tag);
+    if (bits == 16) return launch(tag, sp, pg, KvF16<E>{(E*)k_cache, (E*)v_cache});
+    if (bits == 8)
+      return launch(tag, sp, pg, KvHqq<E, 8>{(uint8_t*)k_cache, (E*)meta[0], (E*)meta[1], (uint8_t*)v_cache, (E*)meta[2], (E*)meta[3], gs, kHd / gs});
+    return launch(tag, sp, pg, KvHqq<E, 4>{(uint8_t*)k_cache, (E*)meta[0], (E*)meta[1], (uint8_t*)v_cache, (E*)meta[2], (E*)meta[3], gs, kHd / gs});
   };
   const PageTable pt{table};
   if (dtype == HQQ_F16) {
@@ -2657,20 +2228,46 @@ static int rope_attn_decode_split_kv8(const char* name, bool seqpos, const void*
   return HQQ_E_INVALID;
 }
 
+extern "C" int hqq_b200_glue_rope_attn_decode_split(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                    void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                    int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split", 16, false, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, 0,
+                                nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                           void* k_cache, void* v_cache, const int64_t* pos, void* out, void* workspace, int n_q_heads,
+                                                           int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_seqpos", 16, true, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, 0,
+                                nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_attn_decode_split_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                          void* k_pool, void* v_pool, const int* table, const int64_t* pos, void* out, void* workspace,
+                                                          int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
+                                                          void* stream) {
+  const char* name = "hqq_b200_glue_rope_attn_decode_split_paged";
+  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  return rope_attn_decode_split(name, 16, true, q, k, v, cos_table, sin_table, k_pool, v_pool, nullptr, 0, table, pos, out, workspace, n_q_heads,
+                                n_kv_heads, cache_len, head_dim, batch, dtype, stream);
+}
+
 extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
                                                         const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
                                                         int head_dim, int group_size, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv8", false, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
-                                    v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_kv8", 8, false, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size,
+                                nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                                void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
                                                                const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
                                                                int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv8_seqpos", true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q,
-                                    v_scale, v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_kv8_seqpos", 8, true, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size,
+                                nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
@@ -2679,25 +2276,27 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_kv8_paged(const void* q, con
                                                               int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
   const char* name = "hqq_b200_glue_rope_attn_decode_split_kv8_paged";
   if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  return rope_attn_decode_split_kv8(name, true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, pos, out, workspace,
-                                    n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_attn_decode_split(name, 8, true, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size, table, pos, out, workspace, n_q_heads,
+                                n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
                                                         const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads, int cache_len,
                                                         int head_dim, int group_size, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv4", false, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
-                                    v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_kv4", 4, false, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size,
+                                nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4_seqpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                                void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
                                                                const int64_t* pos, void* out, void* workspace, int n_q_heads, int n_kv_heads,
                                                                int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
-  return rope_attn_decode_split_kv8("hqq_b200_glue_rope_attn_decode_split_kv4_seqpos", true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q,
-                                    v_scale, v_zero, nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream,
-                                    4);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_attn_decode_split("hqq_b200_glue_rope_attn_decode_split_kv4_seqpos", 4, true, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size,
+                                nullptr, pos, out, workspace, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
@@ -2706,8 +2305,9 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4_paged(const void* q, con
                                                               int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
   const char* name = "hqq_b200_glue_rope_attn_decode_split_kv4_paged";
   if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  return rope_attn_decode_split_kv8(name, true, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, pos, out, workspace,
-                                    n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_attn_decode_split(name, 4, true, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size, table, pos, out, workspace, n_q_heads,
+                                n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
 // The fixed-length (pos0_v == nullptr: uniform pos0, T) and variable-length (host pos0_v / n_tok_v) appends into a quantised cache
