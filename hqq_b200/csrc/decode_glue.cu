@@ -1771,10 +1771,21 @@ __device__ __forceinline__ unsigned long long sample_counter(PosKeys k, uint32_t
   return (unsigned long long)(0x80000000u | ((uint32_t)__ldg(k.seq + slot) & 0x7FFFFFFFu)) << 32 | p;
 }
 
-template <typename T, typename Keys>
-__global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __restrict__ logits, int n, long long ld, float temperature, int top_k,
-                                                                float top_p, uint32_t seed_lo, uint32_t seed_hi, Keys keys,
-                                                                long long* __restrict__ out) {
+// A row's temperature, top_k and top_p.  ScalarParams (hqq_b200_glue_sample, _pos): one set for the launch, by value.  SlotParams
+// (hqq_b200_glue_sample_slots): device arrays indexed by the slot r / T, read after the PDL wait; temperature 0 asks for the argmax.
+struct ScalarParams { float temperature; int top_k; float top_p; static constexpr bool kSlots = false; };
+struct SlotParams { const float* temperature; const int* top_k; const float* top_p; int T; static constexpr bool kSlots = true; };
+
+__device__ __forceinline__ void sample_params(ScalarParams p, uint32_t, float& t, int& k, float& tp) { t = p.temperature; k = p.top_k; tp = p.top_p; }
+
+__device__ __forceinline__ void sample_params(SlotParams p, uint32_t row, float& t, int& k, float& tp) {
+  const uint32_t slot = row / (uint32_t)p.T;
+  t = __ldg(p.temperature + slot); k = __ldg(p.top_k + slot); tp = __ldg(p.top_p + slot);
+}
+
+template <typename T, typename Keys, typename Params>
+__global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __restrict__ logits, int n, long long ld, Params params, uint32_t seed_lo,
+                                                                uint32_t seed_hi, Keys keys, long long* __restrict__ out) {
   __shared__ unsigned cnt_hi[256], cnt_lo[256];
   __shared__ unsigned long long mass_hi[256], mass_lo[256], best_lo[256], red[32];
   __shared__ unsigned max_key;
@@ -1783,11 +1794,15 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __re
   const int tid = threadIdx.x;
   const uint32_t row = blockIdx.x;
   const T* x = logits + (long long)row * ld;
-  const bool use_k = top_k > 0 && top_k < n, use_p = top_p < 1.0f;
   for (int i = tid; i < 256; i += kSampleThreads) { cnt_hi[i] = 0; cnt_lo[i] = 0; mass_hi[i] = 0; mass_lo[i] = 0; best_lo[i] = 0; }
   if (tid == 0) { max_key = 0; sel_bin = 0; sel_above = 0; }
   pdl_launch_dependents();
   pdl_wait();
+  float temperature, top_p;
+  int top_k;
+  sample_params(params, row, temperature, top_k, top_p);
+  const bool greedy = Params::kSlots && temperature == 0.0f;  // the race below takes the largest value, first index on ties
+  const bool use_k = !greedy && top_k > 0 && top_k < n, use_p = !greedy && top_p < 1.0f;
   uint32_t word1;
   const unsigned long long ctr = sample_counter(keys, row, word1);  // counter words 2, 3
   __syncthreads();
@@ -1880,6 +1895,11 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __re
   const float m_p = split >= 0 ? sample_key_value<T>(max_key) : 0.0f;
   each([&](int i, T v) {
     const uint32_t k = sample_key(bits16(v));
+    if (greedy) {  // the ordered 16-bit key in place of l / T + g
+      const unsigned long long key = ((unsigned long long)k << 32) | (0xFFFFFFFFu - (uint32_t)i);
+      if (key > best) best = key;
+      return;
+    }
     bool edge = false;
     if (split >= 0) {
       const int hi = (int)(k >> 8);
@@ -1931,6 +1951,46 @@ __global__ void __launch_bounds__(kSampleThreads, 1) sample_kernel(const T* __re
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { const unsigned long long t = __shfl_xor_sync(0xffffffffu, best, o); best = t > best ? t : best; }
     if (tid == 0) out[row] = (long long)(0xFFFFFFFFu - (uint32_t)(best & 0xFFFFFFFFull));
+  }
+}
+
+// ---- repetition, frequency and presence penalties (hqq_b200_glue_penalize; the definition is in include/hqq_b200.h) ---------------
+// CTA (x, s) takes columns [x * kPenChunk, (x + 1) * kPenChunk) of every row of slot s, one column per thread and pass.  The thread
+// whose column is tok[s] reads counts[s][tok] once, penalises all of the slot's rows with the count plus one and stores that
+// count back; no other thread touches the entry, so the increment needs no atomic and every row sees this step's token.
+constexpr int kPenThreads = 256;
+constexpr int kPenChunk = 1024;  // 126 CTAs over one row of the 128256-entry vocabulary
+
+template <typename T>
+__global__ void __launch_bounds__(kPenThreads) penalize_kernel(const T* __restrict__ logits, int n, long long ld, int rows_per_slot,
+                                                               const float* __restrict__ rep, const float* __restrict__ freq,
+                                                               const float* __restrict__ pres, int* __restrict__ counts,
+                                                               const unsigned char* __restrict__ prompt, const long long* __restrict__ tok,
+                                                               T* __restrict__ out, long long ld_out) {
+  const int slot = blockIdx.y;
+  pdl_launch_dependents();
+  pdl_wait();
+  const float r = __ldg(rep + slot), f = __ldg(freq + slot), p = __ldg(pres + slot);
+  const long long t = tok ? __ldg(tok + slot) : -1;
+  int* cnt = counts + (long long)slot * n;
+  const unsigned char* pr = prompt + (long long)slot * n;
+  const int end = min(n, (int)(blockIdx.x + 1) * kPenChunk);
+  for (int i = blockIdx.x * kPenChunk + threadIdx.x; i < end; i += kPenThreads) {
+    const int c = cnt[i] + (i == t);
+    if (i == t) cnt[i] = c;
+    const bool seen = c > 0 || pr[i];
+    const float fc = __fmul_rn(f, (float)c);
+    for (int j = 0; j < rows_per_slot; ++j) {
+      const long long row = (long long)slot * rows_per_slot + j;
+      T v = logits[row * ld + i];
+      if (seen) {
+        float x = to_f32<T>(v);
+        x = x < 0.0f ? __fmul_rn(x, r) : __fdiv_rn(x, r);
+        if (c > 0) x = __fsub_rn(__fsub_rn(x, fc), p);
+        v = from_f32<T>(x);
+      }
+      out[row * ld_out + i] = v;
+    }
   }
 }
 
@@ -2842,13 +2902,16 @@ extern "C" int hqq_b200_glue_spec_accept(const int64_t* targets, const int64_t* 
                     batch, K, cache_len);
 }
 
-template <typename Keys>
-static int sample_launch(const char* name, const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
-                         Keys keys, int64_t* out, int dtype, void* stream) {
+template <typename Keys, typename Params>
+static int sample_launch(const char* name, const void* logits, int n, int ld, int rows, Params params, uint64_t seed, Keys keys, int64_t* out, int dtype,
+                         void* stream) {
   HQQ_REQUIRE(dtype == HQQ_F16 || dtype == HQQ_BF16, HQQ_E_INVALID, "%s: dtype must be f16/bf16", name);
-  HQQ_REQUIRE(temperature > 0.0f && temperature <= 3.40282347e38f, HQQ_E_INVALID, "%s: temperature must be finite and > 0 (got %g)", name, (double)temperature);
-  HQQ_REQUIRE(top_k >= 0, HQQ_E_INVALID, "%s: top_k must be >= 0 (got %d)", name, top_k);
-  HQQ_REQUIRE(top_p > 0.0f && top_p <= 1.0f, HQQ_E_INVALID, "%s: top_p must lie in (0, 1] (got %g)", name, (double)top_p);
+  if constexpr (!Params::kSlots) {
+    const float temperature = params.temperature, top_p = params.top_p;
+    HQQ_REQUIRE(temperature > 0.0f && temperature <= 3.40282347e38f, HQQ_E_INVALID, "%s: temperature must be finite and > 0 (got %g)", name, (double)temperature);
+    HQQ_REQUIRE(params.top_k >= 0, HQQ_E_INVALID, "%s: top_k must be >= 0 (got %d)", name, params.top_k);
+    HQQ_REQUIRE(top_p > 0.0f && top_p <= 1.0f, HQQ_E_INVALID, "%s: top_p must lie in (0, 1] (got %g)", name, (double)top_p);
+  }
   HQQ_REQUIRE(n > 0 && ld >= n && rows > 0 && rows <= 65535, HQQ_E_INVALID, "%s: needs n > 0, ld >= n and 1 <= rows <= 65535 (n=%d ld=%d rows=%d)", name,
               n, ld, rows);
   HQQ_REQUIRE(aligned(logits, 16) && ld % 8 == 0, HQQ_E_INVALID, "%s: rows must start on 16-byte boundaries (logits 16-byte aligned, ld %% 8 == 0; ld=%d)",
@@ -2856,27 +2919,70 @@ static int sample_launch(const char* name, const void* logits, int n, int ld, in
   cudaStream_t st = (cudaStream_t)stream;
   auto go = [&](auto t) {
     using E = decltype(t);
-    return launch_pdl("sample", sample_kernel<E, Keys>, dim3((unsigned)rows), dim3(kSampleThreads), 0, st, (const E*)logits, n, (long long)ld, temperature,
-                      top_k, top_p, (uint32_t)seed, (uint32_t)(seed >> 32), keys, (long long*)out);
+    return launch_pdl("sample", sample_kernel<E, Keys, Params>, dim3((unsigned)rows), dim3(kSampleThreads), 0, st, (const E*)logits, n, (long long)ld,
+                      params, (uint32_t)seed, (uint32_t)(seed >> 32), keys, (long long*)out);
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+}
+
+static int rows_per_slot_args(const char* name, int rows_per_slot, int rows) {
+  HQQ_REQUIRE(rows_per_slot >= 1 && rows_per_slot <= 8 && rows % rows_per_slot == 0, HQQ_E_INVALID,
+              "%s: needs 1 <= rows_per_slot <= 8 dividing rows (rows_per_slot=%d rows=%d)", name, rows_per_slot, rows);
+  return HQQ_OK;
 }
 
 extern "C" int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
                                     const uint64_t* counter, int64_t* out, int dtype, void* stream) {
   const char* name = "hqq_b200_glue_sample";
   HQQ_REQUIRE(logits && counter && out, HQQ_E_INVALID, "%s: null pointer", name);
-  return sample_launch(name, logits, n, ld, rows, temperature, top_k, top_p, seed, StepKeys{(const unsigned long long*)counter}, out, dtype, stream);
+  return sample_launch(name, logits, n, ld, rows, ScalarParams{temperature, top_k, top_p}, seed, StepKeys{(const unsigned long long*)counter}, out, dtype,
+                       stream);
 }
 
 extern "C" int hqq_b200_glue_sample_pos(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
                                         int rows_per_slot, const int64_t* pos, const int64_t* seq, int64_t* out, int dtype, void* stream) {
   const char* name = "hqq_b200_glue_sample_pos";
   HQQ_REQUIRE(logits && pos && seq && out, HQQ_E_INVALID, "%s: null pointer", name);
-  HQQ_REQUIRE(rows_per_slot >= 1 && rows_per_slot <= 8 && rows % rows_per_slot == 0, HQQ_E_INVALID,
-              "%s: needs 1 <= rows_per_slot <= 8 dividing rows (rows_per_slot=%d rows=%d)", name, rows_per_slot, rows);
-  return sample_launch(name, logits, n, ld, rows, temperature, top_k, top_p, seed, PosKeys{(const long long*)pos, (const long long*)seq, rows_per_slot},
-                       out, dtype, stream);
+  if (int rc = rows_per_slot_args(name, rows_per_slot, rows)) return rc;
+  return sample_launch(name, logits, n, ld, rows, ScalarParams{temperature, top_k, top_p}, seed,
+                       PosKeys{(const long long*)pos, (const long long*)seq, rows_per_slot}, out, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_sample_slots(const void* logits, int n, int ld, int rows, int rows_per_slot, const float* temperature, const int32_t* top_k,
+                                          const float* top_p, uint64_t seed, const uint64_t* counter, const int64_t* pos, const int64_t* seq, int64_t* out,
+                                          int dtype, void* stream) {
+  const char* name = "hqq_b200_glue_sample_slots";
+  HQQ_REQUIRE(logits && temperature && top_k && top_p && out && (pos ? seq != nullptr : counter != nullptr), HQQ_E_INVALID, "%s: null pointer", name);
+  if (int rc = rows_per_slot_args(name, rows_per_slot, rows)) return rc;
+  const SlotParams params{temperature, (const int*)top_k, top_p, rows_per_slot};
+  if (pos)
+    return sample_launch(name, logits, n, ld, rows, params, seed, PosKeys{(const long long*)pos, (const long long*)seq, rows_per_slot}, out, dtype, stream);
+  return sample_launch(name, logits, n, ld, rows, params, seed, StepKeys{(const unsigned long long*)counter}, out, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_penalize(const void* logits, int n, int ld, int rows, int rows_per_slot, const float* repetition, const float* frequency,
+                                      const float* presence, int32_t* counts, const uint8_t* prompt, const int64_t* tok, void* out, int ld_out, int dtype,
+                                      void* stream) {
+  const char* name = "hqq_b200_glue_penalize";
+  HQQ_REQUIRE(logits && repetition && frequency && presence && counts && prompt && out, HQQ_E_INVALID, "%s: null pointer", name);
+  HQQ_REQUIRE(dtype == HQQ_F16 || dtype == HQQ_BF16, HQQ_E_INVALID, "%s: dtype must be f16/bf16", name);
+  HQQ_REQUIRE(n > 0 && ld >= n && ld_out >= n && rows > 0, HQQ_E_INVALID, "%s: needs n > 0, ld >= n, ld_out >= n and rows >= 1 (n=%d ld=%d ld_out=%d rows=%d)",
+              name, n, ld, ld_out, rows);
+  if (int rc = rows_per_slot_args(name, rows_per_slot, rows)) return rc;
+  HQQ_REQUIRE(rows / rows_per_slot <= 65535, HQQ_E_INVALID, "%s: at most 65535 slots (rows=%d rows_per_slot=%d)", name, rows, rows_per_slot);
+  HQQ_REQUIRE(aligned(out, 16) && ld_out % 8 == 0, HQQ_E_INVALID, "%s: output rows must start on 16-byte boundaries (out 16-byte aligned, ld_out %% 8 == 0; "
+              "ld_out=%d)", name, ld_out);
+  const char *a = (const char*)logits, *b = (const char*)out;
+  const long long span_in = ((long long)(rows - 1) * ld + n) * 2, span_out = ((long long)(rows - 1) * ld_out + n) * 2;
+  HQQ_REQUIRE(b >= a + span_in || a >= b + span_out, HQQ_E_INVALID, "%s: out must not overlap logits", name);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((unsigned)cdiv(n, kPenChunk), (unsigned)(rows / rows_per_slot));
+  auto go = [&](auto t) {
+    using E = decltype(t);
+    return launch_pdl("penalize", penalize_kernel<E>, grid, dim3(kPenThreads), 0, st, (const E*)logits, n, (long long)ld, rows_per_slot, repetition, frequency,
+                      presence, (int*)counts, (const unsigned char*)prompt, (const long long*)tok, (E*)out, (long long)ld_out);
+  };
+  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
 }
 
 #ifndef HQQ_EMU

@@ -168,13 +168,17 @@ def philox_uniforms(n: int, rows: int, seed: int, counter, device=None) -> torch
     return ((x >> 9).double() + 0.5) * 2.0 ** -23
 
 
-def sample_tokens(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, seed: int, counter) -> torch.Tensor:
+def sample_tokens(logits: torch.Tensor, temperature, top_k, top_p, seed: int, counter) -> torch.Tensor:
     """hqq_b200_glue_sample restated on framework ops in float64 (the definition is in include/hqq_b200.h): logits [rows, n] in
     fp16 / bf16, row b sampled with Philox counter (., b, counter), counter as philox_uniforms takes it (per-row words 2 and 3
     restate hqq_b200_glue_sample_pos); returns int64 [rows].  temperature and top_p are taken at fp32
     precision, as the kernel receives them.  Top-k compares the 16-bit values as stored.  The reference generator's
     torch.where(logits < pivot, -inf, logits) on fp16(logits / T) can merge neighbouring values by that rounding; here they stay
-    apart, so its keep set can be larger than ours at the pivot."""
+    apart, so its keep set can be larger than ours at the pivot.
+    temperature, top_k and top_p may also be device tensors [rows] of per-row values (hqq_b200_glue_sample_slots): each row is then
+    drawn with its own, by the same operations and without a host read, and a row at temperature 0 takes its argmax."""
+    if torch.is_tensor(temperature):
+        return _sample_tokens_rows(logits, temperature, top_k, top_p, seed, counter)
     T = float(torch.tensor(temperature, dtype=torch.float32))
     P = float(torch.tensor(top_p, dtype=torch.float32))
     rows, n = logits.shape
@@ -191,6 +195,41 @@ def sample_tokens(logits: torch.Tensor, temperature: float, top_k: int, top_p: f
     u = philox_uniforms(n, rows, seed, counter, logits.device)
     key = torch.where(keep, lv / T - torch.log(-torch.log(u)), torch.full_like(lv, -math.inf))
     return torch.argmax(key, dim=-1)
+
+
+def _sample_tokens_rows(logits, temperature, top_k, top_p, seed, counter):
+    """sample_tokens with per-row parameters (device tensors [rows]): the scalar path's operations with the parameters as columns,
+    the top_k-th value taken from a descending sort in place of torch.topk (the same value)."""
+    rows, n = logits.shape
+    lv = logits.double()
+    T = temperature.to(torch.float32).double().view(rows, 1)
+    P = top_p.to(torch.float32).double().view(rows, 1)
+    k = top_k.to(torch.int64).view(rows, 1)
+    greedy = T == 0
+    T = torch.where(greedy, torch.ones_like(T), T)
+    pivot = torch.sort(lv, dim=-1, descending=True).values.gather(1, (k - 1).clamp(0, n - 1))
+    keep = ((k <= 0) | (k >= n)) | (lv >= pivot)
+    w = torch.where(keep, torch.exp((lv - lv.amax(dim=-1, keepdim=True)) / T), torch.zeros_like(lv))
+    vs, order = torch.sort(torch.where(keep, lv, torch.full_like(lv, -math.inf)), dim=-1, descending=True)
+    cum = w.gather(1, order).cumsum(dim=-1)
+    j = (cum < P * cum[:, -1:]).sum(dim=-1, keepdim=True).clamp(max=n - 1)
+    keep = torch.where(P < 1.0, keep & (lv >= vs.gather(1, j)), keep)
+    u = philox_uniforms(n, rows, seed, counter, logits.device)
+    key = torch.where(keep, lv / T - torch.log(-torch.log(u)), torch.full_like(lv, -math.inf))
+    return torch.where(greedy.view(rows), torch.argmax(logits, dim=-1), torch.argmax(key, dim=-1))
+
+
+def apply_penalties(logits, counts, prompt, repetition, frequency, presence) -> torch.Tensor:
+    """hqq_b200_glue_penalize restated on framework ops (one row per slot): logits [rows, n] in fp16 / bf16, counts int32 and prompt
+    uint8 [rows, n], the penalties fp32 [rows].  An element seen (count > 0 or in the prompt) is divided by r (multiplied when
+    negative); one with count c > 0 then loses f * c and p; the result is rounded once to the logits dtype.  Unseen elements keep
+    their bits.  Each fp32 operation is its own kernel, so nothing is contracted: the kernel's bits."""
+    x = logits.float()
+    r, f, p = repetition.view(-1, 1), frequency.view(-1, 1), presence.view(-1, 1)
+    seen = (counts > 0) | (prompt != 0)
+    y = torch.where(x < 0, x * r, x / r)
+    y = torch.where(counts > 0, (y - f * counts.float()) - p, y)
+    return torch.where(seen, y.to(logits.dtype), logits)
 
 
 KV_PAGE = 64  # positions per page of a paged KV cache (csrc/decode_glue.cu kPage)
@@ -399,7 +438,7 @@ class DecodeModel:
                  n_layers: int | None = None, fused=5, tp_mode: str | None = None, batch: int = 1, shard_from_full: bool = False,
                  kv_bits: int = 16, kv_group_size: int | None = None, do_sample: bool = False, temperature: float = 0.6, top_k: int = 5,
                  top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None, spec_k: int | None = None,
-                 sample_keys: str = "step"):
+                 sample_keys: str = "step", slot_sampling: bool = False):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
         # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
         # top-k, top-p, then a Gumbel race on Philox numbers keyed by sample_seed and countered by _sample_ctr -- instead of the argmax.
@@ -420,7 +459,14 @@ class DecodeModel:
         # lets sampling and speculative decoding combine.  "step" (the default): the counter _sample_ctr, + 1 per sampling call.
         if sample_keys not in ("step", "position"):
             raise ValueError(f"sample_keys must be 'step' or 'position' (got {sample_keys!r})")
-        if sample_keys == "position" and not self.do_sample:
+        # slot_sampling: every slot carries its own temperature, top_k, top_p and repetition / frequency / presence penalties in
+        # device arrays that set_sampling() writes, and every step and prefill head runs hqq_b200_glue_penalize, then
+        # hqq_b200_glue_sample_slots, in place of the argmax or hqq_b200_glue_sample (DESIGN §3.6).  Slots start on the constructor's
+        # parameters (do_sample=False: temperature 0, greedy) with neutral penalties.
+        self.slot_sampling = bool(slot_sampling)
+        if self.slot_sampling and spec_k is not None:
+            raise ValueError("slot_sampling cannot be combined with spec_k: the verify rows' penalties would depend on the drafts ahead of them")
+        if sample_keys == "position" and not (self.do_sample or self.slot_sampling):
             raise ValueError("sample_keys='position' needs do_sample=True")
         self.position_keys = sample_keys == "position"
         # kv_bits 8: every layer's K and V cache in HQQ's 8-bit format (kv8_quantize_rows), groups of kv_group_size along the head dim;
@@ -552,6 +598,14 @@ class DecodeModel:
         self._sample_ctr = torch.zeros(1, dtype=torch.long, device=self.device)  # Philox counter: + 1 per sampled token
         # position keys: slot b's sequence number, + 1 when a prefill starts the slot at position 0, copied by fork()
         self.seq = torch.zeros(self.batch, dtype=torch.long, device=self.device) if self.position_keys else None
+        if self.slot_sampling:  # per-slot parameters, and the token tables [batch, vocab] on every rank (see set_sampling)
+            f32 = lambda v: torch.full((self.batch,), float(v), dtype=torch.float32, device=self.device)
+            self.slot_temperature = f32(self.temperature if self.do_sample else 0.0)
+            self.slot_top_k = torch.full((self.batch,), self.top_k, dtype=torch.int32, device=self.device)
+            self.slot_top_p = f32(self.top_p)
+            self.slot_repetition, self.slot_frequency, self.slot_presence = f32(1.0), f32(0.0), f32(0.0)
+            self.counts = torch.zeros(self.batch, shape.vocab, dtype=torch.int32, device=self.device)
+            self.prompt_seen = torch.zeros(self.batch, shape.vocab, dtype=torch.uint8, device=self.device)
         if kv_pages is not None:
             self.page_table = torch.full((self.batch, cache_len // KV_PAGE), kv_pages, dtype=torch.int32, device=self.device)
         if spec_k is not None:  # hist[b][p] = the token fed at position p; the verify step's static I/O
@@ -622,6 +676,55 @@ class DecodeModel:
             self.seq[dst].copy_(self.seq[src])
         if self.spec_k is not None:
             self.hist[dst].copy_(self.hist[src])
+        if self.slot_sampling:  # the continuation carries the source's token tables (its sampling parameters stay its own)
+            self.counts[dst].copy_(self.counts[src])
+            self.prompt_seen[dst].copy_(self.prompt_seen[src])
+
+    def set_sampling(self, b: int, *, temperature=None, top_k=None, top_p=None, repetition_penalty=None, frequency_penalty=None,
+                     presence_penalty=None):
+        """slot_sampling: slot b's sampling parameters from the next step on; arguments left None keep their value.  temperature 0
+        is greedy (the argmax, first index on ties); top_k 0 and top_p 1 are off; repetition_penalty 1 and frequency / presence
+        penalty 0 are neutral.  Penalties (DESIGN §3.6): a token seen in the slot's prompt or output has its logit divided by
+        repetition_penalty (multiplied when negative); one the slot has emitted c times then loses frequency_penalty * c and
+        presence_penalty.  Checked on the host, written in stream order: no sync, and a captured step needs no re-capture."""
+        if not self.slot_sampling:
+            raise ValueError("set_sampling needs slot_sampling=True")
+        if not (isinstance(b, int) and 0 <= b < self.batch):
+            raise ValueError(f"set_sampling: slot must be an int in [0, {self.batch}) (got {b!r})")
+        num = lambda v: isinstance(v, (int, float)) and not isinstance(v, bool)
+        f32 = lambda v: float(torch.tensor(float(v), dtype=torch.float32)) if num(v) else math.nan
+        writes = []
+        if temperature is not None:
+            if not (math.isfinite(f32(temperature)) and f32(temperature) >= 0):
+                raise ValueError(f"temperature must be finite and >= 0 in fp32, 0 for greedy (got {temperature!r})")
+            writes.append((self.slot_temperature, float(temperature)))
+        if top_k is not None:
+            if not (isinstance(top_k, int) and not isinstance(top_k, bool) and 0 <= top_k < 2 ** 31):
+                raise ValueError(f"top_k must be an int >= 0, 0 for off (got {top_k!r})")
+            writes.append((self.slot_top_k, int(top_k)))
+        if top_p is not None:
+            if not (num(top_p) and 0 < f32(top_p) <= 1 and top_p <= 1):
+                raise ValueError(f"top_p must lie in (0, 1], 1 for off (got {top_p!r})")
+            writes.append((self.slot_top_p, float(top_p)))
+        if repetition_penalty is not None:
+            if not (math.isfinite(f32(repetition_penalty)) and f32(repetition_penalty) > 0):
+                raise ValueError(f"repetition_penalty must be finite and > 0 in fp32, 1 for off (got {repetition_penalty!r})")
+            writes.append((self.slot_repetition, float(repetition_penalty)))
+        for name, v, dst in (("frequency_penalty", frequency_penalty, self.slot_frequency), ("presence_penalty", presence_penalty, self.slot_presence)):
+            if v is not None:
+                if not math.isfinite(f32(v)):
+                    raise ValueError(f"{name} must be finite in fp32, 0 for off (got {v!r})")
+                writes.append((dst, float(v)))
+        for dst, v in writes:
+            dst[b].fill_(v)
+
+    def _slot_tables_prefill(self, b: int, tokens: torch.Tensor, start: int):
+        """slot_sampling: a prefill of slot b at `start` -- from position 0 the slot's token tables start empty -- marks its tokens
+        as prompt tokens."""
+        if start == 0:
+            self.counts[b].zero_()
+            self.prompt_seen[b].zero_()
+        self.prompt_seen[b].index_fill_(0, tokens.reshape(-1), 1)
 
     def _paged_only(self, what):
         if self.kv_pages is None:
@@ -737,7 +840,10 @@ class DecodeModel:
             h = h + y
         h = F.rms_norm(h, (s.hidden,), self.final_norm, s.rms_eps)
         logits = torch.matmul(h, self.lm_head.t())
-        if self.do_sample:
+        if self.slot_sampling:
+            self.next_tok.copy_(self._slot_sample_ref(logits, self.pos.expand(B), self.tok))
+            self._sample_ctr.add_(1)
+        elif self.do_sample:
             self.next_tok.copy_(self._sample_ref(logits, self.pos.expand(B)))
             self._sample_ctr.add_(1)
         elif self.tp > 1:  # vocabulary shards: the global maximum, then the lowest global index that attains it (two small all-reduces)
@@ -777,6 +883,34 @@ class DecodeModel:
             logits = g.view(self.tp, -1, self.vocab_shard).transpose(0, 1).reshape(-1, self.shape.vocab)
         ctr = position_counter(pos, self.seq) if self.position_keys else self._sample_ctr
         return sample_tokens(logits, self.temperature, self.top_k, self.top_p, self.sample_seed, ctr)
+
+    def _slot_sample_ref(self, logits, pos, tok):
+        """slot_sampling on framework ops (fused=False), rows [batch, vocab / tp] one per slot: the full-vocabulary rows (gathered
+        under tensor parallelism), then -- when tok is given, a decode step -- counts[b][tok[b]] += 1, apply_penalties with the
+        slots' tables and penalties, and sample_tokens with the slots' parameters; no host read, so the step captures."""
+        if self.tp > 1:
+            g = torch.empty(self.tp * logits.shape[0], logits.shape[1], dtype=logits.dtype, device=logits.device)
+            torch.distributed.all_gather_into_tensor(g, logits.contiguous(), group=self.pg)
+            logits = g.view(self.tp, -1, self.vocab_shard).transpose(0, 1).reshape(-1, self.shape.vocab)
+        V = self.shape.vocab
+        if tok is not None:  # a token outside [0, vocab) counts nothing, as in the kernel
+            ok = (tok >= 0) & (tok < V)
+            self.counts.view(-1).scatter_add_(0, self._slot_idx * V + tok.clamp(0, V - 1), ok.to(torch.int32))
+        pen = apply_penalties(logits, self.counts, self.prompt_seen, self.slot_repetition, self.slot_frequency, self.slot_presence)
+        ctr = position_counter(pos, self.seq) if self.position_keys else self._sample_ctr
+        return sample_tokens(pen, self.slot_temperature, self.slot_top_k, self.slot_top_p, self.sample_seed, ctr)
+
+    def _slot_sample(self, lib, rows, pen, out, code, st, pos=None, tok=None):
+        """slot_sampling in the fused paths: one hqq_b200_glue_penalize launch from the full-vocabulary rows [batch, >= vocab] into
+        pen (16-byte aligned rows), counting tok first when given (a decode step), then one hqq_b200_glue_sample_slots launch over
+        pen: out[b] = slot b's token (pos: the rows' positions under position keys)."""
+        from ._lib import check, ptr
+        n, R = self.shape.vocab, rows.shape[0]
+        check(lib.hqq_b200_glue_penalize(ptr(rows), n, rows.stride(0), R, 1, ptr(self.slot_repetition), ptr(self.slot_frequency),
+                                         ptr(self.slot_presence), ptr(self.counts), ptr(self.prompt_seen), ptr(tok), ptr(pen), pen.stride(0), code, st))
+        check(lib.hqq_b200_glue_sample_slots(ptr(pen), n, pen.stride(0), R, 1, ptr(self.slot_temperature), ptr(self.slot_top_k), ptr(self.slot_top_p),
+                                             self.sample_seed, ptr(self._sample_ctr), ptr(pos), ptr(self.seq) if pos is not None else None, ptr(out),
+                                             code, st))
 
     def _sample_buffers(self, rows):
         """What _sample_rows needs for `rows` sequences: the all-gather target under tensor parallelism, and padded rows where the
@@ -836,6 +970,10 @@ class DecodeModel:
         from ._lib import check, ptr
         b = self._bufs
         torch.matmul(x, self.lm_head.t(), out=b["logits"])
+        if self.slot_sampling:
+            self._slot_sample(lib, self._sample_rows(b["logits"], b), b["pen_rows"], self.next_tok, code, st,
+                              pos=self._step_pos() if self.position_keys else None, tok=self.tok)
+            return
         if self.do_sample:
             self._sample(lib, self._sample_rows(b["logits"], b), self.next_tok, code, st, pos=self._step_pos() if self.position_keys else None)
             return
@@ -910,7 +1048,7 @@ class DecodeModel:
         norm(delta, self.final_norm)
         self._head(lib, b["x"], code, st)
         self.pos.add_(1).remainder_(self.cache_len)
-        if self.do_sample:
+        if self.do_sample or self.slot_sampling:
             self._sample_ctr.add_(1)
 
     def _setup_exchange(self):
@@ -1004,7 +1142,7 @@ class DecodeModel:
             check(lib.hqq_b200_glue_add_rmsnorm(ptr(h_cur), ptr(delta), ptr(self.final_norm), ptr(b["x"]), s.hidden, s.rms_eps, code, st))
         self._head(lib, b["x"], code, st)
         self.pos.add_(1).remainder_(self.cache_len)
-        if self.do_sample:
+        if self.do_sample or self.slot_sampling:
             self._sample_ctr.add_(1)
 
     def prefill(self, tokens: torch.Tensor, start: int = 0, chunk: int = 2048) -> torch.Tensor:
@@ -1100,6 +1238,9 @@ class DecodeModel:
         if chunk < 1:
             raise ValueError("chunk must be >= 1")
         tokens = tokens.to(torch.long)
+        if self.slot_sampling:
+            for b in range(B):
+                self._slot_tables_prefill(b, tokens[b], start)
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         h_last = d_last = None
         if score is not None:
@@ -1166,6 +1307,9 @@ class DecodeModel:
         if self.spec_k is not None:  # the prompt joins the prompt-lookup history
             for b in slots:
                 self.hist[b, starts[b]:starts[b] + toks[b].numel()] = toks[b].to(torch.int32)
+        if self.slot_sampling:
+            for b in slots:
+                self._slot_tables_prefill(b, toks[b], starts[b])
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         last = {}
         if score is not None:  # slot b's rows t0 .. t0 + n - 1 score entries t0 .. (the last position has no target)
@@ -1386,6 +1530,10 @@ class DecodeModel:
             x = F.rms_norm(h + delta, (s.hidden,), self.final_norm, s.rms_eps)
             logits = torch.matmul(x, self.lm_head.t())
             self.last_logits = logits
+            if self.slot_sampling:  # the prompt's tokens are in the tables; nothing is counted here
+                tok = pick(self._slot_sample_ref(full(logits), kp, None))
+                self._sample_ctr.add_(1)
+                return tok
             if self.do_sample:
                 tok = pick(self._sample_ref(full(logits), kp))
                 self._sample_ctr.add_(1)
@@ -1405,6 +1553,13 @@ class DecodeModel:
         x = torch.empty_like(h)
         check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(delta), ptr(self.final_norm), ptr(x), B, s.hidden, s.rms_eps, code, st))
         self.last_logits = torch.matmul(x, self.lm_head.t())
+        if self.slot_sampling:
+            rows = full(self.last_logits)
+            tok = torch.empty(rows.shape[0], dtype=torch.long, device=self.device)
+            pen = torch.empty(rows.shape[0], -(-s.vocab // 8) * 8, dtype=self.dtype, device=self.device)
+            self._slot_sample(lib, self._sample_rows(rows, self._sample_buffers(rows.shape[0])), pen, tok, code, st, pos=kp)
+            self._sample_ctr.add_(1)
+            return pick(tok)
         if self.do_sample:
             rows = full(self.last_logits)
             tok = torch.empty(rows.shape[0], dtype=torch.long, device=self.device)
@@ -1430,10 +1585,12 @@ class DecodeModel:
                       "v": z(s.n_kv_heads // tp * s.head_dim), "a": z(s.n_heads // tp * s.head_dim), "o": z(s.hidden),
                       "gate": z(s.inter // tp), "up": z(s.inter // tp), "act": z(s.inter // tp), "down": z(s.hidden), "logits": z(self.vocab_shard),
                       "key": torch.zeros(1, dtype=torch.long, device=dev)}
-        if self.do_sample:
+        if self.do_sample or self.slot_sampling:
             self._bufs.update(self._sample_buffers(self.batch))
             if self.position_keys and self.pos.numel() != self.batch:
                 self._bufs["sample_pos"] = torch.zeros(self.batch, dtype=torch.long, device=dev)
+        if self.slot_sampling:  # the penalised rows the sampler reads
+            self._bufs["pen_rows"] = torch.zeros(self.batch, -(-s.vocab // 8) * 8, device=dev, dtype=dt)
         if self.attn_kernel != "single":  # partials + tickets, zeroed once: every launch leaves the tickets at zero
             from ._lib import load
             with torch.cuda.device(dev):
@@ -1448,6 +1605,7 @@ class DecodeModel:
         if fused and self.fused == 5 and self.tp_mode == "p2p" and self.tp > 1 and not hasattr(self, "_xbuf"):
             self._setup_exchange()  # needs symmetric (peer-mapped) memory; ask for tp_mode="nccl" explicitly where that is not available
         step = (self.step_fused5 if self.fused == 5 else self.step_fused) if fused else self.step
+        counts = self.counts.clone() if self.slot_sampling else None  # the warm-up steps count their tokens
         st = torch.cuda.Stream(device=self.device)
         st.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(st), torch.no_grad():
@@ -1455,6 +1613,8 @@ class DecodeModel:
                 step()
         torch.cuda.current_stream(self.device).wait_stream(st)
         torch.cuda.synchronize(self.device)
+        if counts is not None:
+            self.counts.copy_(counts)
         self.pos.zero_()
         if self.kv_pages is not None:
             self.pages.pos = [0] * self.batch
@@ -1475,6 +1635,9 @@ class DecodeModel:
             self.page_table.fill_(self.kv_pages)
         if self.spec_k is not None:
             self.hist.zero_()
+        if self.slot_sampling:  # the token tables; the slots' parameters stay as set
+            self.counts.zero_()
+            self.prompt_seen.zero_()
         for blk in self.blocks:
             for name in ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero"):
                 if name in blk:

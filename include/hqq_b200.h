@@ -579,6 +579,31 @@ int hqq_b200_glue_sample(const void* logits, int n, int ld, int rows, float temp
  * slot at position 0, copied by a fork.  pos and seq are read, never written. */
 int hqq_b200_glue_sample_pos(const void* logits, int n, int ld, int rows, float temperature, int top_k, float top_p, uint64_t seed,
                              int rows_per_slot, const int64_t* pos, const int64_t* seq, int64_t* out, int dtype, void* stream);
+/* Per-slot parameters: the same kernel body, with row r (slot b = r / rows_per_slot, rows_per_slot in [1, 8] dividing rows) taking
+ * temperature[b], top_k[b] and top_p[b] from device arrays [rows / rows_per_slot] (read in stream order, so a captured step sees
+ * whatever was last written there).  temperature[b] == 0 makes the row's token its argmax, first index on ties, as torch.argmax
+ * gives it (-0 equals +0); otherwise the row is drawn as above.  The caller keeps every slot's temperature finite and >= 0,
+ * top_k >= 0 and top_p in (0, 1]; they are not checked on the device.  pos == NULL: the keys of hqq_b200_glue_sample (row index
+ * r, *counter; counter non-null); pos != NULL: those of hqq_b200_glue_sample_pos (seq non-null; counter unused).  With every slot
+ * on the same parameters the tokens are those of hqq_b200_glue_sample / _pos. */
+int hqq_b200_glue_sample_slots(const void* logits, int n, int ld, int rows, int rows_per_slot, const float* temperature, const int32_t* top_k,
+                               const float* top_p, uint64_t seed, const uint64_t* counter, const int64_t* pos, const int64_t* seq, int64_t* out,
+                               int dtype, void* stream);
+/* Repetition, frequency and presence penalties ahead of hqq_b200_glue_sample_slots.  Row r of logits [rows, n] (ld elements apart,
+ * any alignment) belongs to slot b = r / rows_per_slot (rows_per_slot in [1, 8] dividing rows, at most 65535 slots) and is
+ * written to out + r * ld_out (16-byte aligned rows: out 16-byte aligned, ld_out % 8 == 0; out must not overlap logits, which
+ * stay untouched).  counts int32 [slots, n] and prompt uint8 [slots, n] are the slot's token tables.  First, when tok is not
+ * NULL and t = tok[b] lies in [0, n), counts[b][t] += 1 (once per slot, whatever rows_per_slot): the step that consumes a token
+ * counts it before its own logits are penalised.  Then for every element, with c = counts[b][i], seen = c > 0 || prompt[b][i],
+ * x = fp32(l), r = repetition[b], f = frequency[b], p = presence[b]:
+ *   if seen:  x = x < 0 ? x * r : x / r
+ *   if c > 0: x = (x - f * c) - p
+ * and the output is x rounded once to the logits dtype; an element that is not seen is copied bit for bit.  Every operation is
+ * round-to-nearest fp32 without contraction (f * c with c converted to fp32), so an fp32 restatement matches the bits; r = 1,
+ * f = p = 0 reproduce every input bit pattern but NaN payloads. */
+int hqq_b200_glue_penalize(const void* logits, int n, int ld, int rows, int rows_per_slot, const float* repetition, const float* frequency,
+                           const float* presence, int32_t* counts, const uint8_t* prompt, const int64_t* tok, void* out, int ld_out, int dtype,
+                           void* stream);
 
 /* Number of kernels launched by this library on the calling thread since the last reset
  * (used by bench.py for its gpu_launches claim).                                        */
