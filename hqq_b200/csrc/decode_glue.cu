@@ -645,6 +645,18 @@ struct KvF16 {
       v[pr * kHd + tid] = kf[kHd + tid];
     }
   }
+  // The append's store (rope_append_rows_kernel): lane l's elements 4 l .. 4 l + 3 of a rotated k row (isv 0) or a v row to cache row
+  // crow.  Returns them as the cache holds them, packed as two T2.
+  __device__ uint2 put(int isv, long long crow, const T (&x)[4]) const {
+    const int lane = (int)threadIdx.x & 31;
+    T* dst = (isv ? v : k) + crow * kHd + 4 * lane;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) dst[j] = x[j];
+    uint2 y;
+    y.x = bits16(x[0]) | (bits16(x[1]) << 16);
+    y.y = bits16(x[2]) | (bits16(x[3]) << 16);
+    return y;
+  }
   __device__ void scores(float (&s)[4], const char* st, const uint32_t (&qb)[8][2], int lane) const {
     const int kr = (lane & 7) + ((lane >> 3) & 1) * 8, kc = lane >> 4;  // ldmatrix row / chunk, K (a0..a3: rows +8, then k +8)
 #pragma unroll
@@ -760,6 +772,22 @@ struct KvHqq {
       kv_quant_row<T, BITS>(x, gs, lq, ls, lz, sc, ze);
     }
     __syncthreads();
+  }
+  // The append's store, as KvF16::put: the row quantised by kv_quant_row into cache row crow (the levels and meta fresh writes for
+  // the same row); returns the lane's elements as the cache holds them, T(T(q - z) * s) (kv8_deq2).  Every lane must call it.
+  __device__ uint2 put(int isv, long long crow, const T (&x)[4]) const {
+    float f[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) f[j] = to_f32<T>(x[j]);
+    T sc, ze;
+    const uint32_t lv = kv_quant_row<T, BITS>(f, gs, (isv ? v : k) + crow * kRowBytes, (isv ? v_s : k_s) + crow * ng, (isv ? v_z : k_z) + crow * ng, sc, ze);
+    typename Pair<T>::type s2, z2;
+    s2.x = s2.y = sc;
+    z2.x = z2.y = ze;
+    uint2 y;
+    y.x = kv8_deq2<T, 0>(lv, z2, s2);
+    y.y = kv8_deq2<T, 1>(lv, z2, s2);
+    return y;
   }
   __device__ void scores(float (&s)[4], const char* st, const uint32_t (&qb)[8][2], int lane) const {
     const int g = lane >> 2, qd = lane & 3;
@@ -1300,109 +1328,82 @@ constexpr int kPreTileBytes = kPreTile * kHd * 2;         // one K or V tile, 16
 constexpr int kPreStageBytes = 2 * kPreTileBytes;
 constexpr int kPreSmemBytes = kPreStages * kPreStageBytes;  // 96 KB
 
-// Variable-length prefill (VARLEN instantiations of the three prefill kernels): slot b contributes n_tok[b] >= 0 rows at positions
-// pos0[b] .. pos0[b] + n_tok[b] - 1, packed in slot order from token row row0[b] = sum of n_tok[b'] for b' < b (equal lengths give
-// the b T + t layout).  The grids are sized by the longest slot; CTAs past their slot's rows exit, so a slot with no rows is neither
-// read nor written.  The arrays travel by value in the parameter block (3 KB), so a launch needs no upload and no workspace.
+// Variable-length prefill (VARLEN instantiations of the prefill attention, the VarlenRows layout of the append and the staging refill):
+// slot b contributes n_tok[b] >= 0 rows at positions pos0[b] .. pos0[b] + n_tok[b] - 1, packed in slot order from token row row0[b] =
+// sum of n_tok[b'] for b' < b (equal lengths give the b T + t layout).  The grids are sized by the longest slot; CTAs past their slot's
+// rows exit, so a slot with no rows is neither read nor written.  The arrays travel by value in the parameter block (3 KB), so a launch
+// needs no upload and no workspace.
+//
+// The row layouts of rope_append_rows_kernel: place(t, b, L, p, row) gives CTA (t, b) = (blockIdx.x, blockIdx.y) its position p and
+// token row, or returns false when the CTA has nothing to do; kStages says whether the layout writes staging rows.
 constexpr int kVarlenMaxBatch = 256;
 struct VarlenRows {
   int pos0[kVarlenMaxBatch];
   int n_tok[kVarlenMaxBatch];
   int row0[kVarlenMaxBatch];
+  static constexpr bool kStages = true;
+  __device__ bool place(int t, int b, int, int& p, long long& row) const {
+    if (t >= n_tok[b]) return false;  // past this slot's rows
+    p = pos0[b] + t;
+    row = (long long)row0[b] + t;
+    return true;
+  }
 };
 struct NoVarlen {};  // the fixed-length instantiations: their uniform pos0 / T are the scalar arguments
 template <bool VARLEN> using VarlenArg = typename std::conditional<VARLEN, VarlenRows, NoVarlen>::type;
-// Device positions (DEVPOS instantiations, the speculative verify step): slot b's T rows b T + t go to positions pos[b] + t, and only
-// the n[b] = min(T, L - pos[b]) rows that fit in the cache are rotated and written.  pos is read before griddepcontrol.wait, so it
-// must have been written by an earlier, completed launch (the previous step's accept kernel).
-struct DevPos { const long long* pos; };
-template <bool VARLEN, bool DEVPOS> using RowsArg = typename std::conditional<DEVPOS, DevPos, VarlenArg<VARLEN>>::type;
+// The fixed-length append: T rows a slot at the uniform positions pos0 .. pos0 + T - 1, row b T + t.
+struct FixedRows {
+  int pos0, T;
+  static constexpr bool kStages = true;
+  __device__ bool place(int t, int b, int, int& p, long long& row) const {
+    p = pos0 + t;
+    row = (long long)b * T + t;
+    return true;
+  }
+};
+// Device positions (the speculative verify step): slot b's T rows b T + t go to positions pos[b] + t, and only the
+// n[b] = min(T, L - pos[b]) rows that fit in the cache are rotated and written.  pos is read before griddepcontrol.wait, so it must
+// have been written by an earlier, completed launch (the previous step's accept kernel).  No staging rows: the verify attention
+// dequantises the cache itself.
+struct DevPos {
+  const long long* pos;
+  int T;
+  static constexpr bool kStages = false;
+  __device__ bool place(int t, int b, int L, int& p, long long& row) const {
+    const int p0 = (int)pos[b];
+    if (t >= L - p0) return false;  // past the end of the cache: neither written nor rotated
+    p = p0 + t;
+    row = (long long)b * T + t;
+    return true;
+  }
+};
 
-// grid = (T, batch), block = 256.  q / q_out [batch T, n_q 128], k / v [batch T, n_kv 128] (row b T + t), caches [batch, n_kv, L, 128].
-// VARLEN: grid = (max T, batch), rows as VarlenRows lays them out.  PAGED (VARLEN or DEVPOS): page pools, the CTA's position found with
-// one table read.  DEVPOS: grid = (T, batch), positions from the device (see DevPos).
-template <typename T, bool VARLEN = false, bool PAGED = false, bool DEVPOS = false>
+// The prefill and verify append of every cache format and row layout.  Each k and v row goes to the cache through the format's put:
+// KvF16 copies it, KvHqq quantises it as the split decode kernel quantises row pos (the same levels and meta bit for bit).  A quantised
+// format under a staging layout also writes the row as the cache holds it to the staging pair k_st / v_st [batch, n_kv, L, 128] T at
+// the same row, which the prefill attention reads.
+// grid = (T | max T, batch), block = 256: threads take the q elements in turn, then warp w the rows w, w + 8, ... of the 2 n_kv rows
+// of a position (k and v of each kv head), four elements per lane.  q / q_out [rows, n_q 128], k / v [rows, n_kv 128], caches
+// [batch, n_kv, L, .] in the format's layout.  PAGED: page pools (the staging pair stays contiguous), the CTA's position found with one
+// table read.
+template <typename T, typename Cache, typename Rows, bool PAGED>
 __global__ void __launch_bounds__(256) rope_append_rows_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
-                                                               const T* __restrict__ cos_t, const T* __restrict__ sin_t, T* __restrict__ k_cache,
-                                                               T* __restrict__ v_cache, T* __restrict__ q_out, int pos0, int n_tok, int n_q,
-                                                               int n_kv, int L, const RowsArg<VARLEN, DEVPOS> vl, const PageArg<PAGED> pg) {
-  static_assert(VARLEN || DEVPOS || !PAGED, "a paged cache needs per-slot positions");
-  static_assert(!(VARLEN && DEVPOS), "one row layout");
-  const int t = (int)blockIdx.x, b = (int)blockIdx.y;
-  long long row = (long long)b * n_tok + t;
-  if constexpr (VARLEN) {
-    if (t >= vl.n_tok[b]) return;  // past this slot's rows
-    pos0 = vl.pos0[b];
-    row = (long long)vl.row0[b] + t;
-  }
-  if constexpr (DEVPOS) {
-    pos0 = (int)vl.pos[b];
-    if (t >= L - pos0) return;  // past the end of the cache: neither written nor rotated
-  }
-  const int p = pos0 + t;
-  {
-    q += row * n_q * kHd; q_out += row * n_q * kHd;
-    k += row * n_kv * kHd; v += row * n_kv * kHd;
-    if constexpr (!PAGED) { k_cache += (long long)b * n_kv * L * kHd; v_cache += (long long)b * n_kv * L * kHd; }
-  }
-  long long c0 = 0;  // PAGED: pool row of position p of kv head 0
-  if constexpr (PAGED) c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
-  pdl_launch_dependents();
-  pdl_wait();
-  for (int i = (int)threadIdx.x; i < (n_q + 2 * n_kv) * kHd; i += (int)blockDim.x) {
-    const int h = i >> 7, d = i & (kHd - 1);
-    if (h < n_q + n_kv) {
-      const T r = rope_rounded<T>(h < n_q ? q + h * kHd : k + (h - n_q) * kHd, d, cos_t + (long long)p * kHd, sin_t + (long long)p * kHd);
-      if (h < n_q) q_out[h * kHd + d] = r;
-      else if constexpr (PAGED) k_cache[(c0 + (long long)(h - n_q) * kPage) * kHd + d] = r;
-      else k_cache[((long long)(h - n_q) * L + p) * kHd + d] = r;
-    } else {
-      const int kvh = h - n_q - n_kv;
-      if constexpr (PAGED) v_cache[(c0 + (long long)kvh * kPage) * kHd + d] = v[kvh * kHd + d];
-      else v_cache[((long long)kvh * L + p) * kHd + d] = v[kvh * kHd + d];
-    }
-  }
-}
-
-// Prefill into an 8-bit cache: rope_append_rows_kernel's RoPE, then every k and v row quantised by kv_quant_row, as the split decode
-// kernel quantises row pos (the same levels and meta bit for bit), and its dequantisation written to the staging caches at the same row.
-// grid = (T, batch), block = 256: warp w takes rows w, w + 8, ... of the 2 n_kv rows of a position (k and v of each kv head).
-// Levels [batch, n_kv, L, 128] uint8, meta [batch, n_kv, L, 128 / gs] T, staging [batch, n_kv, L, 128] T.  VARLEN as
-// rope_append_rows_kernel.  PAGED as there: levels and meta in the page pools, the staging pair stays [batch, n_kv, L, 128].
-// DEVPOS as rope_append_rows_kernel (positions from the device, rows past the cache end skipped); it writes no staging rows (k_st /
-// v_st unused): the verify attention dequantises the cache itself.  BITS 4: the 4-bit cache (the split decode kernel's
-// quantisation and packing, levels [.., 64]).
-template <typename T, bool VARLEN = false, bool PAGED = false, bool DEVPOS = false, int BITS = 8>
-__global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v,
-                                                                   const T* __restrict__ cos_t, const T* __restrict__ sin_t, uint8_t* __restrict__ k_q,
-                                                                   T* __restrict__ k_s, T* __restrict__ k_z, uint8_t* __restrict__ v_q,
-                                                                   T* __restrict__ v_s, T* __restrict__ v_z, T* __restrict__ k_st, T* __restrict__ v_st,
-                                                                   T* __restrict__ q_out, int pos0, int n_tok, int n_q, int n_kv, int L, int gs,
-                                                                   const RowsArg<VARLEN, DEVPOS> vl, const PageArg<PAGED> pg) {
-  static_assert(VARLEN || DEVPOS || !PAGED, "a paged cache needs per-slot positions");
-  static_assert(!(VARLEN && DEVPOS), "one row layout");
-  constexpr int LB = kHd * BITS / 8;  // level bytes a row
-  const int t = (int)blockIdx.x, b = (int)blockIdx.y, ng = kHd / gs;
-  long long row = (long long)b * n_tok + t;
-  if constexpr (VARLEN) {
-    if (t >= vl.n_tok[b]) return;  // past this slot's rows
-    pos0 = vl.pos0[b];
-    row = (long long)vl.row0[b] + t;
-  }
-  if constexpr (DEVPOS) {
-    pos0 = (int)vl.pos[b];
-    if (t >= L - pos0) return;  // past the end of the cache: neither written nor rotated
-  }
-  const int p = pos0 + t;
+                                                               const T* __restrict__ cos_t, const T* __restrict__ sin_t, const Cache cache,
+                                                               T* __restrict__ k_st, T* __restrict__ v_st, T* __restrict__ q_out, int n_q, int n_kv,
+                                                               int L, const Rows rows, const PageArg<PAGED> pg) {
+  static_assert(!PAGED || !std::is_same<Rows, FixedRows>::value, "a paged cache needs per-slot positions");
+  constexpr bool kStage = Rows::kStages && !std::is_same<Cache, KvF16<T>>::value;
+  const int b = (int)blockIdx.y;
+  int p;
+  long long row;
+  if (!rows.place((int)blockIdx.x, b, L, p, row)) return;
+  Cache c = cache;
   {
     const long long kv = (long long)b * n_kv;
     q += row * n_q * kHd; q_out += row * n_q * kHd;
     k += row * n_kv * kHd; v += row * n_kv * kHd;
-    if constexpr (!PAGED) {
-      k_q += kv * L * LB; v_q += kv * L * LB;
-      k_s += kv * L * ng; k_z += kv * L * ng; v_s += kv * L * ng; v_z += kv * L * ng;
-    }
-    if constexpr (!DEVPOS) { k_st += kv * L * kHd; v_st += kv * L * kHd; }
+    if constexpr (!PAGED) c.advance(kv, L);
+    if constexpr (kStage) { k_st += kv * L * kHd; v_st += kv * L * kHd; }
   }
   long long c0 = 0;  // PAGED: pool row of position p of kv head 0
   if constexpr (PAGED) c0 = page_row(pg.table + (long long)b * (L / kPage), n_kv, 0, p);
@@ -1410,28 +1411,19 @@ __global__ void __launch_bounds__(256) rope_append_rows_kv8_kernel(const T* __re
   pdl_wait();
   const T* cs = cos_t + (long long)p * kHd;
   const T* sn = sin_t + (long long)p * kHd;
-  for (int i = (int)threadIdx.x; i < n_q * kHd; i += (int)blockDim.x) {  // rope(q) as rope_append_rows_kernel
+  for (int i = (int)threadIdx.x; i < n_q * kHd; i += (int)blockDim.x) {
     const int h = i >> 7, d = i & (kHd - 1);
     q_out[h * kHd + d] = rope_rounded<T>(q + h * kHd, d, cs, sn);
   }
   const int warp = (int)threadIdx.x >> 5, lane = (int)threadIdx.x & 31;
   for (int r = warp; r < 2 * n_kv; r += (int)blockDim.x >> 5) {
     const int kvh = r >> 1, isv = r & 1;
-    float x[4];
+    T x[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) x[j] = to_f32<T>(isv ? v[kvh * kHd + 4 * lane + j] : rope_rounded<T>(k + kvh * kHd, 4 * lane + j, cs, sn));
-    const long long row = (long long)kvh * L + p;
-    long long crow = row;
-    if constexpr (PAGED) crow = c0 + (long long)kvh * kPage;
-    T sc, ze;
-    const uint32_t lv = kv_quant_row<T, BITS>(x, gs, (isv ? v_q : k_q) + crow * LB, (isv ? v_s : k_s) + crow * ng, (isv ? v_z : k_z) + crow * ng, sc, ze);
-    typename Pair<T>::type s2, z2;
-    s2.x = s2.y = sc;
-    z2.x = z2.y = ze;
-    uint2 y;
-    y.x = kv8_deq2<T, 0>(lv, z2, s2);
-    y.y = kv8_deq2<T, 1>(lv, z2, s2);
-    if constexpr (!DEVPOS) *reinterpret_cast<uint2*>((isv ? v_st : k_st) + row * kHd + 4 * lane) = y;
+    for (int j = 0; j < 4; ++j) x[j] = isv ? v[kvh * kHd + 4 * lane + j] : rope_rounded<T>(k + kvh * kHd, 4 * lane + j, cs, sn);
+    const long long crow = PAGED ? c0 + (long long)kvh * kPage : (long long)kvh * L + p;
+    const uint2 y = c.put(isv, crow, x);
+    if constexpr (kStage) *reinterpret_cast<uint2*>((isv ? v_st : k_st) + ((long long)kvh * L + p) * kHd + 4 * lane) = y;
   }
 }
 
@@ -2370,105 +2362,217 @@ extern "C" int hqq_b200_glue_rope_attn_decode_split_kv4_paged(const void* q, con
                                 n_kv_heads, cache_len, head_dim, batch, dtype, stream);
 }
 
-// The fixed-length (pos0_v == nullptr: uniform pos0, T) and variable-length (host pos0_v / n_tok_v) appends into a quantised cache
-static int rope_append_rows_kvq(const char* name, int bits, const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage, void* v_stage, void* q_out,
-                                int pos0, int T, const int* pos0_v, const int* n_tok_v, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
-                                int group_size, int batch, int dtype, void* stream) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
+// The checks of the device-position entry points: the prefill shape checks, 1 <= T <= 8 rows per slot, T G <= 64 columns.
+static int spec_args(const char* name, int T, int n_q, int n_kv, int L, int hd, int batch, int dtype) {
+  if (int rc = prefill_args(name, 0, 1, n_q, n_kv, L, hd, batch, dtype)) return rc;
+  HQQ_REQUIRE(T >= 1 && T <= kVerMaxT && T <= L, HQQ_E_INVALID, "%s: needs 1 <= T <= %d and T <= cache_len (T=%d)", name, kVerMaxT, T);
+  HQQ_REQUIRE(T * (n_q / n_kv) <= kVerMaxCols, HQQ_E_UNSUPPORTED, "%s: T * n_q_heads / n_kv_heads must be <= %d", name, kVerMaxCols);
+  return HQQ_OK;
+}
+
+// The row layout of an append: uniform pos0 / T (FixedRows), host pos0_v / n_tok_v of `batch` slots (VarlenRows), or device positions
+// pos with T rows a slot (DevPos)
+enum AppendRows { kAppendFixed, kAppendVarlen, kAppendDevPos };
+
+// Every append entry point (rope_append_rows_kernel).  bits 16: k_cache / v_cache are the 16-bit caches (meta, gs unused); bits 8 or 4:
+// they are the HQQ level caches, meta = {k_scale, k_zero, v_scale, v_zero} and gs their group size.  paged: page pools through table.
+// k_stage / v_stage: the staging pair of a quantised cache under the host-position layouts (unused otherwise).
+static int rope_append_rows(const char* name, int bits, AppendRows lay, bool paged, const void* q, const void* k, const void* v,
+                            const void* cos_table, const void* sin_table, void* k_cache, void* v_cache, void* const* meta, int gs,
+                            const int* table, void* k_stage, void* v_stage, void* q_out, int pos0, int T, const int* pos0_v,
+                            const int* n_tok_v, const int64_t* pos, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch,
+                            int n_pages, int dtype, void* stream) {
+  const bool quant = bits != 16, dev = lay == kAppendDevPos;
+  if (paged && dev) {  // the device-position forms check the table before the pointers
+    if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  }
+  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && (!quant || (meta[0] && meta[1] && meta[2] && meta[3])) &&
+                  (!quant || dev || (k_stage && v_stage)) && q_out && (!dev || pos),
               HQQ_E_INVALID, "%s: null pointer", name);
+  if (paged && !dev) {
+    if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
+  }
   VarlenRows vl;
   int max_t = 0;
-  if (pos0_v) {
+  if (lay == kAppendVarlen) {
     if (int rc = varlen_args(name, pos0_v, n_tok_v, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
+  } else if (dev) {
+    if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
   } else if (int rc = prefill_args(name, pos0, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) {
     return rc;
   }
-  if (int rc = kv_group_args(name, bits, group_size)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag, auto kernel, auto rows, dim3 grid) {
-    using E = decltype(tag);
-    return launch_pdl(name, kernel, grid, dim3(256), 0, st, (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table,
-                      (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q, (E*)v_scale, (E*)v_zero, (E*)k_stage, (E*)v_stage, (E*)q_out, pos0_v ? 0 : pos0,
-                      pos0_v ? 0 : T, n_q_heads, n_kv_heads, cache_len, group_size, rows, NoPages());
-  };
-  const dim3 gf((unsigned)T, (unsigned)batch), gv((unsigned)max_t, (unsigned)batch);
-  if (bits == 8) {
-    if (pos0_v) return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true>, vl, gv)
-                                        : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true>, vl, gv);
-    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half>, NoVarlen(), gf)
-                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16>, NoVarlen(), gf);
+  if (quant) {
+    if (int rc = kv_group_args(name, bits, gs)) return rc;
   }
-  if (pos0_v) return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true, false, false, 4>, vl, gv)
-                                      : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true, false, false, 4>, vl, gv);
-  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, false, false, 4>, NoVarlen(), gf)
-                          : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, false, false, 4>, NoVarlen(), gf);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((unsigned)(lay == kAppendVarlen ? max_t : T), (unsigned)batch);
+  auto launch = [&](auto tag, auto cache, auto rows, auto pg) {
+    using E = decltype(tag);
+    constexpr bool PG = std::is_same<decltype(pg), PageTable>::value;
+    return launch_pdl(name, rope_append_rows_kernel<E, decltype(cache), decltype(rows), PG>, grid, dim3(256), 0, st, (const E*)q, (const E*)k,
+                      (const E*)v, (const E*)cos_table, (const E*)sin_table, cache, (E*)k_stage, (E*)v_stage, (E*)q_out, n_q_heads, n_kv_heads,
+                      cache_len, rows, pg);
+  };
+  auto by_rows = [&](auto tag, auto cache) {
+    const PageTable pt{table};
+    if (lay == kAppendFixed) return launch(tag, cache, FixedRows{pos0, T}, NoPages());
+    if (lay == kAppendVarlen) return paged ? launch(tag, cache, vl, pt) : launch(tag, cache, vl, NoPages());
+    const DevPos dp{(const long long*)pos, T};
+    return paged ? launch(tag, cache, dp, pt) : launch(tag, cache, dp, NoPages());
+  };
+  auto by_format = [&](auto tag) {
+    using E = decltype(tag);
+    if (bits == 16) return by_rows(tag, KvF16<E>{(E*)k_cache, (E*)v_cache});
+    if (bits == 8) return by_rows(tag, KvHqq<E, 8>{(uint8_t*)k_cache, (E*)meta[0], (E*)meta[1], (uint8_t*)v_cache, (E*)meta[2], (E*)meta[3], gs, kHd / gs});
+    return by_rows(tag, KvHqq<E, 4>{(uint8_t*)k_cache, (E*)meta[0], (E*)meta[1], (uint8_t*)v_cache, (E*)meta[2], (E*)meta[3], gs, kHd / gs});
+  };
+  return dtype == HQQ_F16 ? by_format(__half()) : by_format(__nv_bfloat16());
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache,
+                                              void* v_cache, void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                              int batch, int dtype, void* stream) {
+  return rope_append_rows("hqq_b200_glue_rope_append_rows", 16, kAppendFixed, false, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, 0,
+                          nullptr, nullptr, nullptr, q_out, pos0, T, nullptr, nullptr, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch, 0,
+                          dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                     void* k_cache, void* v_cache, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                                     int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_varlen", 16, kAppendVarlen, false, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr,
+                          0, nullptr, nullptr, nullptr, q_out, 0, 0, pos0, n_tok, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch, 0, dtype,
+                          stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                    void* k_pool, void* v_pool, const int* table, void* q_out, const int* pos0, const int* n_tok,
+                                                    int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
+                                                    void* stream) {
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_paged", 16, kAppendVarlen, true, q, k, v, cos_table, sin_table, k_pool, v_pool, nullptr, 0,
+                          table, nullptr, nullptr, q_out, 0, 0, pos0, n_tok, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch, n_pages, dtype,
+                          stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                     void* k_cache, void* v_cache, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                                     int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_devpos", 16, kAppendDevPos, false, q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr,
+                          0, nullptr, nullptr, nullptr, q_out, 0, T, nullptr, nullptr, pos, n_q_heads, n_kv_heads, cache_len, head_dim, batch, 0, dtype,
+                          stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                           void* k_pool, void* v_pool, const int* table, void* q_out, const int64_t* pos, int T,
+                                                           int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
+                                                           void* stream) {
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_devpos_paged", 16, kAppendDevPos, true, q, k, v, cos_table, sin_table, k_pool, v_pool,
+                          nullptr, 0, table, nullptr, nullptr, q_out, 0, T, nullptr, nullptr, pos, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          n_pages, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows_kv8(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_q,
                                                   void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage, void* v_stage,
                                                   void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                                   int group_size, int batch, int dtype, void* stream) {
-  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv8", 8, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, k_stage,
-                              v_stage, q_out, pos0, T, nullptr, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv8", 8, kAppendFixed, false, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size,
+                          nullptr, k_stage, v_stage, q_out, pos0, T, nullptr, nullptr, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch, 0,
+                          dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows_kv8_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                          void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage,
                                                          void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads,
                                                          int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
-  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv8_varlen", 8, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero,
-                              k_stage, v_stage, q_out, 0, 0, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv8_varlen", 8, kAppendVarlen, false, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, nullptr, k_stage, v_stage, q_out, 0, 0, pos0, n_tok, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          0, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
+                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
+                                                        void* stream) {
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv8_paged", 8, kAppendVarlen, true, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, table, k_stage, v_stage, q_out, 0, 0, pos0, n_tok, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          n_pages, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* q_out,
+                                                         const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                         int group_size, int batch, int dtype, void* stream) {
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv8_devpos", 8, kAppendDevPos, false, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, nullptr, nullptr, nullptr, q_out, 0, T, nullptr, nullptr, pos, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          0, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv8_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                               const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
+                                                               void* v_zero, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                                               int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages,
+                                                               int dtype, void* stream) {
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv8_devpos_paged", 8, kAppendDevPos, true, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, table, nullptr, nullptr, q_out, 0, T, nullptr, nullptr, pos, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          n_pages, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows_kv4(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_q,
                                                   void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage, void* v_stage,
                                                   void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
                                                   int group_size, int batch, int dtype, void* stream) {
-  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv4", 4, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, k_stage,
-                              v_stage, q_out, pos0, T, nullptr, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv4", 4, kAppendFixed, false, q, k, v, cos_table, sin_table, k_q, v_q, meta, group_size,
+                          nullptr, k_stage, v_stage, q_out, pos0, T, nullptr, nullptr, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch, 0,
+                          dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_rope_append_rows_kv4_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
                                                          void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* k_stage,
                                                          void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads, int n_kv_heads,
                                                          int cache_len, int head_dim, int group_size, int batch, int dtype, void* stream) {
-  return rope_append_rows_kvq("hqq_b200_glue_rope_append_rows_kv4_varlen", 4, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero,
-                              k_stage, v_stage, q_out, 0, 0, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv4_varlen", 4, kAppendVarlen, false, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, nullptr, k_stage, v_stage, q_out, 0, 0, pos0, n_tok, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          0, dtype, stream);
 }
 
-extern "C" int hqq_b200_glue_rope_append_rows(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table, void* k_cache,
-                                              void* v_cache, void* q_out, int pos0, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
-                                              int batch, int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows";
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && q_out, HQQ_E_INVALID, "%s: null pointer", name);
-  if (int rc = prefill_args(name, pos0, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag) {
-    using E = decltype(tag);
-    return launch_pdl("rope_append_rows", rope_append_rows_kernel<E>, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k,
-                      (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, pos0, T, n_q_heads, n_kv_heads,
-                      cache_len, NoVarlen(), NoPages());
-  };
-  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+extern "C" int hqq_b200_glue_rope_append_rows_kv4_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
+                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
+                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
+                                                        void* stream) {
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv4_paged", 4, kAppendVarlen, true, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, table, k_stage, v_stage, q_out, 0, 0, pos0, n_tok, nullptr, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          n_pages, dtype, stream);
 }
 
-extern "C" int hqq_b200_glue_rope_append_rows_varlen(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                     void* k_cache, void* v_cache, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
-                                                     int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_varlen";
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && q_out, HQQ_E_INVALID, "%s: null pointer", name);
-  VarlenRows vl;
-  int max_t = 0;
-  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag) {
-    using E = decltype(tag);
-    return launch_pdl("rope_append_rows_varlen", rope_append_rows_kernel<E, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
-                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, 0, 0,
-                      n_q_heads, n_kv_heads, cache_len, vl, NoPages());
-  };
-  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
+extern "C" int hqq_b200_glue_rope_append_rows_kv4_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
+                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* q_out,
+                                                         const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
+                                                         int group_size, int batch, int dtype, void* stream) {
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv4_devpos", 4, kAppendDevPos, false, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, nullptr, nullptr, nullptr, q_out, 0, T, nullptr, nullptr, pos, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          0, dtype, stream);
+}
+
+extern "C" int hqq_b200_glue_rope_append_rows_kv4_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
+                                                               const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
+                                                               void* v_zero, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
+                                                               int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages,
+                                                               int dtype, void* stream) {
+  void* const meta[4] = {k_scale, k_zero, v_scale, v_zero};
+  return rope_append_rows("hqq_b200_glue_rope_append_rows_kv4_devpos_paged", 4, kAppendDevPos, true, q, k, v, cos_table, sin_table, k_q, v_q, meta,
+                          group_size, table, nullptr, nullptr, q_out, 0, T, nullptr, nullptr, pos, n_q_heads, n_kv_heads, cache_len, head_dim, batch,
+                          n_pages, dtype, stream);
 }
 
 extern "C" int hqq_b200_glue_attn_prefill(const void* q_rot, const void* k_cache, const void* v_cache, void* out, int pos0, int T, int n_q_heads,
@@ -2506,71 +2610,6 @@ extern "C" int hqq_b200_glue_attn_prefill_varlen(const void* q_rot, const void* 
                       (const E*)k_cache, (const E*)v_cache, (E*)out, 0, 0, n_q_heads, n_kv_heads, cache_len, scale_log2, vl, NoPages());
   };
   return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                    void* k_pool, void* v_pool, const int* table, void* q_out, const int* pos0, const int* n_tok,
-                                                    int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
-                                                    void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_paged";
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_pool && v_pool && q_out, HQQ_E_INVALID, "%s: null pointer", name);
-  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  VarlenRows vl;
-  int max_t = 0;
-  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag) {
-    using E = decltype(tag);
-    return launch_pdl("rope_append_rows_paged", rope_append_rows_kernel<E, true, true>, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st,
-                      (const E*)q, (const E*)k, (const E*)v, (const E*)cos_table, (const E*)sin_table, (E*)k_pool, (E*)v_pool, (E*)q_out, 0, 0,
-                      n_q_heads, n_kv_heads, cache_len, vl, PageTable{table});
-  };
-  return dtype == HQQ_F16 ? go(__half()) : go(__nv_bfloat16());
-}
-
-static int rope_append_rows_kvq_paged(const char* name, int bits, const void* q, const void* k, const void* v, const void* cos_table,
-                                      const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero,
-                                      const int* table, void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
-                                      int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype, void* stream) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && k_stage && v_stage && q_out,
-              HQQ_E_INVALID, "%s: null pointer", name);
-  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  VarlenRows vl;
-  int max_t = 0;
-  if (int rc = varlen_args(name, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, vl, max_t)) return rc;
-  if (int rc = kv_group_args(name, bits, group_size)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  auto go = [&](auto tag, auto kernel) {
-    using E = decltype(tag);
-    return launch_pdl(name, kernel, dim3((unsigned)max_t, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k, (const E*)v,
-                      (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q, (E*)v_scale, (E*)v_zero,
-                      (E*)k_stage, (E*)v_stage, (E*)q_out, 0, 0, n_q_heads, n_kv_heads, cache_len, group_size, vl, PageTable{table});
-  };
-  if (bits == 8)
-    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true, true>)
-                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true, true>);
-  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, true, true, false, 4>)
-                          : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, true, true, false, 4>);
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_kv8_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
-                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
-                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
-                                                        void* stream) {
-  return rope_append_rows_kvq_paged("hqq_b200_glue_rope_append_rows_kv8_paged", 8, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
-                                    v_zero, table, k_stage, v_stage, q_out, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch,
-                                    n_pages, dtype, stream);
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_kv4_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                        void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table,
-                                                        void* k_stage, void* v_stage, void* q_out, const int* pos0, const int* n_tok, int n_q_heads,
-                                                        int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages, int dtype,
-                                                        void* stream) {
-  return rope_append_rows_kvq_paged("hqq_b200_glue_rope_append_rows_kv4_paged", 4, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
-                                    v_zero, table, k_stage, v_stage, q_out, pos0, n_tok, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch,
-                                    n_pages, dtype, stream);
 }
 
 // Staging rows [0, pos0[b]) of the slots with n_tok[b] > 0 from a quantised cache: page pools through the table, or (table == nullptr,
@@ -2651,124 +2690,6 @@ extern "C" int hqq_b200_glue_attn_prefill_paged(const void* q_rot, const void* k
 }
 
 // ---- speculative decoding (DESIGN.md 3.5)
-// The checks of the device-position entry points: the prefill shape checks, 1 <= T <= 8 rows per slot, T G <= 64 columns.
-static int spec_args(const char* name, int T, int n_q, int n_kv, int L, int hd, int batch, int dtype) {
-  if (int rc = prefill_args(name, 0, 1, n_q, n_kv, L, hd, batch, dtype)) return rc;
-  HQQ_REQUIRE(T >= 1 && T <= kVerMaxT && T <= L, HQQ_E_INVALID, "%s: needs 1 <= T <= %d and T <= cache_len (T=%d)", name, kVerMaxT, T);
-  HQQ_REQUIRE(T * (n_q / n_kv) <= kVerMaxCols, HQQ_E_UNSUPPORTED, "%s: T * n_q_heads / n_kv_heads must be <= %d", name, kVerMaxCols);
-  return HQQ_OK;
-}
-
-// table == nullptr: contiguous caches; else page pools
-static int rope_append_rows_devpos(const char* name, const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                   void* k_cache, void* v_cache, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
-                                   int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_cache && v_cache && q_out && pos, HQQ_E_INVALID, "%s: null pointer", name);
-  if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  const DevPos dp{(const long long*)pos};
-  auto go = [&](auto tag, auto kernel, auto pg) {
-    using E = decltype(tag);
-    return launch_pdl("rope_append_rows_devpos", kernel, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k, (const E*)v,
-                      (const E*)cos_table, (const E*)sin_table, (E*)k_cache, (E*)v_cache, (E*)q_out, 0, T, n_q_heads, n_kv_heads, cache_len, dp, pg);
-  };
-  if (table) {
-    const PageTable pt{table};
-    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kernel<__half, false, true, true>, pt)
-                            : go(__nv_bfloat16(), rope_append_rows_kernel<__nv_bfloat16, false, true, true>, pt);
-  }
-  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kernel<__half, false, false, true>, NoPages())
-                          : go(__nv_bfloat16(), rope_append_rows_kernel<__nv_bfloat16, false, false, true>, NoPages());
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                     void* k_cache, void* v_cache, void* q_out, const int64_t* pos, int T, int n_q_heads,
-                                                     int n_kv_heads, int cache_len, int head_dim, int batch, int dtype, void* stream) {
-  return rope_append_rows_devpos("hqq_b200_glue_rope_append_rows_devpos", q, k, v, cos_table, sin_table, k_cache, v_cache, nullptr, q_out, pos, T,
-                                 n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype, stream);
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                           void* k_pool, void* v_pool, const int* table, void* q_out, const int64_t* pos, int T,
-                                                           int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int batch, int n_pages, int dtype,
-                                                           void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_devpos_paged";
-  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  return rope_append_rows_devpos(name, q, k, v, cos_table, sin_table, k_pool, v_pool, table, q_out, pos, T, n_q_heads, n_kv_heads, cache_len, head_dim,
-                                 batch, dtype, stream);
-}
-
-// table == nullptr: contiguous quantised caches; else page pools.  bits 8 or 4.
-static int rope_append_rows_kv8_devpos(const char* name, const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                       void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, const int* table, void* q_out,
-                                       const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim, int group_size, int batch,
-                                       int dtype, void* stream, int bits = 8) {
-  HQQ_REQUIRE(q && k && v && cos_table && sin_table && k_q && k_scale && k_zero && v_q && v_scale && v_zero && q_out && pos, HQQ_E_INVALID,
-              "%s: null pointer", name);
-  if (int rc = spec_args(name, T, n_q_heads, n_kv_heads, cache_len, head_dim, batch, dtype)) return rc;
-  if (int rc = kv_group_args(name, bits, group_size)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  const DevPos dp{(const long long*)pos};
-  auto go = [&](auto tag, auto kernel, auto pg) {
-    using E = decltype(tag);
-    return launch_pdl("rope_append_rows_kv8_devpos", kernel, dim3((unsigned)T, (unsigned)batch), dim3(256), 0, st, (const E*)q, (const E*)k,
-                      (const E*)v, (const E*)cos_table, (const E*)sin_table, (uint8_t*)k_q, (E*)k_scale, (E*)k_zero, (uint8_t*)v_q, (E*)v_scale,
-                      (E*)v_zero, (E*)nullptr, (E*)nullptr, (E*)q_out, 0, T, n_q_heads, n_kv_heads, cache_len, group_size, dp, pg);
-  };
-  const PageTable pt{table};
-  if (bits == 4) {
-    if (table)
-      return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, true, true, 4>, pt)
-                              : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, true, true, 4>, pt);
-    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, false, true, 4>, NoPages())
-                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, false, true, 4>, NoPages());
-  }
-  if (table) {
-    return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, true, true>, pt)
-                            : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, true, true>, pt);
-  }
-  return dtype == HQQ_F16 ? go(__half(), rope_append_rows_kv8_kernel<__half, false, false, true>, NoPages())
-                          : go(__nv_bfloat16(), rope_append_rows_kv8_kernel<__nv_bfloat16, false, false, true>, NoPages());
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_kv8_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* q_out,
-                                                         const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
-                                                         int group_size, int batch, int dtype, void* stream) {
-  return rope_append_rows_kv8_devpos("hqq_b200_glue_rope_append_rows_kv8_devpos", q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
-                                     v_zero, nullptr, q_out, pos, T, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_kv8_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
-                                                               const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
-                                                               void* v_zero, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
-                                                               int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages,
-                                                               int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_kv8_devpos_paged";
-  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  return rope_append_rows_kv8_devpos(name, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, q_out, pos, T, n_q_heads,
-                                     n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream);
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_kv4_devpos(const void* q, const void* k, const void* v, const void* cos_table, const void* sin_table,
-                                                         void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale, void* v_zero, void* q_out,
-                                                         const int64_t* pos, int T, int n_q_heads, int n_kv_heads, int cache_len, int head_dim,
-                                                         int group_size, int batch, int dtype, void* stream) {
-  return rope_append_rows_kv8_devpos("hqq_b200_glue_rope_append_rows_kv4_devpos", q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale,
-                                     v_zero, nullptr, q_out, pos, T, n_q_heads, n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
-}
-
-extern "C" int hqq_b200_glue_rope_append_rows_kv4_devpos_paged(const void* q, const void* k, const void* v, const void* cos_table,
-                                                               const void* sin_table, void* k_q, void* k_scale, void* k_zero, void* v_q, void* v_scale,
-                                                               void* v_zero, const int* table, void* q_out, const int64_t* pos, int T, int n_q_heads,
-                                                               int n_kv_heads, int cache_len, int head_dim, int group_size, int batch, int n_pages,
-                                                               int dtype, void* stream) {
-  const char* name = "hqq_b200_glue_rope_append_rows_kv4_devpos_paged";
-  if (int rc = paged_args(name, table, cache_len, n_pages)) return rc;
-  return rope_append_rows_kv8_devpos(name, q, k, v, cos_table, sin_table, k_q, k_scale, k_zero, v_q, v_scale, v_zero, table, q_out, pos, T, n_q_heads,
-                                     n_kv_heads, cache_len, head_dim, group_size, batch, dtype, stream, 4);
-}
-
 // column groups of one kv head in the verify attention
 static int verify_groups(int n_q_heads, int n_kv_heads, int T) { return (int)cdiv((int64_t)T * (n_q_heads / n_kv_heads), kVerCols); }
 

@@ -736,33 +736,25 @@ class DecodeModel:
         names = ("k_cache", "v_cache", "k_scale", "k_zero", "v_scale", "v_zero")
         return sum(blk[n].numel() * blk[n].element_size() for blk in self.blocks for n in names if n in blk)
 
+    def _kv_args(self, blk):
+        """blk's cache arguments in the entry points' order -- [k, v], or [k_q, k_s, k_z, v_q, v_s, v_z] for a quantised cache --
+        the entry-point name suffix of the format ("", "_kv8" or "_kv4") and the arguments after head_dim ([] or [group_size])."""
+        from ._lib import ptr
+        if not self._kvq:
+            return "", [ptr(blk["k_cache"]), ptr(blk["v_cache"])], []
+        names = ("k_cache", "k_scale", "k_zero", "v_cache", "v_scale", "v_zero")
+        return f"_kv{self.kv_bits}", [ptr(blk[n]) for n in names], [self.kv_group_size]
+
     def _attn_split(self, lib, blk, hq, hkv, code, st):
         from ._lib import check, ptr
         b = self._bufs
+        fmt, cache, gs = self._kv_args(blk)
         paged = self.kv_pages is not None
-        kvq = f"kv{self.kv_bits}"
-        if paged and self._kvq:
-            check(getattr(lib, f"hqq_b200_glue_rope_attn_decode_split_{kvq}_paged")(
-                ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]),
-                ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(self.page_table), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq,
-                hkv, self.cache_len, self.shape.head_dim, self.kv_group_size, self.batch, self.kv_pages, code, st))
-            return
-        if paged:
-            check(lib.hqq_b200_glue_rope_attn_decode_split_paged(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                                 ptr(blk["v_cache"]), ptr(self.page_table), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq,
-                                                                 hkv, self.cache_len, self.shape.head_dim, self.batch, self.kv_pages, code, st))
-            return
-        if self._kvq:
-            fn = getattr(lib, f"hqq_b200_glue_rope_attn_decode_split_{kvq}" + ("_seqpos" if self.ragged else ""))
-            check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                     ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
-                     ptr(blk["v_zero"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
-                     self.shape.head_dim, self.kv_group_size, self.batch, code, st))
-            return
-        fn = lib.hqq_b200_glue_rope_attn_decode_split_seqpos if self.ragged else lib.hqq_b200_glue_rope_attn_decode_split
-        check(fn(ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                 ptr(blk["v_cache"]), ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq, hkv, self.cache_len,
-                 self.shape.head_dim, self.batch, code, st))
+        pg, npg = ([ptr(self.page_table)], [self.kv_pages]) if paged else ([], [])
+        lay = "_paged" if paged else "_seqpos" if self.ragged else ""
+        check(getattr(lib, f"hqq_b200_glue_rope_attn_decode_split{fmt}{lay}")(
+            ptr(b["q"]), ptr(b["k"]), ptr(b["v"]), ptr(self.cos), ptr(self.sin), *cache, *pg, ptr(self.pos), ptr(b["a"]), ptr(b["attn_ws"]), hq,
+            hkv, self.cache_len, self.shape.head_dim, *gs, self.batch, *npg, code, st))
 
     # bytes one decode step must read from HBM (SURVEY.md 8d): packed weights + meta + fp16 lm_head row-major
     def bytes_per_token(self, nbits=None, group_size=None) -> float:
@@ -1387,10 +1379,10 @@ class DecodeModel:
         norm = lambda d, w: check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(d), ptr(w), ptr(x), M, s.hidden, s.rms_eps, code, st))
         delta = None
         kv8 = self._kvq  # 8 or 4 bits: the staging pair, as below
-        kvq = f"kv{self.kv_bits}"
         paged = self.kv_pages is not None
-        if paged:
-            pt, npg = ptr(self.page_table), self.kv_pages
+        pg, npg = ([ptr(self.page_table)], [self.kv_pages]) if paged else ([], [])
+        rows = [vp0, vnt] if varlen is not None else [p0, n]
+        lay = "_paged" if paged else "_varlen" if varlen is not None else ""
         if kv8 and attn is None and self._kv8_stage is None:  # one staging pair for all layers: [batch, n_kv, cache_len, 128] each
             self._kv8_stage = tuple(torch.zeros(B, hkv, self.cache_len, hd, device=self.device, dtype=self.dtype) for _ in range(2))
         for blk in self.blocks:
@@ -1398,59 +1390,34 @@ class DecodeModel:
             self._lin(x, (blk["q"], blk["k"], blk["v"]), [q, k, v])
             if attn is not None:
                 attn(blk, q, k, v, qr, a)
-            elif kv8:
-                # staging rows [0, p0) dequantised from the 8-bit cache, rows [p0, p0 + n) written by the rows kernel; the attention
-                # kernel is the one of the fp16 cache, reading the staging pair
-                kst, vst = self._kv8_stage
-                for bi in range(0 if paged or self.kv_bits == 4 else B):
-                    sp0 = p0 if varlen is None else (varlen[0][bi] if varlen[1][bi] else 0)  # slots outside the chunk: nothing
-                    for hh in range(hkv):
-                        for c, dst in (("k", kst), ("v", vst)):
-                            if sp0 > 0:
-                                check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][bi, hh]), ptr(blk[c + "_scale"][bi, hh]), ptr(blk[c + "_zero"][bi, hh]),
-                                                              ptr(dst[bi, hh]), sp0, hd, self.kv_group_size, 8, 1, code, st))
-                if self.kv_bits == 4 and not paged:  # every row is packed on its own: one launch refills the staging rows [0, pos0)
-                    check(lib.hqq_b200_glue_kv4_stage(ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
-                                                      ptr(blk["v_zero"]), ptr(kst), ptr(vst), vp0, vnt, hkv, self.cache_len, hd, self.kv_group_size, B,
-                                                      code, st))
-                if paged:  # one launch refills the staging rows [0, pos0) of the slots in the chunk, through the table
-                    check(getattr(lib, f"hqq_b200_glue_{kvq}_stage_paged")(ptr(blk["k_cache"]), ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]),
-                                                            ptr(blk["v_scale"]), ptr(blk["v_zero"]), pt, ptr(kst), ptr(vst), vp0, vnt, hkv, self.cache_len, hd,
-                                                            self.kv_group_size, B, npg, code, st))
-                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_paged")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                                       ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
-                                                                       ptr(blk["v_zero"]), pt, ptr(kst), ptr(vst), ptr(qr), vp0, vnt, hq, hkv, self.cache_len,
-                                                                       hd, self.kv_group_size, B, npg, code, st))
-                elif varlen is not None:
-                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_varlen")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                                        ptr(blk["k_scale"]), ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]),
-                                                                        ptr(blk["v_zero"]), ptr(kst), ptr(vst), ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd,
-                                                                        self.kv_group_size, B, code, st))
-                else:
-                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["k_scale"]),
-                                                                 ptr(blk["k_zero"]), ptr(blk["v_cache"]), ptr(blk["v_scale"]), ptr(blk["v_zero"]), ptr(kst),
-                                                                 ptr(vst), ptr(qr), p0, n, hq, hkv, self.cache_len, hd, self.kv_group_size, B, code, st))
-                kc, vc = kst, vst
-            elif paged:
-                check(lib.hqq_b200_glue_rope_append_rows_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
-                                                               pt, ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd, B, npg, code, st))
-                kc, vc = blk["k_cache"], blk["v_cache"]
-            elif varlen is not None:
-                check(lib.hqq_b200_glue_rope_append_rows_varlen(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                                ptr(blk["v_cache"]), ptr(qr), vp0, vnt, hq, hkv, self.cache_len, hd, B, code, st))
-                kc, vc = blk["k_cache"], blk["v_cache"]
             else:
-                check(lib.hqq_b200_glue_rope_append_rows(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]), ptr(blk["v_cache"]),
-                                                         ptr(qr), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
+                fmt, cache, gs = self._kv_args(blk)
                 kc, vc = blk["k_cache"], blk["v_cache"]
-            if attn is not None:
-                pass  # the hook's attention output is in a already
-            elif paged and not kv8:
-                check(lib.hqq_b200_glue_attn_prefill_paged(ptr(qr), ptr(kc), ptr(vc), pt, ptr(a), vp0, vnt, hq, hkv, self.cache_len, hd, B, npg, code, st))
-            elif varlen is not None:
-                check(lib.hqq_b200_glue_attn_prefill_varlen(ptr(qr), ptr(kc), ptr(vc), ptr(a), vp0, vnt, hq, hkv, self.cache_len, hd, B, code, st))
-            else:
-                check(lib.hqq_b200_glue_attn_prefill(ptr(qr), ptr(kc), ptr(vc), ptr(a), p0, n, hq, hkv, self.cache_len, hd, B, code, st))
+                stage = []
+                if kv8:
+                    # staging rows [0, p0) dequantised from the quantised cache, rows [p0, p0 + n) written by the append; the attention
+                    # kernel is the one of the fp16 cache, reading the staging pair
+                    kc, vc = self._kv8_stage
+                    stage = [ptr(kc), ptr(vc)]
+                    for bi in range(0 if paged or self.kv_bits == 4 else B):
+                        sp0 = p0 if varlen is None else (varlen[0][bi] if varlen[1][bi] else 0)  # slots outside the chunk: nothing
+                        for hh in range(hkv):
+                            for c, dst in (("k", kc), ("v", vc)):
+                                if sp0 > 0:
+                                    check(lib.hqq_b200_dequantize(ptr(blk[c + "_cache"][bi, hh]), ptr(blk[c + "_scale"][bi, hh]), ptr(blk[c + "_zero"][bi, hh]),
+                                                                  ptr(dst[bi, hh]), sp0, hd, self.kv_group_size, 8, 1, code, st))
+                    if self.kv_bits == 4 and not paged:  # every row is packed on its own: one launch refills the staging rows [0, pos0)
+                        check(lib.hqq_b200_glue_kv4_stage(*cache, *stage, vp0, vnt, hkv, self.cache_len, hd, self.kv_group_size, B, code, st))
+                    if paged:  # one launch refills the staging rows [0, pos0) of the slots in the chunk, through the table
+                        check(getattr(lib, f"hqq_b200_glue{fmt}_stage_paged")(*cache, *pg, *stage, vp0, vnt, hkv, self.cache_len, hd, self.kv_group_size, B,
+                                                                             *npg, code, st))
+                check(getattr(lib, f"hqq_b200_glue_rope_append_rows{fmt}{lay}")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *cache, *pg, *stage,
+                                                                               ptr(qr), *rows, hq, hkv, self.cache_len, hd, *gs, B, *npg, code, st))
+                if paged and not kv8:
+                    check(lib.hqq_b200_glue_attn_prefill_paged(ptr(qr), ptr(kc), ptr(vc), *pg, ptr(a), *rows, hq, hkv, self.cache_len, hd, B, *npg, code, st))
+                else:  # the contiguous caches, or the staging pair
+                    check(getattr(lib, "hqq_b200_glue_attn_prefill" + ("_varlen" if varlen is not None else ""))(
+                        ptr(qr), ptr(kc), ptr(vc), ptr(a), *rows, hq, hkv, self.cache_len, hd, B, code, st))
             self._lin(a, (blk["o"],), [o])
             if self.tp > 1:
                 torch.distributed.all_reduce(o, group=self.pg)
@@ -1689,34 +1656,16 @@ class DecodeModel:
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
         ws = self._bufs["verify_ws"]
 
+        paged = self.kv_pages is not None
+        pg, npg = ([ptr(self.page_table)], [self.kv_pages]) if paged else ([], [])
+        lay = "_paged" if paged else ""
+
         def attn(blk, q, k, v, qr, a):
-            if self._kvq:
-                c8 = [ptr(blk[n]) for n in ("k_cache", "k_scale", "k_zero", "v_cache", "v_scale", "v_zero")]
-                gs = self.kv_group_size
-                kvq = f"kv{self.kv_bits}"
-                if self.kv_pages is None:
-                    check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_devpos")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, ptr(qr), ptr(self.pos), T,
-                                                                        hq, hkv, L, hd, gs, B, code, st))
-                    check(getattr(lib, f"hqq_b200_glue_attn_verify_split_{kvq}")(ptr(qr), *c8, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B, code, st))
-                    return
-                pt = ptr(self.page_table)
-                check(getattr(lib, f"hqq_b200_glue_rope_append_rows_{kvq}_devpos_paged")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *c8, pt, ptr(qr),
-                                                                          ptr(self.pos), T, hq, hkv, L, hd, gs, B, self.kv_pages, code, st))
-                check(getattr(lib, f"hqq_b200_glue_attn_verify_split_{kvq}_paged")(ptr(qr), *c8, pt, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, gs, T, B,
-                                                                    self.kv_pages, code, st))
-                return
-            if self.kv_pages is None:
-                check(lib.hqq_b200_glue_rope_append_rows_devpos(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                                ptr(blk["v_cache"]), ptr(qr), ptr(self.pos), T, hq, hkv, L, hd, B, code, st))
-                check(lib.hqq_b200_glue_attn_verify_split(ptr(qr), ptr(blk["k_cache"]), ptr(blk["v_cache"]), ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L,
-                                                          hd, T, B, code, st))
-                return
-            pt = ptr(self.page_table)
-            check(lib.hqq_b200_glue_rope_append_rows_devpos_paged(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), ptr(blk["k_cache"]),
-                                                                  ptr(blk["v_cache"]), pt, ptr(qr), ptr(self.pos), T, hq, hkv, L, hd, B, self.kv_pages,
-                                                                  code, st))
-            check(lib.hqq_b200_glue_attn_verify_split_paged(ptr(qr), ptr(blk["k_cache"]), ptr(blk["v_cache"]), pt, ptr(self.pos), ptr(a), ptr(ws), hq,
-                                                            hkv, L, hd, T, B, self.kv_pages, code, st))
+            fmt, cache, gs = self._kv_args(blk)
+            check(getattr(lib, f"hqq_b200_glue_rope_append_rows{fmt}_devpos{lay}")(ptr(q), ptr(k), ptr(v), ptr(self.cos), ptr(self.sin), *cache, *pg, ptr(qr),
+                                                                                 ptr(self.pos), T, hq, hkv, L, hd, *gs, B, *npg, code, st))
+            check(getattr(lib, f"hqq_b200_glue_attn_verify_split{fmt}{lay}")(ptr(qr), *cache, *pg, ptr(self.pos), ptr(a), ptr(ws), hq, hkv, L, hd, *gs, T, B,
+                                                                            *npg, code, st))
 
         h, delta = self._prefill_chunk_fused(self._spec_window_ids(), 0, hd, hq, hkv, attn=attn)
         x = torch.empty_like(h)
