@@ -48,6 +48,10 @@ SIGNATURES = {
     "hqq_b200_linear_fwd_multi": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
                                           c_int, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "hqq_b200_linear_fwd_route": (c_int, [c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int]),
+    "hqq_b200_linear_fwd_grouped": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
+                                            c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p]),
+    "hqq_b200_glue_moe_route": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int] + [c_void_p] * 7 + [c_int, c_void_p]),
+    "hqq_b200_glue_moe_combine": (c_int, [c_void_p] * 5 + [c_int] * 4 + [c_void_p]),
     "hqq_b200_decode_linear_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p]),
     "hqq_b200_decode_linear_fwd_desc": (c_int, [c_void_p, c_void_p]),

@@ -135,6 +135,145 @@ __global__ void __launch_bounds__(256) silu_mul_kernel(const T* __restrict__ g, 
   }
 }
 
+// ---- mixture-of-experts router and combine (Mixtral-style sparse MLP) -------------------------------------------------------
+// Router: one CTA per token row m of x [M, H]; router [E, H].
+//   l[e] = T(sum_k x[m][k] router[e][k])  (fp32 sum, one rounding to T: transformers computes F.linear in the model dtype)
+//   p = softmax(l) in fp32; the k largest p, ties to the lower expert index, in descending order; w_j = p_j / sum_j p_j (fp32)
+// ids / weights [M, k] take them in that order.  The last CTA to finish (a ticket counter, reset to zero by that CTA) groups the
+// M k pairs by expert: pairs of expert e are the slots [off[e], off[e] + cnt[e]) in ascending token order, token[slot] the row a
+// pair came from, pair_of[m][j] the slot of (m, j).  Every thread of that CTA owns a contiguous run of tokens, counts its pairs per
+// expert, and a scan over the threads in thread order hands each run its first slot per expert: no atomics touch the output.
+constexpr int kRouteThreads = 256;
+constexpr int kMaxExperts = 64;
+
+template <typename T>
+__global__ void __launch_bounds__(kRouteThreads) moe_route_kernel(const T* __restrict__ x, const T* __restrict__ router, int M, int H, int E, int k,
+                                                                 int* __restrict__ ids, float* __restrict__ weights, int* __restrict__ pair_of,
+                                                                 int* __restrict__ off, int* __restrict__ cnt, int* __restrict__ token,
+                                                                 unsigned* ticket) {
+  __shared__ float part[kRouteThreads / 32][kMaxExperts];
+  __shared__ unsigned short run[kMaxExperts * kRouteThreads];  // [e][thread]: pairs of expert e in the thread's tokens, then its next slot
+  __shared__ int first[kMaxExperts];
+  __shared__ int is_last;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int m = blockIdx.x;
+  pdl_launch_dependents();
+  pdl_wait();
+  const T* xr = x + (long long)m * H;
+  for (int e = 0; e < E; ++e) {
+    const T* wr = router + (long long)e * H;
+    float acc = 0.0f;
+    for (int i = tid * 8; i < H; i += kRouteThreads * 8) {
+      const Vec<T, 8> a = *reinterpret_cast<const Vec<T, 8>*>(xr + i);
+      const Vec<T, 8> b = *reinterpret_cast<const Vec<T, 8>*>(wr + i);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc += to_f32<T>(a.v[j]) * to_f32<T>(b.v[j]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (lane == 0) part[warp][e] = acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float p[kMaxExperts];
+    float mx = -INFINITY;
+    for (int e = 0; e < E; ++e) {
+      float l = 0.0f;
+      for (int w = 0; w < kRouteThreads / 32; ++w) l += part[w][e];
+      p[e] = to_f32<T>(from_f32<T>(l));
+      mx = fmaxf(mx, p[e]);
+    }
+    float sum = 0.0f;
+    for (int e = 0; e < E; ++e) { p[e] = expf(p[e] - mx); sum += p[e]; }
+    for (int e = 0; e < E; ++e) p[e] = p[e] / sum;
+    unsigned long long taken = 0;
+    int sel[8];
+    float top = 0.0f;
+    for (int j = 0; j < k; ++j) {
+      int best = -1;
+      for (int e = 0; e < E; ++e)
+        if (!((taken >> e) & 1ull) && (best < 0 || p[e] > p[best])) best = e;  // strict: the lower index keeps a tie
+      taken |= 1ull << best;
+      sel[j] = best;
+      top += p[best];
+    }
+    for (int j = 0; j < k; ++j) {
+      ids[(long long)m * k + j] = sel[j];
+      weights[(long long)m * k + j] = p[sel[j]] / top;
+    }
+    __threadfence();
+    is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  // ---- the last CTA: group the pairs by expert
+  const int per = (M + kRouteThreads - 1) / kRouteThreads;
+  const int t0 = min(M, tid * per), t1 = min(M, t0 + per);
+  for (int e = 0; e < E; ++e) run[e * kRouteThreads + tid] = 0;
+  for (int t = t0; t < t1; ++t)
+    for (int j = 0; j < k; ++j) ++run[__ldcg(ids + (long long)t * k + j) * kRouteThreads + tid];
+  __syncthreads();
+  if (tid < E) {  // exclusive scan over the threads, in thread order (a count never exceeds M <= 65535)
+    int c = 0;
+    for (int i = 0; i < kRouteThreads; ++i) {
+      const int v = run[tid * kRouteThreads + i];
+      run[tid * kRouteThreads + i] = (unsigned short)c;
+      c += v;
+    }
+    first[tid] = c;  // the expert's pair count, for now
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int o = 0;
+    for (int e = 0; e < E; ++e) {
+      const int c = first[e];
+      off[e] = o; cnt[e] = c; first[e] = o;
+      o += c;
+    }
+    *ticket = 0;  // every launch leaves the counter at zero (graph replays)
+  }
+  __syncthreads();
+  for (int t = t0; t < t1; ++t)
+    for (int j = 0; j < k; ++j) {
+      const int e = __ldcg(ids + (long long)t * k + j);
+      const int slot = first[e] + run[e * kRouteThreads + tid]++;
+      token[slot] = t;
+      pair_of[(long long)t * k + j] = slot;
+    }
+}
+
+// Combine: delta[m] = sum over token m's k pairs in ascending expert id of T(y[pair] * w), accumulated in T from 0 -- the arithmetic
+// of transformers' MixtralExperts (fp32 product, .to(dtype), index_add_ one expert at a time).  One CTA per row.
+template <typename T>
+__global__ void __launch_bounds__(256) moe_combine_kernel(const T* __restrict__ y, const int* __restrict__ ids, const float* __restrict__ weights,
+                                                         const int* __restrict__ pair_of, T* __restrict__ delta, int H, int k) {
+  __shared__ int s_pair[8];
+  __shared__ float s_w[8];
+  const int m = blockIdx.x;
+  pdl_launch_dependents();
+  pdl_wait();
+  if (threadIdx.x == 0) {
+    int e[8];
+    for (int j = 0; j < k; ++j) { e[j] = ids[(long long)m * k + j]; s_pair[j] = pair_of[(long long)m * k + j]; s_w[j] = weights[(long long)m * k + j]; }
+    for (int j = 1; j < k; ++j)  // insertion sort by expert id (ids of a token are distinct)
+      for (int i = j; i > 0 && e[i - 1] > e[i]; --i) {
+        const int te = e[i]; e[i] = e[i - 1]; e[i - 1] = te;
+        const int tp = s_pair[i]; s_pair[i] = s_pair[i - 1]; s_pair[i - 1] = tp;
+        const float tw = s_w[i]; s_w[i] = s_w[i - 1]; s_w[i - 1] = tw;
+      }
+  }
+  __syncthreads();
+  for (int h = threadIdx.x; h < H; h += blockDim.x) {
+    T acc = from_f32<T>(0.0f);
+    for (int j = 0; j < k; ++j) {
+      const T term = from_f32<T>(to_f32<T>(y[(long long)s_pair[j] * H + h]) * s_w[j]);
+      acc = from_f32<T>(to_f32<T>(acc) + to_f32<T>(term));
+    }
+    delta[(long long)m * H + h] = acc;
+  }
+}
+
 // Paged KV cache (PAGED instantiations of the ragged kernels): a cache is a pool of pages [pages, n_kv, 64, 128], a page holding 64
 // positions of one sequence for every kv head, and row p of slot b, kv head h lives at row (table[b][p / 64] n_kv + h) 64 + p % 64 of
 // the pool; table is int32 [batch, L / 64].  Decode tiles (16 positions) and prefill tiles (64), aligned to absolute positions, never
@@ -2125,6 +2264,44 @@ extern "C" int hqq_b200_glue_silu_mul(const void* gate, const void* up, void* y,
   if (dtype == HQQ_F16) return launch_pdl("silu_mul", silu_mul_kernel<__half>, grid, dim3(256), 0, st, (const __half*)gate, (const __half*)up, (__half*)y, n);
   if (dtype == HQQ_BF16) return launch_pdl("silu_mul", silu_mul_kernel<__nv_bfloat16>, grid, dim3(256), 0, st, (const __nv_bfloat16*)gate, (const __nv_bfloat16*)up, (__nv_bfloat16*)y, n);
   set_error("hqq_b200_glue_silu_mul: dtype must be f16/bf16");
+  return HQQ_E_INVALID;
+}
+
+extern "C" int hqq_b200_glue_moe_route(const void* x, const void* router, int M, int H, int n_experts, int k, int32_t* ids, float* weights,
+                                       int32_t* pair_of, int32_t* expert_off, int32_t* expert_cnt, int32_t* pair_token, void* ticket, int dtype,
+                                       void* stream) {
+  HQQ_REQUIRE(x && router && ids && weights && pair_of && expert_off && expert_cnt && pair_token && ticket, HQQ_E_INVALID,
+              "hqq_b200_glue_moe_route: null pointer");
+  HQQ_REQUIRE(n_experts >= 2 && n_experts <= kMaxExperts, HQQ_E_INVALID, "hqq_b200_glue_moe_route: n_experts must be in [2, %d] (got %d)", kMaxExperts,
+              n_experts);
+  HQQ_REQUIRE(k >= 1 && k <= 8 && k <= n_experts, HQQ_E_INVALID, "hqq_b200_glue_moe_route: k must be in [1, min(8, n_experts)] (got %d)", k);
+  HQQ_REQUIRE(M >= 1 && M <= 65535, HQQ_E_INVALID, "hqq_b200_glue_moe_route: M must be in [1, 65535] (got %d)", M);
+  HQQ_REQUIRE(H > 0 && H % 8 == 0 && aligned(x, 16) && aligned(router, 16), HQQ_E_INVALID,
+              "hqq_b200_glue_moe_route: H must be a positive multiple of 8 and x / router 16-byte aligned (H=%d)", H);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == HQQ_F16)
+    return launch_pdl("moe_route", moe_route_kernel<__half>, dim3(M), dim3(kRouteThreads), 0, st, (const __half*)x, (const __half*)router, M, H,
+                      n_experts, k, (int*)ids, weights, (int*)pair_of, (int*)expert_off, (int*)expert_cnt, (int*)pair_token, (unsigned*)ticket);
+  if (dtype == HQQ_BF16)
+    return launch_pdl("moe_route", moe_route_kernel<__nv_bfloat16>, dim3(M), dim3(kRouteThreads), 0, st, (const __nv_bfloat16*)x,
+                      (const __nv_bfloat16*)router, M, H, n_experts, k, (int*)ids, weights, (int*)pair_of, (int*)expert_off, (int*)expert_cnt,
+                      (int*)pair_token, (unsigned*)ticket);
+  set_error("hqq_b200_glue_moe_route: dtype must be f16/bf16");
+  return HQQ_E_INVALID;
+}
+
+extern "C" int hqq_b200_glue_moe_combine(const void* y, const int32_t* ids, const float* weights, const int32_t* pair_of, void* delta, int M, int H,
+                                         int k, int dtype, void* stream) {
+  HQQ_REQUIRE(y && ids && weights && pair_of && delta, HQQ_E_INVALID, "hqq_b200_glue_moe_combine: null pointer");
+  HQQ_REQUIRE(M >= 1 && M <= 65535 && H > 0 && k >= 1 && k <= 8, HQQ_E_INVALID, "hqq_b200_glue_moe_combine: bad shape (M=%d H=%d k=%d)", M, H, k);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == HQQ_F16)
+    return launch_pdl("moe_combine", moe_combine_kernel<__half>, dim3(M), dim3(256), 0, st, (const __half*)y, (const int*)ids, weights,
+                      (const int*)pair_of, (__half*)delta, H, k);
+  if (dtype == HQQ_BF16)
+    return launch_pdl("moe_combine", moe_combine_kernel<__nv_bfloat16>, dim3(M), dim3(256), 0, st, (const __nv_bfloat16*)y, (const int*)ids, weights,
+                      (const int*)pair_of, (__nv_bfloat16*)delta, H, k);
+  set_error("hqq_b200_glue_moe_combine: dtype must be f16/bf16");
   return HQQ_E_INVALID;
 }
 

@@ -9,6 +9,9 @@ int linear_small_multi(const void* x, int nprob, const void* const* Wq, const vo
                        void* ws, size_t ws_bytes, cudaStream_t st, int xop = 0, const void* x2 = nullptr, const void* xw = nullptr,
                        void* h_out = nullptr, float eps = 0.0f, const TpExchange* tpx = nullptr);
 bool small_xop_ok(int64_t M, int64_t K);
+int linear_small_grouped(const void* x, const int* x_rows, int nprob, const void* const* Wq, const void* const* scale, const void* const* zero,
+                         void* const* y, const int64_t* N, int64_t K, int n_experts, const int* expert_off, const int* expert_cnt,
+                         int64_t max_pairs, int gs, int nbits, int dtype, cudaStream_t st);
 bool gemm_route_ok(int64_t M, int64_t N, int64_t K, int gs, int nbits, int axis, int dtype);
 size_t gemm_workspace_bytes(int64_t M, int64_t N, int64_t K, int gs, int nbits, int dtype);
 int linear_gemm(const void* x, const void* Wq, const void* scale, const void* zero, const void* bias, void* y, int64_t M,
@@ -116,6 +119,32 @@ extern "C" int hqq_b200_linear_fwd_multi(const void* x, int count, const void* c
     }
   }
   return linear_small_multi(x, count, W_q, scale, zero, bias, y, N, M, K, group_size, nbits, dtype, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int hqq_b200_linear_fwd_grouped(const void* x, const int32_t* x_rows, int count, const void* const* W_q, const void* const* scale,
+                                           const void* const* zero, void* const* y, const int64_t* N, int64_t K, int n_experts,
+                                           const int32_t* expert_off, const int32_t* expert_cnt, int64_t max_pairs, int group_size, int nbits,
+                                           int dtype, void* stream) {
+  int rc = check_common(x, 1, K, group_size, nbits, 1);
+  if (rc) return rc;
+  HQQ_REQUIRE(count >= 1 && count <= 4 && W_q && scale && zero && y && N, HQQ_E_INVALID, "hqq_b200_linear_fwd_grouped: 1..4 matrices, non-null arrays");
+  HQQ_REQUIRE(n_experts >= 1 && n_experts <= 64, HQQ_E_INVALID, "hqq_b200_linear_fwd_grouped: 1..64 experts (got %d)", n_experts);
+  HQQ_REQUIRE(expert_off && expert_cnt, HQQ_E_INVALID, "hqq_b200_linear_fwd_grouped: null expert tables");
+  HQQ_REQUIRE(max_pairs >= 1 && max_pairs <= 65535LL * 8, HQQ_E_INVALID, "hqq_b200_linear_fwd_grouped: max_pairs must be in [1, 524280] (got %lld)",
+              (long long)max_pairs);
+  HQQ_REQUIRE(aligned(x, 16), HQQ_E_INVALID, "hqq_b200_linear_fwd_grouped: x must be 16-byte aligned");
+  for (int i = 0; i < count; ++i) {
+    HQQ_REQUIRE(W_q[i] && scale[i] && zero[i] && y[i] && N[i] > 0, HQQ_E_INVALID, "hqq_b200_linear_fwd_grouped: null pointer or empty matrix %d", i);
+    HQQ_REQUIRE(aligned(W_q[i], 16) && aligned(scale[i], 8) && aligned(zero[i], 8), HQQ_E_INVALID,
+                "hqq_b200_linear_fwd_grouped: W_q must be 16-byte and scale/zero 8-byte aligned");
+    if (!small_route_ok(1, N[i], K, group_size, nbits, 1, dtype)) {
+      set_error("hqq_b200_linear_fwd_grouped: matrix %d (N=%lld K=%lld gs=%d nbits=%d dtype=%d) is outside the small-M kernel", i, (long long)N[i],
+                (long long)K, group_size, nbits, dtype);
+      return HQQ_E_UNSUPPORTED;
+    }
+  }
+  return linear_small_grouped(x, x_rows, count, W_q, scale, zero, y, N, K, n_experts, expert_off, expert_cnt, max_pairs, group_size, nbits, dtype,
+                              (cudaStream_t)stream);
 }
 
 extern "C" int hqq_b200_decode_linear_fwd(const void* x, int x_op, const void* x2, const void* x_weight, void* h_out, float eps, int count,

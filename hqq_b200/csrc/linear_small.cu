@@ -19,6 +19,12 @@
 // in shared memory (per warp ST stages of one 256-k unit, 2 KB, or 4 KB at 8 bits; ST - 1 of them in flight, prefetching
 // across tile boundaries), then reduce through shared memory in a fixed order: deterministic, no atomics, no workspace.
 // Launched with programmatic dependent launch: the weight prefetch starts before the producer of x has finished.
+//
+// Grouped mode (GR = true, mixture-of-experts): every matrix is a stack of g_E experts, each in the layout above, back to back.  The
+// router's tables in device memory say how many pairs (rows) each expert takes and where its pairs start; the work list is then
+// (chunk, tile) with a chunk at most 8 MT pairs of one expert, so experts without pairs cost nothing.  Those tables are written by
+// the kernel in front, so they -- and with them every weight address -- are read after the programmatic-dependency wait: this
+// mode cannot prefetch weights under its producer's tail.
 #include <string.h>
 #include <type_traits>
 
@@ -79,6 +85,12 @@ struct SKArgs {
   const uint32_t* x2tag;
   const int* step_ctr;
   int x_index, x_per_step;
+  // grouped mode: pair p of expert e (p in [g_off[e], g_off[e] + g_cnt[e])) reads x row g_rows[p] (g_rows null: row p) and writes
+  // output row p; g_tiles = the 16-row tiles of one chunk over all matrices
+  const int* g_off;
+  const int* g_cnt;
+  const int* g_rows;
+  int g_E, g_tiles;
 };
 
 #ifdef HQQ_EMU
@@ -275,6 +287,7 @@ struct SKCfg {
   static constexpr int P_BYTES = 2 * 8 * MT * 128 * 4;  // double-buffered split-K partials, one 16x8 tile per warp
   static constexpr int SMEM = W_BYTES + P_BYTES;
   static constexpr int MIN_CTAS = (SMEM <= 110 * 1024 && MT <= 2) ? 2 : 1;
+  static constexpr int G_BYTES = 1024;  // grouped mode: per expert its first chunk, first pair and pair count (E <= 64)
 };
 
 // Persistent CTAs; CTA b owns the 16-row tiles b, b+grid, b+2*grid, ... of the concatenated tile list of up to four
@@ -282,7 +295,7 @@ struct SKCfg {
 // per-thread cp.async rings (the ring keeps prefetching across tile boundaries, so HBM requests never drain).  Partials
 // meet in shared memory once per tile (one block barrier, double-buffered) and warp (tile % 8) adds them in warp order:
 // deterministic, no atomics, no global workspace.
-template <typename T, int NBITS, int GS, int MT>
+template <typename T, int NBITS, int GS, int MT, bool GR = false>
 __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT>::MIN_CTAS) linear_small_kernel(const __grid_constant__ SKArgs a) {
   using C = SKCfg<T, NBITS, GS, MT>;
   constexpr int F = C::F, P = C::P, MPG = C::MPG, GPB = C::GPB, NWV = C::NWV, ST = C::ST;
@@ -301,18 +314,41 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT>::MIN_CTAS) linear
   // this warp's k-chunk of every tile (the same for all tiles: all matrices share K)
   const int kb0 = a.KB * warp / 8, kb1 = a.KB * (warp + 1) / 8;
   const int upt = kb1 - kb0;  // units per tile for this warp (may be 0 when K < 2048)
-  const int n_tiles = (a.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles owned by this CTA
+  constexpr int R = 8 * MT;   // grouped mode: pairs per chunk
+  int* g_chunk = reinterpret_cast<int*>(smem + C::SMEM);  // grouped mode: [E + 1] first chunk, [E] first pair, [E] pair count
+  int* g_off = g_chunk + 65;
+  int* g_cnt = g_off + 64;
+  int total_tiles = a.total_tiles;
+  if constexpr (GR) {
+    pdl_launch_dependents();
+    pdl_wait();
+    if (tid == 0) {
+      int ch = 0;
+      for (int e = 0; e < a.g_E; ++e) {
+        const int n = a.g_cnt[e];
+        g_chunk[e] = ch; g_off[e] = a.g_off[e]; g_cnt[e] = n;
+        ch += (n + R - 1) / R;
+      }
+      g_chunk[a.g_E] = ch;
+    }
+    __syncthreads();
+    total_tiles = g_chunk[a.g_E] * a.g_tiles;
+  }
+  const int n_tiles = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;  // tiles owned by this CTA
   if (n_tiles <= 0) return;
 
   struct Tile {
     const uint8_t* Wq; const T* scale; const T* zero; const T* bias; T* y;
     int N, step, tile0;
+    int r0, rows;  // the tile's output rows: [r0, r0 + rows)
   };
   auto locate = [&](int gt, Tile& t) {
+    int ch = 0, lt = gt;  // grouped mode: chunk, and tile within the chunk
+    if constexpr (GR) { ch = gt / a.g_tiles; lt = gt - ch * a.g_tiles; }
     int pi = 0;
 #pragma unroll
     for (int i = 1; i < kMaxProb; ++i)
-      if (i < a.nprob && gt >= a.p[i].tile0) pi = i;
+      if (i < a.nprob && lt >= a.p[i].tile0) pi = i;
     const uint8_t* Wq = a.p[0].Wq; const void* sc = a.p[0].scale; const void* ze = a.p[0].zero; const void* bi = a.p[0].bias;
     void* y = a.p[0].y; int N = a.p[0].N, step = a.p[0].step, tile0 = a.p[0].tile0;
 #pragma unroll
@@ -320,6 +356,21 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT>::MIN_CTAS) linear
       if (pi == i) { Wq = a.p[i].Wq; sc = a.p[i].scale; ze = a.p[i].zero; bi = a.p[i].bias; y = a.p[i].y; N = a.p[i].N; step = a.p[i].step; tile0 = a.p[i].tile0; }
     t.Wq = Wq; t.scale = reinterpret_cast<const T*>(sc); t.zero = reinterpret_cast<const T*>(ze);
     t.bias = reinterpret_cast<const T*>(bi); t.y = reinterpret_cast<T*>(y); t.N = N; t.step = step; t.tile0 = tile0;
+    t.r0 = 0; t.rows = a.M;
+    if constexpr (GR) {
+      int lo = 0, hi = a.g_E;  // the expert: the last e with g_chunk[e] <= ch (experts without pairs own no chunk)
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (g_chunk[mid] <= ch) lo = mid; else hi = mid;
+      }
+      const int j = (ch - g_chunk[lo]) * R;
+      t.r0 = g_off[lo] + j;
+      t.rows = min(R, g_cnt[lo] - j);
+      t.Wq += (long long)lo * step * a.K;
+      t.scale += (long long)lo * N * a.Gk;
+      t.zero += (long long)lo * N * a.Gk;
+      t.tile0 += ch * a.g_tiles;
+    }
   };
   auto rows = [&](int gt, Tile& t, int& prow_a, int& prow_b) {
     locate(gt, t);
@@ -390,16 +441,28 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT>::MIN_CTAS) linear
   // so under PDL this prologue overlaps the tail of whatever produced x.
 #pragma unroll
   for (int s = 0; s < ST - 1; ++s) issue(s);
-  pdl_launch_dependents();
-  pdl_wait();
+  if constexpr (!GR) {
+    pdl_launch_dependents();
+    pdl_wait();
+  }
 
   const T* xbase[MT];
+  auto set_x = [&](int ti) {  // the x rows of this CTA's tile ti
+    int r0 = 0, rows = a.M;
+    if constexpr (GR) {
+      Tile t;
+      locate((int)blockIdx.x + ti * (int)gridDim.x, t);
+      r0 = t.r0; rows = t.rows;
+    }
 #pragma unroll
-  for (int mt = 0; mt < MT; ++mt) {
-    // token columns >= M alias the last real token: MMA columns are independent and never stored
-    const int m = min(mt * 8 + r, a.M - 1);
-    xbase[mt] = reinterpret_cast<const T*>(a.x) + (long long)m * a.K + 16 * c;
-  }
+    for (int mt = 0; mt < MT; ++mt) {
+      // token columns >= rows alias the last real token: MMA columns are independent and never stored
+      long long m = r0 + min(mt * 8 + r, rows - 1);
+      if (GR && a.g_rows) m = a.g_rows[m];
+      xbase[mt] = reinterpret_cast<const T*>(a.x) + m * a.K + 16 * c;
+    }
+  };
+  set_x(0);
   // activations are software-pipelined one k64 step ahead (they come from L1/L2, 16 consecutive k per thread)
   uint4 xa[MT], xb[MT];
   auto load_x = [&](int kb, int us) {
@@ -440,7 +503,12 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT>::MIN_CTAS) linear
         uint4 ya[MT], yb[MT];
 #pragma unroll
         for (int mt = 0; mt < MT; ++mt) { ya[mt] = xa[mt]; yb[mt] = xb[mt]; }
-        if (us < 3) load_x(kb, us + 1); else load_x(kb_next, 0);
+        if (us < 3) {
+          load_x(kb, us + 1);
+        } else {
+          if (GR && ku + 1 == upt && ti + 1 < n_tiles) set_x(ti + 1);  // grouped mode: the next tile may take other rows
+          load_x(kb_next, 0);
+        }
         const uint4 va = wring[(stage * NWV + us) * 256 + tid];
         uint4 vb = va;
         if (F == 1) vb = wring[(stage * NWV + 4 + us) * 256 + tid];
@@ -502,13 +570,14 @@ __global__ void __launch_bounds__(256, SKCfg<T, NBITS, GS, MT>::MIN_CTAS) linear
           acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
         }
         const int m0 = mt * 8 + 2 * c;
-        if (m0 < a.M) {
-          if (ok_a) MM::st(t.y, (long long)m0 * t.N + n_a, acc.x, t.bias, n_a);
-          if (ok_b) MM::st(t.y, (long long)m0 * t.N + n_b, acc.z, t.bias, n_b);
+        const long long o0 = (long long)(t.r0 + m0) * t.N;
+        if (m0 < t.rows) {
+          if (ok_a) MM::st(t.y, o0 + n_a, acc.x, t.bias, n_a);
+          if (ok_b) MM::st(t.y, o0 + n_b, acc.z, t.bias, n_b);
         }
-        if (m0 + 1 < a.M) {
-          if (ok_a) MM::st(t.y, (long long)(m0 + 1) * t.N + n_a, acc.y, t.bias, n_a);
-          if (ok_b) MM::st(t.y, (long long)(m0 + 1) * t.N + n_b, acc.w, t.bias, n_b);
+        if (m0 + 1 < t.rows) {
+          if (ok_a) MM::st(t.y, o0 + t.N + n_a, acc.y, t.bias, n_a);
+          if (ok_b) MM::st(t.y, o0 + t.N + n_b, acc.w, t.bias, n_b);
         }
       }
     }
@@ -915,23 +984,25 @@ __global__ void __launch_bounds__(256, MC) linear_decode1_kernel(const __grid_co
 }
 
 // ---------------------------------------------------------------------------------------------------------
-template <typename T, int NBITS, int GS, int MT>
+template <typename T, int NBITS, int GS, int MT, bool GR>
 static int launch_sk(SKArgs& a, cudaStream_t st) {
   using C = SKCfg<T, NBITS, GS, MT>;
-  int rc = reserve_smem<linear_small_kernel<T, NBITS, GS, MT>>(C::SMEM);
+  const int smem = C::SMEM + (GR ? C::G_BYTES : 0);
+  int rc = reserve_smem<linear_small_kernel<T, NBITS, GS, MT, GR>>(smem);
   if (rc) return rc;
   static int per_sm[kMaxDevices] = {};  // resident CTAs per SM, at most 2
   int& occ = per_sm[current_device()];
   if (!occ) {
     int n = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, linear_small_kernel<T, NBITS, GS, MT>, 256, C::SMEM);
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, linear_small_kernel<T, NBITS, GS, MT, GR>, 256, smem);
     HQQ_REQUIRE(e == cudaSuccess && n > 0, HQQ_E_CUDA, "hqq_b200_linear_fwd: occupancy query failed: %s", cudaGetErrorString(e));
     occ = n > 2 ? 2 : n;
   }
-  // one CTA per tile up to every resident slot: the kernel is bound per SM, so filling every slot wins over evening out rounds
+  // one CTA per tile up to every resident slot: the kernel is bound per SM, so filling every slot wins over evening out rounds.
+  // Grouped mode: a.total_tiles is the bound from the host's upper bound on the pairs; the kernel walks the tiles that exist.
   const int max_grid = sm_count() * occ;
-  return launch_pdl("hqq_b200_linear_fwd/small", linear_small_kernel<T, NBITS, GS, MT>, dim3((unsigned)(a.total_tiles < max_grid ? a.total_tiles : max_grid)),
-                    dim3(256), C::SMEM, st, a);
+  return launch_pdl(GR ? "hqq_b200_linear_fwd/grouped" : "hqq_b200_linear_fwd/small", linear_small_kernel<T, NBITS, GS, MT, GR>,
+                    dim3((unsigned)(a.total_tiles < max_grid ? a.total_tiles : max_grid)), dim3(256), smem, st, a);
 }
 
 template <typename T, int NBITS, int GS, int ST, int MC, int MR = 0>
@@ -948,9 +1019,9 @@ static int launch_d1(SKArgs& a, cudaStream_t st) {
 
 bool small_xop_ok(int64_t M, int64_t K) { return M == 1 && K <= 16384; }  // the one-token kernel
 
-template <typename T, int NBITS, int GS>
+template <typename T, int NBITS, int GS, bool GR>
 static int sk_mt(SKArgs& a, cudaStream_t st) {
-  if (small_xop_ok(a.M, a.K)) {
+  if (!GR && small_xop_ok(a.M, a.K)) {
     if constexpr (NBITS == 8) {
       return launch_d1<T, NBITS, GS, 2, 2>(a, st);
     } else {
@@ -964,29 +1035,29 @@ static int sk_mt(SKArgs& a, cudaStream_t st) {
       return launch_d1<T, NBITS, GS, 4, 2>(a, st);
     }
   }
-  if (a.M <= 8) return launch_sk<T, NBITS, GS, 1>(a, st);
-  if (a.M <= 16) return launch_sk<T, NBITS, GS, 2>(a, st);
-  return launch_sk<T, NBITS, GS, 4>(a, st);
+  if (a.M <= 8) return launch_sk<T, NBITS, GS, 1, GR>(a, st);
+  if (a.M <= 16) return launch_sk<T, NBITS, GS, 2, GR>(a, st);
+  return launch_sk<T, NBITS, GS, 4, GR>(a, st);
 }
 
-template <typename T, int NBITS>
+template <typename T, int NBITS, bool GR>
 static int sk_gs(SKArgs& a, int gs, cudaStream_t st) {
   switch (gs) {
-    case 64: return sk_mt<T, NBITS, 64>(a, st);
-    case 128: return sk_mt<T, NBITS, 128>(a, st);
+    case 64: return sk_mt<T, NBITS, 64, GR>(a, st);
+    case 128: return sk_mt<T, NBITS, 128, GR>(a, st);
   }
   return HQQ_E_UNSUPPORTED;
 }
 
-template <typename T>
+template <typename T, bool GR = false>
 static int sk_bits(SKArgs& a, int gs, int nbits, cudaStream_t st) {
   switch (nbits) {
     case 8:
-      if constexpr (std::is_same<T, __half>::value) return sk_gs<T, 8>(a, gs, st);
+      if constexpr (std::is_same<T, __half>::value) return sk_gs<T, 8, GR>(a, gs, st);
       else return HQQ_E_UNSUPPORTED;
-    case 4: return sk_gs<T, 4>(a, gs, st);
-    case 2: return sk_gs<T, 2>(a, gs, st);
-    case 1: return sk_gs<T, 1>(a, gs, st);
+    case 4: return sk_gs<T, 4, GR>(a, gs, st);
+    case 2: return sk_gs<T, 2, GR>(a, gs, st);
+    case 1: return sk_gs<T, 1, GR>(a, gs, st);
   }
   return HQQ_E_UNSUPPORTED;
 }
@@ -1029,6 +1100,7 @@ int linear_small_multi(const void* x, int nprob, const void* const* Wq, const vo
   }
   a.tp = 1; a.rank = 0; a.red_data = nullptr; a.xtag = nullptr; a.x2tag = nullptr; a.step_ctr = nullptr; a.x_index = 0; a.x_per_step = 1;
   for (int i = 0; i < 8; ++i) a.peer_data[i] = nullptr;
+  a.g_off = a.g_cnt = a.g_rows = nullptr; a.g_E = a.g_tiles = 0;
   if (tpx && !tpx->step_ctr) tpx = nullptr;
   if (tpx) {
     HQQ_REQUIRE(small_xop_ok(M, K) && nprob >= 1, HQQ_E_UNSUPPORTED, "hqq_b200_decode_linear_fwd_desc: needs the M == 1 kernel");
@@ -1061,6 +1133,34 @@ int linear_small_multi(const void* x, int nprob, const void* const* Wq, const vo
   a.total_tiles = yop ? (int)cdiv(a.p[0].step, P / 2) : tiles;
   if (dtype == HQQ_F16) return sk_bits<__half>(a, gs, nbits, st);
   return sk_bits<__nv_bfloat16>(a, gs, nbits, st);
+}
+
+// Grouped mode (see linear_small_kernel): the caller has checked the arguments and the format (small_route_ok)
+int linear_small_grouped(const void* x, const int* x_rows, int nprob, const void* const* Wq, const void* const* scale, const void* const* zero,
+                         void* const* y, const int64_t* N, int64_t K, int n_experts, const int* expert_off, const int* expert_cnt,
+                         int64_t max_pairs, int gs, int nbits, int dtype, cudaStream_t st) {
+  const int F = 8 / nbits, P = 16 / F;
+  SKArgs a;
+  memset(&a, 0, sizeof(a));
+  a.nprob = nprob; a.x = x; a.K = (int)K; a.Gk = (int)(K / gs); a.KB = (int)(K / 256);
+  a.M = (int)(max_pairs < 32 ? max_pairs : 32);  // picks the row tile: 8, 16 or 32 pairs per chunk
+  a.tp = 1; a.x_per_step = 1;
+  a.g_off = expert_off; a.g_cnt = expert_cnt; a.g_rows = x_rows; a.g_E = n_experts;
+  int tiles = 0;
+  for (int i = 0; i < kMaxProb; ++i) {
+    const int j = i < nprob ? i : 0;
+    a.p[i].Wq = (const uint8_t*)Wq[j]; a.p[i].scale = scale[j]; a.p[i].zero = zero[j]; a.p[i].bias = nullptr;
+    a.p[i].y = y[j]; a.p[i].ytag = nullptr; a.p[i].N = (int)N[j]; a.p[i].step = (int)(N[j] / F); a.p[i].tile0 = tiles;
+    if (i < nprob) tiles += (int)cdiv(a.p[i].step, P);
+  }
+  a.g_tiles = tiles;
+  // at most ceil(pairs / R) chunks plus one partial chunk per expert that has pairs
+  const int R = a.M <= 8 ? 8 : a.M <= 16 ? 16 : 32;
+  const int64_t chunks = cdiv(max_pairs, R) + (max_pairs < n_experts ? max_pairs : n_experts);
+  const int64_t bound = chunks * tiles;
+  a.total_tiles = (int)(bound < (int64_t(1) << 30) ? bound : (int64_t(1) << 30));
+  if (dtype == HQQ_F16) return sk_bits<__half, true>(a, gs, nbits, st);
+  return sk_bits<__nv_bfloat16, true>(a, gs, nbits, st);
 }
 
 }  // namespace hqq

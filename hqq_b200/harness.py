@@ -37,6 +37,17 @@ class LlamaShape:
     rms_eps: float = 1e-5
     # None: plain RoPE frequencies.  {"rope_type": "llama3", ...}: the Llama-3.1 frequency scaling (transformers' "llama3" rope type)
     rope_scaling: dict | None = None
+    # n_experts > 0: every block's MLP is a Mixtral-style sparse mixture of n_experts SwiGLU experts of width `inter`, each token
+    # routed to experts_per_token of them (transformers' MixtralSparseMoeBlock).  0: the dense MLP.
+    n_experts: int = 0
+    experts_per_token: int = 2
+
+    def __post_init__(self):
+        if self.n_experts:
+            if not (isinstance(self.n_experts, int) and 2 <= self.n_experts <= 64):
+                raise ValueError(f"n_experts must be 0 (dense) or an int in [2, 64] (got {self.n_experts!r})")
+            if not (isinstance(self.experts_per_token, int) and 1 <= self.experts_per_token <= min(8, self.n_experts)):
+                raise ValueError(f"experts_per_token must be an int in [1, min(8, n_experts)] (got {self.experts_per_token!r})")
 
     @property
     def head_dim(self) -> int:
@@ -49,6 +60,8 @@ TINY = LlamaShape(hidden=512, inter=1024, n_layers=2, n_heads=8, n_kv_heads=2, v
 # Llama-3.1 / 3.3 (128k context): the Llama-3 shapes with the llama3 RoPE scaling
 LLAMA31_8B = LlamaShape(rope_scaling={"rope_type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0,
                                       "original_max_position_embeddings": 8192})
+MIXTRAL_8X7B = LlamaShape(hidden=4096, inter=14336, n_layers=32, n_heads=32, n_kv_heads=8, vocab=32000, rope_theta=1e6, rms_eps=1e-5,
+                          n_experts=8, experts_per_token=2)
 
 # Above this many cache positions the fused steps run the split-KV attention kernel (csrc/decode_glue.cu): the one-CTA-per-head
 # kernel keeps a score per position in shared memory and stops here.  At or below it they run that kernel as before.
@@ -440,6 +453,8 @@ class DecodeModel:
                  top_p: float = 1.0, sample_seed: int = 0, ragged: bool = False, kv_pages: int | None = None, spec_k: int | None = None,
                  sample_keys: str = "step", slot_sampling: bool = False):
         self.shape, self.dtype, self.device = shape, dtype, torch.device(device)
+        if shape.n_experts and tp > 1:
+            raise ValueError(f"a mixture-of-experts shape runs on one GPU: tp must be 1 (got {tp})")
         # do_sample: every token (decode steps, batch rows, the token prefill returns) is drawn by hqq_b200_glue_sample -- temperature,
         # top-k, top-p, then a Gumbel race on Philox numbers keyed by sample_seed and countered by _sample_ctr -- instead of the argmax.
         # The defaults are those of the reference's HFGenerator; like there, the parameters are fixed for the model's life.
@@ -521,8 +536,10 @@ class DecodeModel:
                 raise ValueError("spec_k verifies greedy targets: it cannot be combined with do_sample")
             if not (isinstance(spec_k, int) and 1 <= spec_k <= 7):
                 raise ValueError(f"spec_k must be an int in [1, 7] (got {spec_k!r})")
-        if (self.batch > 1 or self.ragged) and fused:
-            fused = True  # the 8-launch path with the batched glue kernels; the one-token kernels (fused=5) and their exchange are M = 1 only
+        if (self.batch > 1 or self.ragged or shape.n_experts) and fused:
+            # the 8-launch path with the batched glue kernels; the one-token kernels (fused=5) and their exchange are M = 1 only, and
+            # their prologue / epilogue fusions are those of the dense MLP
+            fused = True
         self.fused = fused
         import os
         # "p2p": the row-parallel partials meet through tagged words over NVLink peer memory inside the kernels (default);
@@ -562,9 +579,12 @@ class DecodeModel:
         # (same levels, scales, zeros), which per-shard quantisation of per-rank random weights (the default, cheaper) does not
         full_dims = shard_dims(shape, 1)
         par = {"q": "column", "k": "column", "v": "column", "gate": "column", "up": "column", "o": "row", "down": "row"}
+        mlp = ("gate", "up", "down")
         for _ in range(self.n_layers):
             blk = {}
             for name, (n, k) in dims.items():
+                if shape.n_experts and name in mlp:
+                    continue
                 if shard_from_full and tp > 1:
                     from .models.tp import shard_hqq_linear
                     fn, fk = full_dims[name]
@@ -575,6 +595,8 @@ class DecodeModel:
                     blk[name] = HQQLinear.from_weights(rnd(n, k, gshared if shard_from_full else g), None, cfg, compute_dtype=dtype,
                                                        device=str(self.device))
                 self.quantized_weights += n * k
+            if shape.n_experts:
+                self._make_experts(blk, dims, cfg, lambda n, k: rnd(n, k, g))
             blk["norm1"] = torch.ones(shape.hidden, device=self.device, dtype=dtype)
             blk["norm2"] = torch.ones(shape.hidden, device=self.device, dtype=dtype)
             hkv = shape.n_kv_heads // tp
@@ -618,6 +640,33 @@ class DecodeModel:
             self.spec_logits = None  # [batch, K + 1, vocab / tp]: the last verify step's logits
         self.graph = None
         self.last_logits = None  # set by prefill(): logits of the last prompt position of each sequence
+        if shape.n_experts:  # the router's ticket counter (include/hqq_b200.h): zero, and every router launch leaves it zero
+            self._moe_ticket = torch.zeros(1, dtype=torch.int32, device=self.device)
+
+    def _make_experts(self, blk, dims, cfg, rnd):
+        """A mixture-of-experts block: the router [E, hidden] in the compute dtype (not quantised, as the reference keeps
+        block_sparse_moe.gate), and every expert's gate / up / down quantised by HQQLinear.from_weights like the dense matrices.  Each
+        kind's W_q / scale / zero live in ONE stacked tensor [E, ...] in the per-expert layout HQQLinear stores (what
+        hqq_b200_linear_fwd_grouped reads); blk["experts"][e] holds HQQLinear objects over views of the stacks (the fused=False path)."""
+        E = self.shape.n_experts
+        blk["router"] = rnd(E, self.shape.hidden)
+        blk["experts"] = [{} for _ in range(E)]
+        blk["stack"] = {}
+        for name in ("gate", "up", "down"):
+            n, k = dims[name]
+            stack = None
+            for e in range(E):
+                lin = HQQLinear.from_weights(rnd(n, k), None, cfg, compute_dtype=self.dtype, device=str(self.device))
+                parts = (lin.W_q.data, lin.meta["scale"], lin.meta["zero"])
+                if stack is None:
+                    stack = tuple(torch.empty((E, *t.shape), dtype=t.dtype, device=t.device) for t in parts)
+                for dst, src in zip(stack, parts):
+                    dst[e].copy_(src)
+                lin.W_q = torch.nn.Parameter(stack[0][e], requires_grad=False)
+                lin.meta["scale"], lin.meta["zero"] = stack[1][e], stack[2][e]
+                blk["experts"][e][name] = lin
+                self.quantized_weights += n * k
+            blk["stack"][name] = stack
 
     @property
     def attn_kernel(self) -> str:
@@ -777,6 +826,60 @@ class DecodeModel:
         x1, x2 = x[..., : hd // 2], x[..., hd // 2:]
         return x * cos + torch.cat((-x2, x1), dim=-1) * sin
 
+    def _mlp_ref(self, blk, x):
+        """The MLP of the framework-op path on x [M, hidden]: gate/up, SiLU*mul, down; or, with experts, transformers'
+        MixtralSparseMoeBlock restated so that it stays capturable (no host reads): the router in the model dtype, softmax in fp32,
+        top-k, the k weights renormalised; EVERY expert runs on every row, the unselected ones weighted by 0, and the terms
+        T(y_e * w_e) accumulate in the model dtype in ascending expert order (MixtralExperts' .to(dtype) and index_add_: the zero
+        terms leave that sum exact)."""
+        s = self.shape
+        if not s.n_experts:
+            g, u = self._multi(x, (blk["gate"], blk["up"]))
+            return blk["down"](F.silu(g) * u)
+        p = torch.softmax(F.linear(x, blk["router"]).float(), dim=-1)
+        top, idx = torch.topk(p, s.experts_per_token, dim=-1)
+        w = torch.zeros_like(p).scatter_(1, idx, top / top.sum(dim=-1, keepdim=True))
+        out = torch.zeros_like(x)
+        for e, ex in enumerate(blk["experts"]):
+            g, u = self._multi(x, (ex["gate"], ex["up"]))
+            y = ex["down"](F.silu(g) * u)
+            out = (out.float() + (y.float() * w[:, e:e + 1]).to(x.dtype).float()).to(x.dtype)
+        return out
+
+    def _mlp_bufs(self, M, alloc):
+        """Scratch of _mlp_fused for M rows, from alloc(rows, width) (the model dtype) and torch.empty for the router's tables."""
+        s = self.shape
+        inter = s.inter // self.tp
+        if not s.n_experts:
+            return {"gate": alloc(M, inter), "up": alloc(M, inter), "act": alloc(M, inter), "down": alloc(M, s.hidden)}
+        E, k = s.n_experts, s.experts_per_token
+        i32 = lambda *sh: torch.zeros(*sh, dtype=torch.int32, device=self.device)
+        return {"gate": alloc(M * k, inter), "up": alloc(M * k, inter), "act": alloc(M * k, inter), "pairs": alloc(M * k, s.hidden),
+                "down": alloc(M, s.hidden), "ids": i32(M, k), "pair_of": i32(M, k), "off": i32(E), "cnt": i32(E), "token": i32(M * k),
+                "w": torch.zeros(M, k, dtype=torch.float32, device=self.device)}
+
+    def _mlp_fused(self, lib, blk, x, b, M, code, st):
+        """The MLP on the package's kernels for x [M, hidden] into b["down"] (scratch b from _mlp_bufs): fused gate/up, SiLU*mul,
+        down; or, with experts, the router (hqq_b200_glue_moe_route), the expert-grouped gate/up over the rows gathered by token, SiLU*mul
+        over the M k pair rows, the grouped down in pair order and the combine (hqq_b200_glue_moe_combine)."""
+        from ._lib import check, ptr
+        s = self.shape
+        inter = s.inter // self.tp
+        if not s.n_experts:
+            self._lin(x, (blk["gate"], blk["up"]), [b["gate"], b["up"]])
+            check(lib.hqq_b200_glue_silu_mul(ptr(b["gate"]), ptr(b["up"]), ptr(b["act"]), M * inter, code, st))
+            self._lin(b["act"], (blk["down"],), [b["down"]])
+            return b["down"]
+        E, k = s.n_experts, s.experts_per_token
+        check(lib.hqq_b200_glue_moe_route(ptr(x), ptr(blk["router"]), M, s.hidden, E, k, ptr(b["ids"]), ptr(b["w"]), ptr(b["pair_of"]), ptr(b["off"]),
+                                          ptr(b["cnt"]), ptr(b["token"]), ptr(self._moe_ticket), code, st))
+        st_ = blk["stack"]
+        ops.linear_fwd_grouped(x, b["token"], (st_["gate"], st_["up"]), [b["gate"], b["up"]], b["off"], b["cnt"], M * k, self.group_size, self.nbits)
+        check(lib.hqq_b200_glue_silu_mul(ptr(b["gate"]), ptr(b["up"]), ptr(b["act"]), M * k * inter, code, st))
+        ops.linear_fwd_grouped(b["act"], None, (st_["down"],), [b["pairs"]], b["off"], b["cnt"], M * k, self.group_size, self.nbits)
+        check(lib.hqq_b200_glue_moe_combine(ptr(b["pairs"]), ptr(b["ids"]), ptr(b["w"]), ptr(b["pair_of"]), ptr(b["down"]), M, s.hidden, k, code, st))
+        return b["down"]
+
     def step(self):
         """One token per sequence: reads self.tok [batch] / self.pos, writes self.next_tok and advances self.pos (all on device)."""
         s = self.shape
@@ -825,8 +928,7 @@ class DecodeModel:
                 torch.distributed.all_reduce(o, group=self.pg)
             h = h + o
             x = F.rms_norm(h, (s.hidden,), blk["norm2"], s.rms_eps)
-            gate, up = self._multi(x, (blk["gate"], blk["up"]))
-            y = blk["down"](F.silu(gate) * up)
+            y = self._mlp_ref(blk, x)
             if self.tp > 1:
                 torch.distributed.all_reduce(y, group=self.pg)
             h = h + y
@@ -1000,13 +1102,14 @@ class DecodeModel:
     def step_fused(self):
         """Same token step with the package's glue kernels (8 launches per block): add+RMSNorm, fused q/k/v, RoPE+cache+
         attention, o, add+RMSNorm, fused gate/up, SiLU*mul, down.  With tensor parallelism every rank runs the same launches
-        on its shard (heads / inter split tp ways) and the two row-parallel outputs are summed with one all-reduce each."""
+        on its shard (heads / inter split tp ways) and the two row-parallel outputs are summed with one all-reduce each.  A
+        mixture-of-experts block is 10 launches: its MLP is route, grouped gate/up, SiLU*mul, grouped down, combine (_mlp_fused).
+        A mixture-of-experts model always takes this path (fused=5 included): the one-token kernels' fusions are the dense MLP's."""
         from ._lib import DTYPE_CODE, check, load, ptr, stream_ptr
         lib, s = load(), self.shape
         st = stream_ptr(self.device)
         code = DTYPE_CODE[self.dtype]
         hd, hq, hkv = s.head_dim, s.n_heads // self.tp, s.n_kv_heads // self.tp
-        inter = s.inter // self.tp
         b = self._bufs
         B = self.batch
         self._hist_write()
@@ -1031,12 +1134,9 @@ class DecodeModel:
             if self.tp > 1:
                 torch.distributed.all_reduce(b["o"], group=self.pg)
             norm(b["o"], blk["norm2"])
-            self._lin(b["x"], (blk["gate"], blk["up"]), [b["gate"], b["up"]])
-            check(lib.hqq_b200_glue_silu_mul(ptr(b["gate"]), ptr(b["up"]), ptr(b["act"]), B * inter, code, st))
-            self._lin(b["act"], (blk["down"],), [b["down"]])
+            delta = self._mlp_fused(lib, blk, b["x"], self._moe_bufs if s.n_experts else b, B, code, st)
             if self.tp > 1:
-                torch.distributed.all_reduce(b["down"], group=self.pg)
-            delta = b["down"]
+                torch.distributed.all_reduce(delta, group=self.pg)
         norm(delta, self.final_norm)
         self._head(lib, b["x"], code, st)
         self.pos.add_(1).remainder_(self.cache_len)
@@ -1374,8 +1474,7 @@ class DecodeModel:
         e = lambda w: torch.empty(M, w, device=self.device, dtype=self.dtype)
         h = self.embed.index_select(0, ids.reshape(-1))  # [M, hidden], row b * n + t
         x, q, k, v, qr, a, o = e(s.hidden), e(hq * hd), e(hkv * hd), e(hkv * hd), e(hq * hd), e(hq * hd), e(s.hidden)
-        inter = s.inter // self.tp
-        gate, up, act, down = e(inter), e(inter), e(inter), e(s.hidden)
+        mb = self._mlp_bufs(M, lambda r, w: torch.empty(r, w, device=self.device, dtype=self.dtype))
         norm = lambda d, w: check(lib.hqq_b200_glue_add_rmsnorm_rows(ptr(h), ptr(d), ptr(w), ptr(x), M, s.hidden, s.rms_eps, code, st))
         delta = None
         kv8 = self._kvq  # 8 or 4 bits: the staging pair, as below
@@ -1422,9 +1521,7 @@ class DecodeModel:
             if self.tp > 1:
                 torch.distributed.all_reduce(o, group=self.pg)
             norm(o, blk["norm2"])
-            self._lin(x, (blk["gate"], blk["up"]), [gate, up])
-            check(lib.hqq_b200_glue_silu_mul(ptr(gate), ptr(up), ptr(act), M * inter, code, st))
-            self._lin(act, (blk["down"],), [down])
+            down = self._mlp_fused(lib, blk, x, mb, M, code, st)
             if self.tp > 1:
                 torch.distributed.all_reduce(down, group=self.pg)
             delta = down
@@ -1472,8 +1569,7 @@ class DecodeModel:
                 torch.distributed.all_reduce(o, group=self.pg)
             h = h + o
             x = F.rms_norm(h, (s.hidden,), blk["norm2"], s.rms_eps)
-            g, u = self._multi(x, (blk["gate"], blk["up"]))
-            delta = blk["down"](F.silu(g) * u)
+            delta = self._mlp_ref(blk, x)
             if self.tp > 1:
                 torch.distributed.all_reduce(delta, group=self.pg)
         return h, delta
@@ -1552,6 +1648,8 @@ class DecodeModel:
                       "v": z(s.n_kv_heads // tp * s.head_dim), "a": z(s.n_heads // tp * s.head_dim), "o": z(s.hidden),
                       "gate": z(s.inter // tp), "up": z(s.inter // tp), "act": z(s.inter // tp), "down": z(s.hidden), "logits": z(self.vocab_shard),
                       "key": torch.zeros(1, dtype=torch.long, device=dev)}
+        if s.n_experts:  # step_fused's MoE scratch (the dense MLP works in the buffers above)
+            self._moe_bufs = self._mlp_bufs(self.batch, lambda r, w: torch.zeros(r, w, device=dev, dtype=dt))
         if self.do_sample or self.slot_sampling:
             self._bufs.update(self._sample_buffers(self.batch))
             if self.position_keys and self.pos.numel() != self.batch:
@@ -1718,8 +1816,7 @@ class DecodeModel:
                 torch.distributed.all_reduce(o, group=self.pg)
             h = h + o
             x = F.rms_norm(h, (s.hidden,), blk["norm2"], s.rms_eps)
-            g, u = self._multi(x, (blk["gate"], blk["up"]))
-            y = blk["down"](F.silu(g) * u)
+            y = self._mlp_ref(blk, x)
             if self.tp > 1:
                 torch.distributed.all_reduce(y, group=self.pg)
             h = h + y

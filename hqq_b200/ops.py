@@ -290,6 +290,26 @@ def linear_fwd_multi(x2d: torch.Tensor, layers, outs=None):
     return outs
 
 
+def linear_fwd_grouped(x2d: torch.Tensor, x_rows, stacks, outs, expert_off: torch.Tensor, expert_cnt: torch.Tensor, max_pairs: int,
+                       group_size: int, nbits: int) -> None:
+    """Expert-grouped forward (`hqq_b200_linear_fwd_grouped`): `stacks` are (W_q, scale, zero) tensors [E, ...] holding E experts in
+    the per-expert HQQLinear layout, `outs` their outputs [pairs, N] (up to 4 matrices sharing x2d [rows, K]); pair p of expert e,
+    p in [expert_off[e], expert_off[e] + expert_cnt[e]) (int32 device tables, e.g. from the router), reads x2d row x_rows[p]
+    (x_rows None: row p) and writes row p of each output.  Raises on a configuration outside the kernel: there is no fallback."""
+    import ctypes
+    lib = load()
+    n = len(stacks)
+    E = int(stacks[0][0].shape[0])
+    K = int(x2d.shape[1])
+    VP = ctypes.c_void_p * n
+    arr = lambda ts: VP(*[ptr(t) for t in ts])
+    Narr = (ctypes.c_int64 * n)(*[int(y.shape[1]) for y in outs])
+    with _on(x2d.device):
+        check(lib.hqq_b200_linear_fwd_grouped(ptr(x2d), ptr(x_rows), n, arr([t[0] for t in stacks]), arr([t[1] for t in stacks]),
+                                              arr([t[2] for t in stacks]), arr(outs), Narr, K, E, ptr(expert_off), ptr(expert_cnt), int(max_pairs),
+                                              int(group_size), int(nbits), DTYPE_CODE[x2d.dtype], stream_ptr(x2d.device)))
+
+
 YOP_SILU_MUL_PAIR = 16  # HQQ_YOP_SILU_MUL_PAIR (include/hqq_b200.h): or-ed into x_op
 
 
@@ -342,4 +362,4 @@ def _decode_launch(lib, x, layers, outs, x_op, x2, x_weight, h_out, eps, tpx, n,
     return rc
 
 
-__all__ = ["pack", "unpack", "dequantize", "quantize", "linear_fwd", "linear_fwd_multi", "linear_route", "packed_shape", "HQQB200Error"]
+__all__ = ["pack", "unpack", "dequantize", "quantize", "linear_fwd", "linear_fwd_multi", "linear_fwd_grouped", "linear_route", "packed_shape", "HQQB200Error"]

@@ -179,6 +179,24 @@ int hqq_b200_linear_fwd_multi(const void* x, int count, const void* const* W_q, 
                               int64_t M, int64_t K, int group_size, int nbits, int axis, int dtype,
                               void* workspace, size_t workspace_bytes, void* stream);
 
+/* Expert-grouped forward (mixture-of-experts MLP): the small-M kernel over stacks of n_experts matrices, the experts and their rows
+ * chosen on the device by hqq_b200_glue_moe_route, so a captured CUDA graph can run it.
+ *   W_q[i] / scale[i] / zero[i]: n_experts experts back to back, each in exactly the layout hqq_b200_linear_fwd takes for an
+ *   [N[i], K] matrix (axis 1); y[i] [pairs, N[i]].  Pair p of expert e -- p in [expert_off[e], expert_off[e] + expert_cnt[e]),
+ *   device int32 tables -- reads x row x_rows[p] (x_rows NULL: row p) and writes row p of every y[i]:
+ *     y[i][p] = x[x_rows[p]] @ dequantize(W_q[i] of expert e)^T           (quantize.py:880-898, no bias)
+ *   Up to 4 matrices share x in one launch (gate/up).  max_pairs bounds the sum of expert_cnt: it sizes the grid and the row tile
+ *   (8, 16 or 32 pairs per chunk of an expert); only chunks that exist are walked, so experts without pairs cost no weight bytes.
+ *   A pair's bits depend on its x row, its expert and max_pairs alone.  The tables are read after the programmatic-dependency
+ *   wait: unlike hqq_b200_linear_fwd_multi, no weight is prefetched under the previous kernel's tail.  Rows of y no pair owns
+ *   are not written.  The formats of the small-M kernel (nbits 8/4/2/1, group_size 64/128, K % 256 == 0, f16, bf16 below 8
+ *   bits), else HQQ_E_UNSUPPORTED; HQQ_E_INVALID for null or unaligned pointers (x, W_q 16 bytes; scale, zero 8), n_experts
+ *   outside [1, 64] or max_pairs outside [1, 524280].                                                                           */
+int hqq_b200_linear_fwd_grouped(const void* x, const int32_t* x_rows, int count, const void* const* W_q, const void* const* scale,
+                                const void* const* zero, void* const* y, const int64_t* N, int64_t K, int n_experts,
+                                const int32_t* expert_off, const int32_t* expert_cnt, int64_t max_pairs, int group_size, int nbits,
+                                int dtype, void* stream);
+
 /* Which kernels hqq_b200_linear_fwd would use: 0 none (unsupported), 1 small-M mma.sync weight-streaming kernel,
  * 2 fused wgmma/TMA GEMM, 3 dequantize kernel + dense wgmma GEMM.                                         */
 int hqq_b200_linear_fwd_route(int64_t M, int64_t N, int64_t K, int group_size, int nbits,
@@ -237,6 +255,21 @@ int hqq_b200_glue_add_rmsnorm_rows(void* h, const void* delta, const void* weigh
                                    int rows, int H, float eps, int dtype, void* stream);
 /* y = silu(gate) * up */
 int hqq_b200_glue_silu_mul(const void* gate, const void* up, void* y, int n, int dtype, void* stream);
+/* Mixture-of-experts router (transformers' MixtralTopKRouter), one launch for M token rows of x [M, H] and router [n_experts, H]:
+ *   l = T(x[m] @ router^T) (fp32 sums, one rounding to `dtype`); p = softmax(l) in fp32; the k largest p in descending order,
+ *   ties to the lower expert index; w_j = p_j / sum p_j in fp32.  ids int32 / weights fp32 [M, k] hold them in that order.
+ * It also groups the M k (token, slot) pairs by expert, expert-major, ascending token order within an expert:
+ *   expert_off / expert_cnt int32 [n_experts]: the slots of expert e are [off[e], off[e] + cnt[e]); pair_token int32 [M k]: the
+ *   token row of each slot; pair_of int32 [M, k]: the slot of (m, j).  Deterministic; no host reads (capturable).
+ * ticket: one 4-byte word, zero before the first launch; every launch leaves it zero.  HQQ_E_INVALID for null pointers,
+ * n_experts outside [2, 64], k outside [1, min(8, n_experts)], M outside [1, 65535], H % 8 != 0 or x / router not 16-byte aligned. */
+int hqq_b200_glue_moe_route(const void* x, const void* router, int M, int H, int n_experts, int k, int32_t* ids, float* weights,
+                            int32_t* pair_of, int32_t* expert_off, int32_t* expert_cnt, int32_t* pair_token, void* ticket, int dtype,
+                            void* stream);
+/* delta[m] = sum over token m's k pairs, in ascending expert id, of T(y[pair_of[m][j]] * weights[m][j]), accumulated in `dtype` from 0
+ * (transformers' MixtralExperts: the fp32 product rounded by .to(dtype), index_add_ one expert at a time).  y [M k, H] in slot order. */
+int hqq_b200_glue_moe_combine(const void* y, const int32_t* ids, const float* weights, const int32_t* pair_of, void* delta, int M, int H,
+                              int k, int dtype, void* stream);
 /* RoPE(q,k at *pos) + KV-cache append + one-token GQA attention over cache[0..*pos];
  * caches [n_kv_heads, cache_len, head_dim], cos/sin tables [cache_len, head_dim], pos on device.
  * *pos and cache rows [0, *pos) are read BEFORE the programmatic-dependency wait (L2 prefetch under the previous kernel's
